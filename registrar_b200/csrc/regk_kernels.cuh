@@ -45,11 +45,19 @@ namespace regk {
 #ifndef REGK_TILE
 #define REGK_TILE 128
 #endif
+/*
+ * Minimum resident CTAs per SM for the compose kernels' __launch_bounds__, which sets their register cap
+ * (65536 / (TILE * MINB), rounded down to a multiple of 8).  Shared memory, not registers, decides how many CTAs
+ * fit: a path tile of config 3 or 5 needs about 26 KB, so at most 8 fit in the SM's 228 KB.  The payload kernel's
+ * image and fragment table take about 19 KB, so at most 11 fit.  A cap of 12 (40 registers) made both kernels
+ * spill and bought no occupancy on those workloads.  8 gives the path kernel 64 registers and 10 gives the payload
+ * kernel 48, and neither spills.  On an H100 SXM, that cut the config 3 step by 2.5 % (DESIGN.md §4).
+ */
 #ifndef REGK_MINB_PATH
-#define REGK_MINB_PATH 12
+#define REGK_MINB_PATH 8
 #endif
 #ifndef REGK_MINB_JSON
-#define REGK_MINB_JSON 12
+#define REGK_MINB_JSON 10
 #endif
 constexpr int TILE = REGK_TILE;                 /* records per tile == threads per CTA */
 constexpr int WARPS = TILE / 32;
