@@ -41,7 +41,8 @@ extern "C" {
 #define REGK_OK                 0
 #define REGK_ERR_INVALID_ARG    1   /* NULL pointer, bad flag combination, misaligned device pointer */
 #define REGK_ERR_CUDA           2   /* CUDA runtime error; text in regk_last_error() */
-#define REGK_ERR_OUT_OF_DOMAIN  3   /* >=1 record outside the fenced input domain; nothing is returned */
+#define REGK_ERR_OUT_OF_DOMAIN  3   /* >=1 record outside the fenced input domain; nothing is returned (unless the
+                                       batch has REGK_SKIP_BAD: then only REGK_BAD_TOO_LARGE refuses it) */
 #define REGK_ERR_NOMEM          4
 #define REGK_ERR_STATE          5   /* e.g. type table not set, result already released */
 
@@ -55,6 +56,13 @@ extern "C" {
 #define REGK_JOB_STEP    (1u << 5)  /* this batch is the calling rank's shard of the multi-GPU job bound with
                                        regk_job_bind(): results go straight into every rank's whole-job buffers
                                        (requires REGK_IN_DEVICE | REGK_OUT_DEVICE, paths and payloads) */
+#define REGK_SKIP_BAD    (1u << 6)  /* skip mode: a record whose only faults are value-fence bits (REGK_BAD_DOMAIN_BYTE,
+                                       _HOST_BYTE, _ADDR_BYTE, _TYPE_ID) gets an empty path and payload (off[i] ==
+                                       off[i+1]), every other record is composed exactly as in a batch of the kept records
+                                       alone, and the call returns REGK_OK; bad_bits / first_bad then describe the skipped
+                                       records and regk_skipped_records() lists them.  REGK_BAD_TOO_LARGE still refuses
+                                       the whole batch.  Not with REGK_JOB_STEP.  A clean batch runs exactly the kernels
+                                       of a plain one; a dirty one is composed a second time (DESIGN.md section 4) */
 
 /* ---- per-record validation bits (regk_result.bad_bits) ------------------ */
 #define REGK_BAD_DOMAIN_BYTE  (1u << 0)  /* byte >= 0x80 or '/' in a domain (JS toLowerCase / path.normalize
@@ -201,6 +209,25 @@ typedef struct regk_service_batch {
 } regk_service_batch;
 
 int         regk_service_records(regk_ctx *ctx, const regk_service_batch *batch, regk_result *result);
+
+/*
+ * ---- the records a REGK_SKIP_BAD batch skipped ----------------------------------------------------------------
+ * Describes the batch finished last on this context, which must have been a skip-mode batch (else REGK_ERR_STATE).
+ * The list is compact: a few bad records in 10^7 cost a few bytes, not an n-byte mask.  Downstream calls on "the
+ * batch finished last" (regk_parent_dirs, regk_jute_frames / regk_jute_requests, regk_decode with REGK_DECODE_LAST)
+ * see the KEPT records in order: their record k is the k-th kept record.  flags: REGK_OUT_DEVICE returns device
+ * pointers, otherwise pinned host arrays; both stay valid until the next batch on the context.
+ */
+typedef struct regk_skipped {
+    uint64_t n;                     /* records of the batch */
+    uint64_t n_skipped;
+    uint32_t flags;                 /* REGK_OUT_DEVICE: device pointers, else pinned host arrays */
+    uint32_t bad_bits;              /* OR over the skipped records */
+    const uint64_t *index;          /* [n_skipped] ascending record indices */
+    const uint8_t  *bits;           /* [n_skipped] REGK_BAD_* of each */
+} regk_skipped;
+
+int         regk_skipped_records(regk_ctx *ctx, uint32_t flags, regk_skipped *out);
 
 /* Pinned host memory for callers that want zero-staging H2D/D2H. */
 void       *regk_host_alloc(regk_ctx *ctx, size_t bytes);

@@ -14,7 +14,7 @@ from typing import Optional
 import numpy as np
 
 from .batch import (FLAG_IN_DEVICE, FLAG_JOB_STEP, FLAG_NODE_ALIAS, FLAG_NO_JSON, FLAG_NO_PATH, FLAG_OUT_DEVICE,
-                    RecordBatch)
+                    FLAG_SKIP_BAD, RecordBatch)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("REGK_LIB") or os.path.join(_HERE, "libregk.so")      # REGK_LIB: A/B builds (dev)
@@ -133,12 +133,17 @@ class CParents(C.Structure):         # regk_parents
                 ("parent_len", C.c_void_p), ("unique_first", C.c_void_p), ("kernel_ms", C.c_float)]
 
 
+class CSkipped(C.Structure):         # regk_skipped
+    _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
+                ("index", C.c_void_p), ("bits", C.c_void_p)]
+
+
 EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error", "regk_set_stream",
            "regk_set_types", "regk_register_batch", "regk_finish", "regk_release", "regk_host_alloc",
            "regk_host_free", "regk_dev_alloc", "regk_dev_free", "regk_memcpy_h2d", "regk_memcpy_d2h",
            "regk_sync", "regk_set_option", "regk_get_option", "regk_ipc_export", "regk_ipc_open", "regk_ipc_close",
            "regk_gather_push", "regk_parent_dirs", "regk_job_bind", "regk_service_records",
-           "regk_jute_frames", "regk_jute_requests", "regk_decode"]
+           "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records"]
 
 _lib = None
 
@@ -189,6 +194,7 @@ def load_library():
     lib.regk_jute_frames.argtypes = [vp, u32, C.c_int32, u32, C.POINTER(CFrames)]
     lib.regk_jute_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     lib.regk_decode.argtypes = [vp, C.POINTER(CDecodeIn), C.POINTER(CDecodeOut)]
+    lib.regk_skipped_records.argtypes = [vp, u32, C.POINTER(CSkipped)]
     _lib = lib
     return lib
 
@@ -218,11 +224,14 @@ def host_cbatch(b: RecordBatch, flags: int = 0):
 
 class HostResult:
     """Host copy of a regk_result (NumPy views are copied out of the library's pinned buffers
-    unless copy=False)."""
+    unless copy=False).  A skip-mode result also carries `skipped` (uint64, ascending record indices) and
+    `skipped_bits` (uint8, REGK_BAD_* of each); those records have empty paths and payloads."""
 
     def __init__(self, n, path_bytes, path_off, json_bytes, json_off, kernel_ms, path_ms, json_ms, launches,
                  json_len_ms=0.0, generic_tiles=0):
         self.generic_tiles = generic_tiles
+        self.skipped = None
+        self.skipped_bits = None
         self.n = n
         self.path_bytes, self.path_off = path_bytes, path_off
         self.json_bytes, self.json_off = json_bytes, json_off
@@ -325,10 +334,12 @@ class Context:
 
     # -- the hot path, host buffers in / host buffers out --
     def register_batch(self, batch: RecordBatch, paths: bool = True, payloads: bool = True,
-                       copy: bool = True) -> HostResult:
-        """Host RecordBatch -> HostResult through regk_register_batch (H2D, kernels, D2H)."""
+                       copy: bool = True, skip_bad: bool = False) -> HostResult:
+        """Host RecordBatch -> HostResult through regk_register_batch (H2D, kernels, D2H).  skip_bad=True: records
+        outside the fenced input domain come back empty and are listed in result.skipped instead of refusing the
+        batch (REGK_SKIP_BAD)."""
         self.set_types(batch.types)
-        flags = (0 if paths else FLAG_NO_PATH) | (0 if payloads else FLAG_NO_JSON)
+        flags = (0 if paths else FLAG_NO_PATH) | (0 if payloads else FLAG_NO_JSON) | (FLAG_SKIP_BAD if skip_bad else 0)
         cb, keep = host_cbatch(batch, flags)
         res = CResult()
         rc = self._lib.regk_register_batch(self._h, C.byref(cb), C.byref(res))
@@ -342,8 +353,20 @@ class Context:
             cp(_as_np(res.json_bytes, int(res.json_total), np.uint8)), cp(_offsets(res, "json_off", n)),
             float(res.kernel_ms), float(res.path_kernel_ms), float(res.json_kernel_ms), int(res.launches),
             float(res.json_len_kernel_ms), int(res.generic_tiles))
+        if skip_bad:
+            out.skipped, out.skipped_bits = self.skipped_records()
         self._lib.regk_release(self._h, C.byref(res))
         return out
+
+    def skipped_records(self, device: bool = False):
+        """(index uint64[n_skipped], bad_bits uint8[n_skipped]) of the skip-mode batch finished last on this
+        context (regk_skipped_records).  device=True returns the raw CSkipped (device pointers)."""
+        out = CSkipped()
+        self._check(self._lib.regk_skipped_records(self._h, FLAG_OUT_DEVICE if device else 0, C.byref(out)))
+        if device:
+            return out
+        k = int(out.n_skipped)
+        return _as_np(out.index, k, np.uint64).copy(), _as_np(out.bits, k, np.uint8).copy()
 
     # -- service records (lib/register.js:45-75), host buffers in / host buffers out --
     def service_records(self, sb) -> HostResult:
@@ -421,11 +444,11 @@ class Context:
                 _as_np(out.ports, int(out.ports_len), np.uint32).copy(), float(out.kernel_ms))
 
     # -- two-deep submission of host batches: the next batch's H2D overlaps this batch's result traffic --
-    def submit(self, batch: RecordBatch, paths: bool = True, payloads: bool = True):
+    def submit(self, batch: RecordBatch, paths: bool = True, payloads: bool = True, skip_bad: bool = False):
         """Enqueue a host RecordBatch and return a ticket for collect().  Needs set_option("async", 1); the
         batch's arrays must stay alive and unchanged until collect().  At most two tickets may be open."""
         self.set_types(batch.types)
-        flags = (0 if paths else FLAG_NO_PATH) | (0 if payloads else FLAG_NO_JSON)
+        flags = (0 if paths else FLAG_NO_PATH) | (0 if payloads else FLAG_NO_JSON) | (FLAG_SKIP_BAD if skip_bad else 0)
         cb, keep = host_cbatch(batch, flags)
         res = CResult()
         rc = self._lib.regk_register_batch(self._h, C.byref(cb), C.byref(res))
@@ -447,11 +470,17 @@ class Context:
             cp(_as_np(res.json_bytes, int(res.json_total), np.uint8)), cp(_offsets(res, "json_off", n)),
             float(res.kernel_ms), float(res.path_kernel_ms), float(res.json_kernel_ms), int(res.launches),
             float(res.json_len_kernel_ms), int(res.generic_tiles))
+        if ticket[1].flags & FLAG_SKIP_BAD:
+            out.skipped, out.skipped_bits = self.skipped_records()
         self._lib.regk_release(self._h, C.byref(res))
         return out
 
     # -- raw access for device-resident callers (bench.py, multi-GPU host layer) --
-    def register_raw(self, cbatch: CBatch, cres: Optional[CResult] = None) -> CResult:
+    def register_raw(self, cbatch: CBatch, cres: Optional[CResult] = None, skip_bad: bool = False) -> CResult:
+        """regk_register_batch on a caller-built CBatch.  skip_bad=True adds REGK_SKIP_BAD to its flags; the skipped
+        records are then read with skipped_records()."""
+        if skip_bad:
+            cbatch.flags |= FLAG_SKIP_BAD
         res = cres if cres is not None else CResult()
         rc = self._lib.regk_register_batch(self._h, C.byref(cbatch), C.byref(res))
         self._check(rc, res)

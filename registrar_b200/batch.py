@@ -24,6 +24,7 @@ FLAG_NODE_ALIAS = 1 << 2
 FLAG_NO_JSON = 1 << 3
 FLAG_NO_PATH = 1 << 4
 FLAG_JOB_STEP = 1 << 5
+FLAG_SKIP_BAD = 1 << 6           # skip out-of-domain records instead of refusing the batch (REGK_SKIP_BAD)
 
 BAD_DOMAIN_BYTE = 1 << 0
 BAD_HOST_BYTE = 1 << 1
@@ -172,6 +173,41 @@ class RecordBatch:
                            type_id=self.type_id[lo:hi].copy(), addr_bytes=ab, addr_off=ao,
                            ttl=self.ttl[lo:hi].copy(), ports_off=po, ports=pb,
                            ports_present=None if self.ports_present is None else self.ports_present[lo:hi].copy(),
+                           alias=self.alias, meta=dict(self.meta))
+
+    def take(self, indices) -> "RecordBatch":
+        """The records at `indices` (in that order) as an independent batch, e.g. the records a skip-mode call
+        skipped (HostResult.skipped), to be routed to another implementation."""
+        idx = np.asarray(indices, dtype=np.int64).reshape(-1)
+        if idx.size and (idx.min() < 0 or idx.max() >= self.n):
+            raise IndexError("record index out of range [0, %d)" % self.n)
+
+        def gather(data, off):
+            o = off.astype(np.int64)
+            lo = o[idx]
+            lens = o[idx + 1] - lo
+            noff = np.zeros(idx.size + 1, np.int64)
+            np.cumsum(lens, out=noff[1:])
+            pos = np.repeat(lo - noff[:-1], lens) + np.arange(int(noff[-1]), dtype=np.int64)
+            return data[pos].copy(), noff.astype(np.uint32)
+        db, do = gather(self.domain_bytes, self.domain_off)
+        ab, ao = gather(self.addr_bytes, self.addr_off)
+        if self.alias:
+            hb, ho = self.host_bytes, None
+        elif self.host_off is not None:
+            hb, ho = gather(self.host_bytes, self.host_off)
+        else:
+            s = self.host_stride
+            hb, ho = self.host_bytes[:self.n * s].reshape(self.n, s)[idx].reshape(-1).copy(), None
+        if self.ports_off is not None:
+            pb, po = gather(self.ports, self.ports_off)
+        else:
+            pb, po = None, None
+        return RecordBatch(n=int(idx.size), types=list(self.types), domain_bytes=db, domain_off=do,
+                           host_bytes=hb, host_off=ho, host_stride=self.host_stride,
+                           type_id=self.type_id[idx].copy(), addr_bytes=ab, addr_off=ao,
+                           ttl=self.ttl[idx].copy(), ports_off=po, ports=pb,
+                           ports_present=None if self.ports_present is None else self.ports_present[idx].copy(),
                            alias=self.alias, meta=dict(self.meta))
 
     # ---- accounting (SURVEY.md §8d "algorithmic bytes per record") ----------

@@ -26,6 +26,7 @@
 #include "regk_jute.cuh"
 #include "regk_decode.cuh"
 #include "regk_parents.cuh"
+#include "regk_skip.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -110,6 +111,14 @@ struct regk_ctx {
     cudaEvent_t par_ev[2] = {nullptr, nullptr};
     HostBuf h_par_len, h_par_unique, h_par_count;
     std::vector<cudaEvent_t> pipe_events;
+    /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
+    DevBuf skip_work, skip_in[11], skip_off_p, skip_off_j, skip_index, skip_bits;
+    HostBuf h_skip_status, h_skip_index, h_skip_bits;
+    struct SkipLast {
+        bool valid = false;                     /* the batch finished last was a skip-mode batch */
+        uint64_t n = 0, n_skipped = 0;
+        uint32_t bad_bits = 0;
+    } skip_last;
     /* workspace: DevStatus | two-level byte totals of both halves (stream-ordered reuse; host pipelining) */
     DevBuf work;
     /* device-resident batches rotate through a ring of workspaces that a side stream re-zeroes (and copies
@@ -150,6 +159,10 @@ struct regk_ctx {
         uint64_t n = 0;
         uint32_t flags = 0;
         uint32_t launches = 0;
+        /* REGK_SKIP_BAD: the batch's device inputs as its kernels read them, for the redo of a dirty batch */
+        const void *dev_in[11] = {};
+        uint64_t in_len[4] = {};                /* domain bytes, host bytes, address bytes, port elements */
+        uint32_t in_stride = 0;
     };
     static constexpr int NSLOTS = 64;
     Slot slots[NSLOTS];
@@ -694,9 +707,16 @@ void regk_destroy(regk_ctx *ctx)
     for (auto &ev : ctx->par_ev)
         if (ev)
             cudaEventDestroy(ev);
-    for (HostBuf *b : {&ctx->h_par_len, &ctx->h_par_unique, &ctx->h_par_count})
+    for (HostBuf *b : {&ctx->h_par_len, &ctx->h_par_unique, &ctx->h_par_count, &ctx->h_skip_status, &ctx->h_skip_index,
+             &ctx->h_skip_bits})
         if (b->p)
             cudaFreeHost(b->p);
+    for (auto &b : ctx->skip_in)
+        if (b.p)
+            cudaFree(b.p);
+    for (DevBuf *b : {&ctx->skip_work, &ctx->skip_off_p, &ctx->skip_off_j, &ctx->skip_index, &ctx->skip_bits})
+        if (b->p)
+            cudaFree(b->p);
     for (auto &sl : ctx->slots)
         for (auto &ev : sl.ev)
             if (ev)
@@ -993,6 +1013,8 @@ static void fill_peers(PeerDst &pd, const regk_job &j, void *const *bytes, uint6
     }
 }
 
+static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &first, regk_result *res);
+
 int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
 {
     if (!ctx || !b || !res)
@@ -1014,6 +1036,8 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
     if (n >= (1ull << 32))
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_register_batch: n must be < 2^32 per call");
     if (job) {
+        if (b->flags & REGK_SKIP_BAD)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_register_batch: REGK_SKIP_BAD does not combine with REGK_JOB_STEP");
         if (!ctx->job_bound)
             return fail(ctx, REGK_ERR_STATE, "regk_register_batch: REGK_JOB_STEP without a bound job (regk_job_bind)");
         if (!in_dev || !out_dev || !do_path || !do_json)
@@ -1311,6 +1335,28 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
             hp.dev[i] = need[i] && src[i] ? ctx->in[i].p : nullptr;
         }
         rc = run_pipelined(ctx, b, res, pp, path_smem, jp, json_smem, hp);
+        ctx->skip_last = regk_ctx::SkipLast{};
+        if (rc == REGK_ERR_OUT_OF_DOMAIN && (b->flags & REGK_SKIP_BAD) && !(res->bad_bits & REGK_BAD_TOO_LARGE)) {
+            /* the whole batch is staged in ctx->in: redo it from there like a dirty batch in regk_finish */
+            slot.n = n;
+            slot.flags = b->flags;
+            slot.hset = -1;
+            slot.off32 = false;                 /* the pipelined route returns 64-bit offsets */
+            slot.timed = false;
+            slot.launches = res->launches;
+            for (int i = 0; i < 11; i++)
+                slot.dev_in[i] = dev[i];
+            slot.in_len[0] = dom_len, slot.in_len[1] = host_len, slot.in_len[2] = addr_len, slot.in_len[3] = ports_len;
+            slot.in_stride = b->host_stride;
+            DevStatus st{};
+            st.bad_bits = res->bad_bits;
+            st.first_bad = ~(unsigned long long)res->first_bad;
+            return finish_skip(ctx, &slot, st, res);
+        }
+        if (rc == REGK_OK && (b->flags & REGK_SKIP_BAD)) {
+            ctx->skip_last.valid = true;
+            ctx->skip_last.n = n;
+        }
         if (rc == REGK_OK) {
             ctx->last_path_bytes = do_path ? pp.out_bytes : nullptr;
             ctx->last_path_off = do_path ? pp.out_off : nullptr;
@@ -1433,6 +1479,10 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
     slot.n = n;
     slot.flags = b->flags;
     slot.launches = launches;
+    for (int i = 0; i < 11; i++)
+        slot.dev_in[i] = dev[i];
+    slot.in_len[0] = dom_len, slot.in_len[1] = host_len, slot.in_len[2] = addr_len, slot.in_len[3] = ports_len;
+    slot.in_stride = b->host_stride;
     ctx->seq++;
     ctx->pending++;
     res->n = n;
@@ -1455,6 +1505,281 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
     if (async)
         return REGK_OK;
     return regk_finish(ctx, res);
+}
+
+/*
+ * Skip mode, dirty batch (regk_skip.cuh): the first pass found out-of-domain records and no REGK_BAD_TOO_LARGE.
+ * Fence pass -> compaction of the kept records into ctx->skip_in -> that batch through regk_register_batch as an
+ * ordinary device batch (its outputs, in ctx->path_bytes / json_bytes, are the result's streams and what the
+ * downstream calls on the batch finished last see) -> offsets expanded to all n records.  Timings describe the
+ * first pass, as for the exact-offset redo; launches count every kernel of the call.
+ */
+static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &first, regk_result *res)
+{
+    cudaStream_t s = ctx->stream;
+    const uint64_t n = slot->n;
+    const uint32_t flags = slot->flags;
+    const bool alias = flags & REGK_NODE_ALIAS, do_path = !(flags & REGK_NO_PATH), do_json = !(flags & REGK_NO_JSON);
+    const bool out_dev = flags & REGK_OUT_DEVICE;
+    if (ctx->pending) {
+        /* the redo writes the device outputs and reads this batch's inputs: only other host-set batches may be open */
+        bool ok = slot->hset >= 0;
+        for (const auto &sl : ctx->slots)
+            if (sl.in_use && sl.hset < 0)
+                ok = false;
+        if (!ok)
+            return fail(ctx, REGK_ERR_STATE,
+                "batch needs the skip-mode redo but later batches are in flight; finish them in order");
+    }
+    float ms_p = 0, ms_jl = 0, ms_j = 0;
+    if (slot->timed) {
+        cudaEventElapsedTime(&ms_p, slot->ev[0], slot->ev[1]);
+        cudaEventElapsedTime(&ms_jl, slot->ev[1], slot->ev[2]);
+        cudaEventElapsedTime(&ms_j, slot->ev[2], slot->ev[3]);
+    }
+    int rc;
+
+    /* ---- 1. fence pass: per-record bits, tile totals of the kept records ---- */
+    const uint64_t ntiles = (n + TILE - 1) / TILE, nsuper = ntiles / SUPER + 1;
+    const size_t tt_bytes = align16(ntiles * 4), st_bytes = nsuper * 8;
+    const size_t bits_off = 128 + SKIP_Q * (tt_bytes + st_bytes);
+    static_assert(sizeof(SkipStatus) <= 128, "SkipStatus");
+    if ((rc = ensure_dev(ctx, ctx->skip_work, bits_off + align16(n) + 16)) || (rc = ensure_host(ctx, ctx->h_skip_status, sizeof(SkipStatus))))
+        return rc;
+    uint8_t *wk = (uint8_t *)ctx->skip_work.p;
+    CK(cudaMemsetAsync(wk, 0, bits_off, s));
+    SkipParams sp{};
+    sp.n = n;
+    sp.alias = alias;
+    sp.do_path = do_path;
+    sp.do_json = do_json;
+    sp.ntypes = (uint32_t)ctx->types.size();
+    sp.domain_bytes = (const uint8_t *)slot->dev_in[0];
+    sp.domain_off = (const uint32_t *)slot->dev_in[1];
+    sp.host_bytes = (const uint8_t *)slot->dev_in[2];
+    sp.host_off = (const uint32_t *)slot->dev_in[3];
+    sp.host_stride = slot->in_stride;
+    sp.type_id = (const uint8_t *)slot->dev_in[4];
+    sp.addr_bytes = (const uint8_t *)slot->dev_in[5];
+    sp.addr_off = (const uint32_t *)slot->dev_in[6];
+    sp.ttl = (const int32_t *)slot->dev_in[7];
+    sp.ports_off = (const uint32_t *)slot->dev_in[8];
+    sp.ports = (const uint32_t *)slot->dev_in[9];
+    sp.ports_present = (const uint8_t *)slot->dev_in[10];
+    sp.status = (SkipStatus *)wk;
+    for (int j = 0; j < SKIP_Q; j++) {
+        sp.tile_total[j] = (uint32_t *)(wk + 128 + j * tt_bytes);
+        sp.super_total[j] = (unsigned long long *)(wk + 128 + SKIP_Q * tt_bytes + j * st_bytes);
+    }
+    sp.bits = wk + bits_off;
+    regk_fence_kernel<<<(unsigned)ntiles, TILE, 0, s>>>(sp);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(ctx->h_skip_status.p, sp.status, sizeof(SkipStatus), cudaMemcpyDeviceToHost, s));
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_CUDA, "skip-mode fence pass failed: %s", cudaGetErrorString(e));
+    const SkipStatus fs = *(const SkipStatus *)ctx->h_skip_status.p;
+    if (fs.bad_bits != first.bad_bits || fs.first_bad != first.first_bad)
+        return fail(ctx, REGK_ERR_CUDA,
+            "internal error: the skip-mode fence (bits 0x%x, first record %llu) disagrees with the compose kernels (0x%x, %llu)",
+            fs.bad_bits, ~fs.first_bad, first.bad_bits, ~first.first_bad);
+
+    /* ---- 2. compaction into the scratch batch ---- */
+    const uint64_t kept = fs.total[SKIP_REC], nskip = n - kept;
+    const uint64_t c_dom = fs.total[SKIP_DOM], c_addr = fs.total[SKIP_ADDR], c_ports = fs.total[SKIP_PORTS];
+    const uint64_t c_host = (!do_path || alias) ? 0 : (sp.host_off ? fs.total[SKIP_HOST] : kept * (uint64_t)sp.host_stride);
+    const size_t csz[11] = {(size_t)c_dom, (size_t)(kept + 1) * 4, (size_t)c_host, (size_t)(kept + 1) * 4, (size_t)kept,
+        (size_t)c_addr, (size_t)(kept + 1) * 4, (size_t)kept * 4, (size_t)(kept + 1) * 4, (size_t)c_ports * 4, (size_t)kept};
+    void *cin[11];
+    for (int i = 0; i < 11; i++) {
+        cin[i] = nullptr;
+        if (!slot->dev_in[i])
+            continue;
+        if ((rc = ensure_dev(ctx, ctx->skip_in[i], csz[i] + 16)))
+            return rc;
+        cin[i] = ctx->skip_in[i].p;
+    }
+    if ((rc = ensure_dev(ctx, ctx->skip_index, nskip * 8 + 16)) || (rc = ensure_dev(ctx, ctx->skip_bits, nskip + 16)))
+        return rc;
+    sp.c_domain_bytes = (uint8_t *)cin[0];
+    sp.c_domain_off = (uint32_t *)cin[1];
+    sp.c_host_bytes = (uint8_t *)cin[2];
+    sp.c_host_off = (uint32_t *)cin[3];
+    sp.c_type_id = (uint8_t *)cin[4];
+    sp.c_addr_bytes = (uint8_t *)cin[5];
+    sp.c_addr_off = (uint32_t *)cin[6];
+    sp.c_ttl = (int32_t *)cin[7];
+    sp.c_ports_off = (uint32_t *)cin[8];
+    sp.c_ports = (uint32_t *)cin[9];
+    sp.c_ports_present = (uint8_t *)cin[10];
+    sp.skip_index = (unsigned long long *)ctx->skip_index.p;
+    sp.skip_bits = (uint8_t *)ctx->skip_bits.p;
+    regk_compact_kernel<<<(unsigned)ntiles, TILE, 0, s>>>(sp);
+    CK(cudaGetLastError());
+
+    /* ---- the kept records alone, as an ordinary device batch (exact-offset redo included) ---- */
+    regk_batch cb{};
+    cb.n = kept;
+    cb.flags = REGK_IN_DEVICE | REGK_OUT_DEVICE | (flags & (REGK_NODE_ALIAS | REGK_NO_JSON | REGK_NO_PATH));
+    cb.host_stride = slot->in_stride;
+    cb.domain_bytes_len = c_dom;
+    cb.host_bytes_len = c_host;
+    cb.addr_bytes_len = c_addr;
+    cb.ports_len = c_ports;
+    cb.domain_bytes = c_dom ? (const uint8_t *)cin[0] : nullptr;    /* a device batch declares a non-empty array's length */
+    cb.domain_off = (const uint32_t *)cin[1];
+    cb.host_bytes = c_host ? (const uint8_t *)cin[2] : nullptr;
+    cb.host_off = (const uint32_t *)cin[3];
+    cb.type_id = (const uint8_t *)cin[4];
+    cb.addr_bytes = c_addr ? (const uint8_t *)cin[5] : nullptr;
+    cb.addr_off = (const uint32_t *)cin[6];
+    cb.ttl = (const int32_t *)cin[7];
+    cb.ports_off = (const uint32_t *)cin[8];
+    cb.ports = c_ports ? (const uint32_t *)cin[9] : nullptr;
+    cb.ports_present = (const uint8_t *)cin[10];
+    /* synchronous, and without learning a payload budget: the second run is not a batch the caller submitted */
+    const auto async_it = ctx->opt.find("async");
+    const bool had_async = async_it != ctx->opt.end();
+    const int64_t async_was = had_async ? async_it->second : 0;
+    const int pending_was = ctx->pending;
+    const double mean_was = ctx->json_mean_seen;
+    const uint64_t est_was = ctx->json_est_seen;
+    const bool learning_was = ctx->json_learning;
+    ctx->opt["async"] = 0;
+    ctx->pending = 0;
+    regk_result cres;
+    rc = regk_register_batch(ctx, &cb, &cres);
+    if (had_async)
+        ctx->opt["async"] = async_was;
+    else
+        ctx->opt.erase("async");
+    ctx->pending = pending_was;
+    ctx->json_mean_seen = mean_was;
+    ctx->json_est_seen = est_was;
+    ctx->json_learning = learning_was;
+    if (rc == REGK_ERR_OUT_OF_DOMAIN || (rc == REGK_OK && cres.bad_bits))
+        return fail(ctx, REGK_ERR_CUDA, "internal error: the kept records of a skip-mode batch still fail the fence (bits 0x%x)",
+            cres.bad_bits);
+    if (rc)
+        return rc;
+
+    /* ---- 3. offsets of all n records ---- */
+    if ((rc = ensure_dev(ctx, ctx->skip_off_p, (n + 1) * 8)) || (rc = ensure_dev(ctx, ctx->skip_off_j, (n + 1) * 8)))
+        return rc;
+    ExpandParams ep{};
+    ep.n = n;
+    ep.bits = sp.bits;
+    ep.tile_total = sp.tile_total[SKIP_REC];
+    ep.super_total = sp.super_total[SKIP_REC];
+    ep.c_path_off = do_path ? (const unsigned long long *)cres.path_off : nullptr;
+    ep.c_json_off = do_json ? (const unsigned long long *)cres.json_off : nullptr;
+    ep.path_off = (unsigned long long *)ctx->skip_off_p.p;
+    ep.json_off = (unsigned long long *)ctx->skip_off_j.p;
+    regk_expand_kernel<<<(unsigned)(n / TILE + 1), TILE, 0, s>>>(ep);
+    CK(cudaGetLastError());
+    if (!do_path)
+        CK(cudaMemsetAsync(ctx->skip_off_p.p, 0, (n + 1) * 8, s));
+    if (!do_json)
+        CK(cudaMemsetAsync(ctx->skip_off_j.p, 0, (n + 1) * 8, s));
+    uint32_t launches = slot->launches + 3 + cres.launches;
+    const bool off32 = slot->off32 && !out_dev && cres.path_total < (1ull << 32) && cres.json_total < (1ull << 32);
+    if (off32) {
+        if ((rc = narrow_offsets(ctx, ctx->skip_off_p.p, ctx->off32_p, n, s)) || (rc = narrow_offsets(ctx, ctx->skip_off_j.p, ctx->off32_j, n, s)))
+            return rc;
+        launches += 2;
+    }
+
+    memset(res, 0, sizeof *res);
+    res->n = n;
+    res->bad_bits = first.bad_bits;
+    res->first_bad = ~first.first_bad;
+    res->path_total = cres.path_total;
+    res->json_total = cres.json_total;
+    res->path_kernel_ms = ms_p;
+    res->json_kernel_ms = ms_j;
+    res->json_len_kernel_ms = ms_jl;
+    res->kernel_ms = ms_p + ms_jl + ms_j;
+    res->launches = launches;
+    res->generic_tiles = cres.generic_tiles;
+    if (out_dev) {
+        res->flags = REGK_OUT_DEVICE;
+        res->path_bytes = cres.path_bytes;
+        res->path_off = (uint64_t *)ctx->skip_off_p.p;
+        res->json_bytes = cres.json_bytes;
+        res->json_off = (uint64_t *)ctx->skip_off_j.p;
+        e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess)
+            return fail(ctx, REGK_ERR_CUDA, "skip-mode offset expansion failed: %s", cudaGetErrorString(e));
+    } else {
+        regk_ctx::HostSet *hs = slot->hset >= 0 ? &ctx->hset[slot->hset] : nullptr;
+        HostBuf &hpb = hs ? hs->h_path_bytes : ctx->h_path_bytes, &hpo = hs ? hs->h_path_off : ctx->h_path_off,
+                &hjb = hs ? hs->h_json_bytes : ctx->h_json_bytes, &hjo = hs ? hs->h_json_off : ctx->h_json_off;
+        if ((rc = ensure_host(ctx, hpb, cres.path_total + 16)) || (rc = ensure_host(ctx, hpo, (n + 1) * 8)) ||
+            (rc = ensure_host(ctx, hjb, cres.json_total + 16)) || (rc = ensure_host(ctx, hjo, (n + 1) * 8)))
+            return rc;
+        const size_t ow = off32 ? 4 : 8;
+        if (do_path) {
+            CK(cudaMemcpyAsync(hpb.p, cres.path_bytes, cres.path_total, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(hpo.p, off32 ? ctx->off32_p.p : ctx->skip_off_p.p, (n + 1) * ow, cudaMemcpyDeviceToHost, s));
+        } else {
+            memset(hpo.p, 0, (n + 1) * 8);
+        }
+        if (do_json) {
+            CK(cudaMemcpyAsync(hjb.p, cres.json_bytes, cres.json_total, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(hjo.p, off32 ? ctx->off32_j.p : ctx->skip_off_j.p, (n + 1) * ow, cudaMemcpyDeviceToHost, s));
+        } else {
+            memset(hjo.p, 0, (n + 1) * 8);
+        }
+        e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess)
+            return fail(ctx, REGK_ERR_CUDA, "skip-mode result copy failed: %s", cudaGetErrorString(e));
+        res->flags = 0;
+        res->path_bytes = (uint8_t *)hpb.p;
+        res->json_bytes = (uint8_t *)hjb.p;
+        if (off32) {
+            res->path_off32 = (uint32_t *)hpo.p;
+            res->json_off32 = (uint32_t *)hjo.p;
+        } else {
+            res->path_off = (uint64_t *)hpo.p;
+            res->json_off = (uint64_t *)hjo.p;
+        }
+    }
+    ctx->skip_last.valid = true;
+    ctx->skip_last.n = n;
+    ctx->skip_last.n_skipped = nskip;
+    ctx->skip_last.bad_bits = fs.bad_bits;
+    return REGK_OK;
+}
+
+int regk_skipped_records(regk_ctx *ctx, uint32_t flags, regk_skipped *out)
+{
+    if (!ctx || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_skipped_records: NULL argument");
+    if (!ctx->skip_last.valid)
+        return fail(ctx, REGK_ERR_STATE, "regk_skipped_records: the batch finished last was not a REGK_SKIP_BAD batch");
+    memset(out, 0, sizeof *out);
+    const regk_ctx::SkipLast &sl = ctx->skip_last;
+    out->n = sl.n;
+    out->n_skipped = sl.n_skipped;
+    out->bad_bits = sl.bad_bits;
+    if (!sl.n_skipped)
+        return REGK_OK;
+    if (flags & REGK_OUT_DEVICE) {
+        out->flags = REGK_OUT_DEVICE;
+        out->index = (const uint64_t *)ctx->skip_index.p;
+        out->bits = (const uint8_t *)ctx->skip_bits.p;
+        return REGK_OK;
+    }
+    CK(cudaSetDevice(ctx->device));
+    int rc;
+    if ((rc = ensure_host(ctx, ctx->h_skip_index, sl.n_skipped * 8)) || (rc = ensure_host(ctx, ctx->h_skip_bits, sl.n_skipped)))
+        return rc;
+    CK(cudaMemcpyAsync(ctx->h_skip_index.p, ctx->skip_index.p, sl.n_skipped * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->h_skip_bits.p, ctx->skip_bits.p, sl.n_skipped, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    out->index = (const uint64_t *)ctx->h_skip_index.p;
+    out->bits = (const uint8_t *)ctx->h_skip_bits.p;
+    return REGK_OK;
 }
 
 int regk_finish(regk_ctx *ctx, regk_result *res)
@@ -1524,6 +1849,15 @@ int regk_finish(regk_ctx *ctx, regk_result *res)
     const DevStatus st = *slot->h_status;
     const uint64_t n = slot->n;
     const bool out_dev = slot->flags & REGK_OUT_DEVICE;
+    ctx->skip_last = regk_ctx::SkipLast{};
+    if (slot->flags & REGK_SKIP_BAD) {
+        if (st.bad_bits && !(st.bad_bits & REGK_BAD_TOO_LARGE) && !st.overflow)
+            return finish_skip(ctx, slot, st, res);
+        if (!st.bad_bits) {
+            ctx->skip_last.valid = true;
+            ctx->skip_last.n = n;
+        }
+    }
     ctx->last_path_bytes = st.bad_bits ? nullptr : slot->dev_path_bytes;
     ctx->last_path_off = st.bad_bits ? nullptr : slot->dev_path_off;
     ctx->last_n = (st.bad_bits || !slot->dev_path_off) ? 0 : n;

@@ -872,6 +872,54 @@ RG_HD uint32_t addr_word_bad(uint32_t v, uint32_t keep)
     return ((v & 0x80808080u) | ((ctl | q) & keep)) != 0;
 }
 
+/* Address fence of one record: non-empty (a falsy adminIp means auto-detect upstream, register.js:143) and every byte
+ * passes addr_word_bad. */
+template <class Src>
+RG_HD uint32_t check_addr(const Src &src, uint32_t off, uint32_t al)
+{
+    if (al == 0)
+        return BAD_ADDR_BYTE;
+    uint32_t wi = off >> 2;
+    const uint32_t sh = (off & 3u) * 8u;
+    uint32_t lo = src.word(wi);
+    uint32_t bad = 0;
+    uint32_t rem = al;
+    while (rem) {
+        uint32_t nbytes = rem < 4 ? rem : 4;
+        uint32_t hi = src.word_hi(wi + 1, sh + 8 * nbytes > 32 || rem > 4);
+        uint32_t keep = low_bytes(nbytes);
+        bad |= addr_word_bad(funnel_r(lo, hi, sh) & keep, keep);
+        lo = hi;
+        wi++;
+        rem -= nbytes;
+    }
+    return bad ? (uint32_t)BAD_ADDR_BYTE : 0u;
+}
+
+/*
+ * The value fence of one record (REGK_BAD_DOMAIN_BYTE | _HOST_BYTE | _ADDR_BYTE | _TYPE_ID), for a batch's flags
+ * exactly as the compose kernels apply it: domains only when paths are composed, hostnames only for host nodes,
+ * address and type id only when payloads are composed.  Offsets are not checked here (REGK_BAD_TOO_LARGE is the
+ * compose kernels' business).  The skip-mode fence pass (regk_skip.cuh) runs this per record.
+ */
+template <class DSrc, class HSrc, class ASrc>
+RG_HD uint32_t fence_record(const DSrc &dom, uint32_t d0, uint32_t L, const HSrc &host, uint32_t h0, uint32_t H,
+    const ASrc &addr, uint32_t a0, uint32_t al, uint32_t type_id, uint32_t ntypes, bool alias, bool do_path, bool do_json)
+{
+    uint32_t bad = 0;
+    if (do_path) {
+        bad |= scan_domain(dom, d0, L).bad;
+        if (!alias)
+            bad |= check_host(host, h0, H);
+    }
+    if (do_json) {
+        bad |= check_addr(addr, a0, al);
+        if (type_id >= ntypes)
+            bad |= BAD_TYPE_ID;
+    }
+    return bad;
+}
+
 /*
  * Per-type fragment table (built on the host by regk_set_types, JSON escaping
  * already applied).  For type T:

@@ -19,7 +19,7 @@ var vasync = require('vasync');
 var regk = require('./build/Release/regk_napi.node');
 
 var TTL_ABSENT = -2147483648;
-var FLAG_NODE_ALIAS = 1 << 2, FLAG_NO_JSON = 1 << 3;
+var FLAG_NODE_ALIAS = 1 << 2, FLAG_NO_JSON = 1 << 3, FLAG_SKIP_BAD = 1 << 6;
 
 regk.init(0);
 
@@ -65,14 +65,31 @@ function slices(bytes, off, n) {
     return (out);
 }
 
-function registerBatch(records, cb) {
+/*
+ * registerBatch(records, [opts], cb).  opts.skipBad: a record outside the supported input domain does not fail the
+ * batch; out.skipped = [{index, badBits}] lists those records and their paths[i] / payloads[i] are null, for the
+ * caller to route to the stock lib/register.js (INTEGRATION.md).
+ */
+function registerBatch(records, opts, cb) {
+    if (typeof (opts) === 'function') { cb = opts; opts = {}; }
+    var skip = !!(opts && opts.skipBad);
     var types = [];
     records.forEach(function (r) { if (types.indexOf(r.type) === -1) types.push(r.type); });
     regk.setTypes(types);
-    regk.registerBatch(toBatch(records, types, 0), function (err, res) {
+    regk.registerBatch(toBatch(records, types, skip ? FLAG_SKIP_BAD : 0), function (err, res) {
         if (err) { cb(err); return; }
-        cb(null, { paths: slices(res.pathBytes, res.pathOff, records.length),
-            payloads: slices(res.jsonBytes, res.jsonOff, records.length), kernelMs: res.kernelMs });
+        var out = { paths: slices(res.pathBytes, res.pathOff, records.length),
+            payloads: slices(res.jsonBytes, res.jsonOff, records.length), kernelMs: res.kernelMs };
+        if (skip) {
+            out.skipped = [];
+            for (var k = 0; k < res.skippedBits.length; k++) {
+                var i = Number(res.skippedIndex.readBigUInt64LE(8 * k));
+                out.skipped.push({ index: i, badBits: res.skippedBits[k] });
+                out.paths[i] = null;
+                out.payloads[i] = null;
+            }
+        }
+        cb(null, out);
     });
 }
 

@@ -7,6 +7,8 @@
  *   regk.registerBatch({n, flags, hostStride, domainBytes, domainOff, hostBytes, hostOff?, typeId,
  *                       addrBytes, addrOff, ttl, portsOff?, ports?, portsPresent?},  // Buffers over SoA arrays
  *                      function (err, res) { res.pathBytes, res.pathOff, res.jsonBytes, res.jsonOff, res.kernelMs });
+ *   flags may include REGK_SKIP_BAD (1 << 6): out-of-domain records come back empty and res.skippedIndex (u64 LE) /
+ *   res.skippedBits (u8) list them (regk_skipped_records).
  *   regk.serviceRecords({n, srvceBytes, srvceOff, protoBytes, protoOff, port, ttl, keyOrder?},
  *                       function (err, res) { res.jsonBytes, res.jsonOff });          // regk_service_records
  *
@@ -100,6 +102,9 @@ typedef struct {
     /* the job's own copies of the results (made under the lock, handed to V8 as external buffers) */
     uint8_t *path_bytes, *json_bytes;
     uint64_t *path_off, *json_off;
+    uint64_t n_skipped;                 /* REGK_SKIP_BAD: the skipped records, copied like the results */
+    uint64_t *skip_index;
+    uint8_t *skip_bits;
 } job_t;
 
 static void *dup_bytes(const void *p, size_t n)
@@ -140,7 +145,19 @@ static void job_execute(napi_env env, void *data)
         j->path_off = j->result.path_off ? (uint64_t *)dup_bytes(j->result.path_off, noff) : (uint64_t *)calloc(1, noff);
         j->json_off = (uint64_t *)dup_bytes(j->result.json_off, noff);
         regk_release(g_ctx, &j->result);
-        if (!j->path_bytes || !j->json_bytes || !j->path_off || !j->json_off) {
+        if (!j->is_service && (j->batch.flags & REGK_SKIP_BAD)) {
+            regk_skipped sk;
+            j->status = regk_skipped_records(g_ctx, 0, &sk);
+            if (j->status == REGK_OK) {
+                j->n_skipped = sk.n_skipped;
+                j->skip_index = (uint64_t *)dup_bytes(sk.index, (size_t)sk.n_skipped * 8);
+                j->skip_bits = (uint8_t *)dup_bytes(sk.bits, (size_t)sk.n_skipped);
+            } else {
+                strncpy(j->error, regk_last_error(g_ctx), sizeof j->error - 1);
+            }
+        }
+        if (j->status == REGK_OK && (!j->path_bytes || !j->json_bytes || !j->path_off || !j->json_off ||
+                ((j->batch.flags & REGK_SKIP_BAD) && !j->is_service && (!j->skip_index || !j->skip_bits)))) {
             j->status = REGK_ERR_NOMEM;
             strncpy(j->error, "out of memory copying the results", sizeof j->error - 1);
         }
@@ -185,6 +202,14 @@ static void job_complete(napi_env env, napi_status st, void *data)
         j->path_off = j->json_off = NULL;
         napi_create_double(env, (double)j->result.kernel_ms, &v);
         napi_set_named_property(env, res, "kernelMs", v);
+        if (j->skip_index) {
+            napi_create_external_buffer(env, (size_t)j->n_skipped * 8, j->skip_index, free_hint, NULL, &v);
+            napi_set_named_property(env, res, "skippedIndex", v);
+            napi_create_external_buffer(env, (size_t)j->n_skipped, j->skip_bits, free_hint, NULL, &v);
+            napi_set_named_property(env, res, "skippedBits", v);
+            j->skip_index = NULL;
+            j->skip_bits = NULL;
+        }
         argv[1] = res;
         napi_call_function(env, undef, cb, 2, argv, NULL);
     }
@@ -192,6 +217,8 @@ static void job_complete(napi_env env, napi_status st, void *data)
     free(j->json_bytes);
     free(j->path_off);
     free(j->json_off);
+    free(j->skip_index);
+    free(j->skip_bits);
     types_unref(j->types);
     napi_delete_reference(env, j->cb);
     napi_delete_reference(env, j->keepalive);

@@ -179,14 +179,16 @@ def domain_to_path(domain, ctx: Optional[_native.Context] = None) -> str:
 
 
 def register_batch(records: Iterable[dict], cb: Optional[Callable] = None, ctx: Optional[_native.Context] = None,
-                   alias: bool = False):
+                   alias: bool = False, skip_bad: bool = False):
     """N host records -> (paths, payloads) in one GPU call.
 
     records: dicts {domain, hostname, type, address (adminIp), ttl?, ports?}.  Returns the HostResult
     (path(i) / json(i) accessors, packed byte streams + offsets) and, when cb is given, also calls
-    cb(None, result) / cb(err)."""
+    cb(None, result) / cb(err).  skip_bad=True: a record outside the supported input domain no longer refuses
+    the whole batch; it comes back with an empty path and payload and is listed in result.skipped (record
+    indices) / result.skipped_bits, for the caller to route to another implementation."""
     try:
-        res = (ctx or _ctx()).register_batch(RecordBatch.from_records(records, alias=alias))
+        res = (ctx or _ctx()).register_batch(RecordBatch.from_records(records, alias=alias), skip_bad=skip_bad)
     except Exception as e:  # noqa: BLE001
         if cb is None:
             raise
