@@ -387,6 +387,60 @@ typedef struct regk_jute_opts {
 int         regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *opts, regk_frames *out);
 
 /*
+ * ---- the whole mkdirp set of a batch (reference lib/register.js:107-129: zk.mkdirp(path.dirname(n)) for every node;
+ * mkdirp creates the directory AND every ancestor, and ZooKeeper creates no node whose parent is missing) -----------
+ * Works on the path stream of the batch finished last, as regk_parent_dirs does: a skip-mode batch contributes its
+ * kept records in order; a REGK_NO_PATH batch, an empty batch (it leaves no path stream), a REGK_JOB_STEP result or a
+ * pending batch is REGK_ERR_STATE.
+ * D_i = path.dirname(path_i) (parent_len of regk_parent_dirs).  D_i == "/" creates nothing.  D_i is INVALID when
+ * ZooKeeper's path check rejects it - an empty component ("//"), a trailing '/', or a byte in 0x00-0x1F or 0x7F
+ * (only alias nodes with empty labels and domains with control bytes get there): it contributes nothing and its
+ * first record is listed in invalid[].  Every other D_i contributes each of its prefixes that ends at a component
+ * boundary: /a, /a/b, ..., D_i.  The set is the union, each directory once, in a deterministic order: ascending
+ * depth (components), then ascending first record whose directory has it as a prefix - every parent precedes its
+ * children, so the whole list can be pipelined on one session.  Directory k = path_{dir_rec[k]}[0, dir_len[k]), also
+ * packed as dir_bytes[dir_off[k], dir_off[k+1]).  Bytes are compared byte for byte; a hash only picks a table slot.
+ * flags: REGK_OUT_DEVICE returns device pointers, else pinned host arrays; they stay valid until the next
+ * regk_mkdirp_dirs call (a later batch does not touch them).  Option "mkdirp_tight_table" = 1 shrinks the hash table
+ * to the smallest power of two above the entry count (long probe chains; for testing).
+ */
+typedef struct regk_dirs {
+    uint64_t n;                     /* records of the batch */
+    uint64_t n_dirs;                /* directories to create */
+    uint64_t n_invalid;             /* distinct immediate directories ZooKeeper would reject */
+    uint32_t flags;                 /* REGK_OUT_DEVICE */
+    uint32_t launches;
+    uint32_t max_depth;
+    uint32_t reserved;
+    const uint64_t *dir_rec;        /* [n_dirs] first record whose directory has this one as a prefix */
+    const uint32_t *dir_len;        /* [n_dirs] */
+    const uint64_t *depth_off;      /* [max_depth + 1] depth d is directories depth_off[d-1] .. depth_off[d]; [0] = 0 */
+    const uint8_t  *dir_bytes;      /* [dir_bytes_len] packed directory paths */
+    const uint64_t *dir_off;        /* [n_dirs + 1] */
+    const uint64_t *invalid;        /* [n_invalid] first record of each rejected directory, ascending */
+    uint64_t dir_bytes_len;
+    float kernel_ms;                /* parent_ms + closure_ms + gather_ms */
+    float parent_ms;                /* the distinct immediate directories (regk_parents.cuh kernels) */
+    float closure_ms;               /* classify + every depth's passes, including the host's read of two counters per depth */
+    float gather_ms;                /* dir_off and dir_bytes */
+} regk_dirs;
+
+int         regk_mkdirp_dirs(regk_ctx *ctx, uint32_t flags, regk_dirs *out);
+
+/*
+ * The mkdirp set of the last regk_mkdirp_dirs call (REGK_ERR_STATE without one) as ready-to-send frames: directory k
+ * becomes len | RequestHeader{xid = xid_base + k (wrapping), type = 1} | CreateRequest{path, data = empty buffer
+ * (length 0), acl = [OPEN_ACL_UNSAFE], flags = zk_flags}, in set order - the same kernel and layout as
+ * regk_jute_requests(REGK_ZK_CREATE, group = 0).  Single requests only: a multi transaction would abort as a whole on
+ * the first directory that already exists, and a NODE_EXISTS reply to one of these frames is expected (zkplus'
+ * mkdirp tolerates it).  PARITY UNPINNED: the data bytes and flags zkplus' own mkdirp sends are not in the reference
+ * tree (zkplus is a dependency, package.json:20), hence an empty buffer and zk_flags as a parameter (0 = persistent).
+ * flags: REGK_OUT_DEVICE returns device pointers, else pinned host arrays; valid until the next call.  These buffers
+ * are separate from regk_jute_requests', so the create frames of the batch and the mkdirp frames can be held together.
+ */
+int         regk_mkdirp_requests(regk_ctx *ctx, int32_t xid_base, uint32_t zk_flags, uint32_t flags, regk_frames *out);
+
+/*
  * ---- the reader side: decode paths and payloads back into records (README.md:462-480, :587-664) -----------------
  * Inverse of regk_register_batch / regk_service_records for audits of registry contents and round-trip checks:
  *   path    -> domain (labels reversed back, '/' -> '.'); for host nodes the last component is the instance name

@@ -133,6 +133,36 @@ class CParents(C.Structure):         # regk_parents
                 ("parent_len", C.c_void_p), ("unique_first", C.c_void_p), ("kernel_ms", C.c_float)]
 
 
+class CDirs(C.Structure):            # regk_dirs
+    _fields_ = [("n", C.c_uint64), ("n_dirs", C.c_uint64), ("n_invalid", C.c_uint64), ("flags", C.c_uint32),
+                ("launches", C.c_uint32), ("max_depth", C.c_uint32), ("reserved", C.c_uint32),
+                ("dir_rec", C.c_void_p), ("dir_len", C.c_void_p), ("depth_off", C.c_void_p), ("dir_bytes", C.c_void_p),
+                ("dir_off", C.c_void_p), ("invalid", C.c_void_p), ("dir_bytes_len", C.c_uint64),
+                ("kernel_ms", C.c_float), ("parent_ms", C.c_float), ("closure_ms", C.c_float), ("gather_ms", C.c_float)]
+
+
+class DirSet:
+    """Host copy of a regk_dirs: the directories register() must create for a batch, parents first.  Directory k is
+    dir_bytes[dir_off[k]:dir_off[k+1]] == path(dir_rec[k])[:dir_len[k]]; depth d is directories
+    depth_off[d-1]:depth_off[d]; `invalid` lists the first record of every directory ZooKeeper would reject."""
+
+    def __init__(self, out):
+        nd, ni = int(out.n_dirs), int(out.n_invalid)
+        self.n, self.n_dirs, self.max_depth, self.launches = int(out.n), nd, int(out.max_depth), int(out.launches)
+        self.dir_rec = _as_np(out.dir_rec, nd, np.uint64).copy()
+        self.dir_len = _as_np(out.dir_len, nd, np.uint32).copy()
+        self.depth_off = _as_np(out.depth_off, self.max_depth + 1, np.uint64).copy()
+        self.dir_bytes = _as_np(out.dir_bytes, int(out.dir_bytes_len), np.uint8).copy()
+        self.dir_off = _as_np(out.dir_off, nd + 1, np.uint64).copy()
+        self.invalid = _as_np(out.invalid, ni, np.uint64).copy()
+        self.kernel_ms, self.parent_ms = float(out.kernel_ms), float(out.parent_ms)
+        self.closure_ms, self.gather_ms = float(out.closure_ms), float(out.gather_ms)
+
+    def dirs(self):
+        b = self.dir_bytes.tobytes()
+        return [b[int(self.dir_off[k]):int(self.dir_off[k + 1])] for k in range(self.n_dirs)]
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -143,7 +173,8 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_host_free", "regk_dev_alloc", "regk_dev_free", "regk_memcpy_h2d", "regk_memcpy_d2h",
            "regk_sync", "regk_set_option", "regk_get_option", "regk_ipc_export", "regk_ipc_open", "regk_ipc_close",
            "regk_gather_push", "regk_parent_dirs", "regk_job_bind", "regk_service_records",
-           "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records"]
+           "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records", "regk_mkdirp_dirs",
+           "regk_mkdirp_requests"]
 
 _lib = None
 
@@ -195,6 +226,8 @@ def load_library():
     lib.regk_jute_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     lib.regk_decode.argtypes = [vp, C.POINTER(CDecodeIn), C.POINTER(CDecodeOut)]
     lib.regk_skipped_records.argtypes = [vp, u32, C.POINTER(CSkipped)]
+    lib.regk_mkdirp_dirs.argtypes = [vp, u32, C.POINTER(CDirs)]
+    lib.regk_mkdirp_requests.argtypes = [vp, C.c_int32, u32, u32, C.POINTER(CFrames)]
     _lib = lib
     return lib
 
@@ -501,6 +534,28 @@ class Context:
             return out
         n, nu = int(out.n), int(out.n_unique)
         return (_as_np(out.parent_len, n, np.uint32).copy(), _as_np(out.unique_first, nu, np.uint64).copy(),
+                float(out.kernel_ms))
+
+    def mkdirp_dirs(self, device: bool = False):
+        """regk_mkdirp_dirs: every directory register()'s setupDirectories must create for the batch finished last
+        (each ancestor of each node's directory once, by depth, then by first record) as a DirSet.  device=True
+        returns the raw CDirs (device pointers)."""
+        out = CDirs()
+        self._check(self._lib.regk_mkdirp_dirs(self._h, FLAG_OUT_DEVICE if device else 0, C.byref(out)))
+        return out if device else DirSet(out)
+
+    def mkdirp_requests(self, xid_base: int = 1, zk_flags: int = 0, device: bool = False):
+        """regk_mkdirp_requests: one CreateRequest (empty data, OPEN_ACL_UNSAFE, zk_flags) per directory of the last
+        mkdirp_dirs() call, xid = xid_base + k.  Returns (frame_bytes, frame_off uint64[n_dirs+1], kernel_ms), or the
+        raw CFrames with device=True."""
+        out = CFrames()
+        xid = (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31
+        self._check(self._lib.regk_mkdirp_requests(self._h, xid, int(zk_flags), FLAG_OUT_DEVICE if device else 0,
+                                                   C.byref(out)))
+        if device:
+            return out
+        n = int(out.n)
+        return (_as_np(out.frame_bytes, int(out.total), np.uint8).copy(), _as_np(out.frame_off, n + 1, np.uint64).copy(),
                 float(out.kernel_ms))
 
     # -- multi-GPU reassembly (regk_gather_push over CUDA-IPC mapped peer buffers) --

@@ -27,6 +27,7 @@
 #include "regk_decode.cuh"
 #include "regk_parents.cuh"
 #include "regk_skip.cuh"
+#include "regk_mkdirp.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -110,6 +111,14 @@ struct regk_ctx {
     DevBuf par_len, par_slot, par_table, par_totals, par_unique;
     cudaEvent_t par_ev[2] = {nullptr, nullptr};
     HostBuf h_par_len, h_par_unique, h_par_count;
+    /* regk_mkdirp_dirs (regk_mkdirp.cuh): its own parent pass, work lists, table, the set; regk_mkdirp_requests */
+    enum { MK_PLEN, MK_PSLOT, MK_PTABLE, MK_PTOTALS, MK_PUNIQUE, MK_FLAGS, MK_LIST0, MK_LIST1, MK_TOTALS, MK_TABLE,
+           MK_COUNT, MK_DREC, MK_DLEN, MK_DBYTES, MK_DOFF, MK_DEPTH, MK_INVALID, MK_ZERO, MK_FBYTES, MK_FOFF, MK_NBUF };
+    DevBuf mk[MK_NBUF];
+    HostBuf h_mk_count, h_mk_drec, h_mk_dlen, h_mk_dbytes, h_mk_doff, h_mk_depth, h_mk_invalid, h_mk_fbytes, h_mk_foff;
+    cudaEvent_t mk_ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    bool mk_valid = false;                      /* the set of the last regk_mkdirp_dirs call is in mk[MK_D*] */
+    uint64_t mk_n_dirs = 0, mk_bytes = 0;
     std::vector<cudaEvent_t> pipe_events;
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     DevBuf skip_work, skip_in[11], skip_off_p, skip_off_j, skip_index, skip_bits;
@@ -570,6 +579,162 @@ static cudaError_t launch_jute(const JuteParams &p, size_t smem, int device, cud
     return cudaGetLastError();
 }
 
+/* The request frames of one (path, payload) stream pair on the device - regk_jute_requests on the batch finished last,
+   regk_mkdirp_requests on the mkdirp set - into the given buffers.  json_off == NULL: no data (delete). */
+struct FrameSrc {
+    uint64_t n;
+    const uint8_t *path_bytes;
+    const unsigned long long *path_off;
+    const uint8_t *json_bytes;
+    const unsigned long long *json_off;
+    const char *who = "regk_jute_requests";
+};
+
+static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts *o, DevBuf &db, DevBuf &doff, HostBuf &hb,
+    HostBuf &hoff, regk_frames *out)
+{
+    const uint64_t n = src.n;
+    const bool has_data = src.json_off != nullptr;
+    const bool multi = o->group != 0;
+    const uint64_t g = multi ? o->group : 1, frames = (n + g - 1) / g;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    const bool dev_out = o->flags & REGK_OUT_DEVICE;
+    out->n = frames;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    /* totals of the two streams: the closing offsets on the device */
+    unsigned long long tot[2] = {0, 0};
+    CK(cudaMemcpyAsync(&tot[0], src.path_off + n, 8, cudaMemcpyDeviceToHost, s));
+    if (has_data)
+        CK(cudaMemcpyAsync(&tot[1], src.json_off + n, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    JuteParams p{};
+    p.n = n;
+    p.op = o->op;
+    p.mid = has_data ? 4u : 0u;
+    p.group = (uint32_t)g;
+    p.multi = multi ? 1u : 0u;
+    /* what follows the data: create - acl vector [OPEN_ACL_UNSAFE] + flags; delete / setData - the expected version */
+    uint8_t tail[48] = {0};
+    if (o->op == REGK_ZK_CREATE) {
+        static const uint8_t acl[27] = {0, 0, 0, 1, 0, 0, 0, 31, 0, 0, 0, 5, 'w', 'o', 'r', 'l', 'd', 0, 0, 0, 6, 'a', 'n', 'y', 'o', 'n', 'e'};
+        memcpy(tail, acl, 27);
+        for (int k = 0; k < 4; k++)
+            tail[27 + k] = (uint8_t)(o->zk_flags >> (24 - 8 * k));
+        p.tail_len = 31;
+    } else {
+        for (int k = 0; k < 4; k++)
+            tail[k] = (uint8_t)((uint32_t)o->version >> (24 - 8 * k));
+        p.tail_len = 4;
+    }
+    static const uint8_t multi_end[9] = {0xFF, 0xFF, 0xFF, 0xFF, 1, 0xFF, 0xFF, 0xFF, 0xFF};   /* MultiHeader {type -1, done, err -1} */
+    memcpy(tail + p.tail_len, multi_end, 9);
+    memcpy(p.tail, tail, sizeof p.tail);
+    p.per_rec = (multi ? JUTE_MULTI_HEAD : 0u) + 4u + p.mid + p.tail_len;
+    const uint64_t total = tot[0] + tot[1] + (uint64_t)p.per_rec * n + (uint64_t)JUTE_FRAME_HEAD * frames +
+        (multi ? (uint64_t)JUTE_MULTI_HEAD * frames : 0);
+    int rc;
+    if ((rc = ensure_dev(ctx, db, total + 32)) || (rc = ensure_dev(ctx, doff, (frames + 1) * 8)))
+        return rc;
+    if ((rc = ensure_dev(ctx, ctx->svc_work, 256)))
+        return rc;
+    CK(cudaMemsetAsync(ctx->svc_work.p, 0, sizeof(DevStatus), s));
+    if (n == 0)
+        CK(cudaMemsetAsync(doff.p, 0, 8, s));
+    cudaEvent_t e0 = ctx->slots[0].ev[0], e1 = ctx->slots[0].ev[1];
+    if (n) {
+        p.path_bytes = src.path_bytes;
+        p.path_off = src.path_off;
+        p.json_bytes = src.json_bytes;
+        p.json_off = src.json_off;
+        p.out_bytes = (uint8_t *)db.p;
+        p.out_off = (unsigned long long *)doff.p;
+        p.out_capacity = total;
+        p.xid_base = o->xid_base;
+        p.status = (DevStatus *)ctx->svc_work.p;
+        /* staging budgets: 9/8 of a tile's mean share of each stream plus slack (tiles beyond it go byte-wise) */
+        p.path_cap = (uint32_t)align16(std::min<uint64_t>(tot[0] * JUTE_TILE / n * 9 / 8 + 1024, 65520));
+        p.json_cap = has_data ? (uint32_t)align16(std::min<uint64_t>(tot[1] * JUTE_TILE / n * 9 / 8 + 1024, 65520)) : 0u;  /* lengths travel as 16 bits */
+        p.path_limit = tot[0] + 16;                 /* every stream buffer of this library has >= 16 bytes of slack */
+        p.json_limit = has_data ? tot[1] + 16 : 0;
+        /* ... + one owner byte and one list entry per 16-byte output block of a tile that fits the staging budgets */
+        const uint32_t max_fixed = p.per_rec + JUTE_FRAME_HEAD + JUTE_MULTI_HEAD;
+        const size_t owner_bytes = 3 * ((p.path_cap + p.json_cap + max_fixed * JUTE_TILE) / 16 + 32);   /* owner u8 + list u16 per block */
+        const size_t smem = 34 * 16 + 16 + JUTE_TILE * JUTE_SLOT + 16 + 48 + 16 + (size_t)p.path_cap + 16 + p.json_cap + 48 + owner_bytes;
+        CK(cudaEventRecord(e0, s));
+        CK(multi ? (has_data ? launch_jute<true, true>(p, smem, ctx->device, s) : launch_jute<true, false>(p, smem, ctx->device, s))
+                 : (has_data ? launch_jute<false, true>(p, smem, ctx->device, s) : launch_jute<false, false>(p, smem, ctx->device, s)));
+        CK(cudaEventRecord(e1, s));
+        out->launches = 1;
+    }
+    CK(cudaMemcpyAsync(ctx->slots[0].h_status, ctx->svc_work.p, sizeof(DevStatus), cudaMemcpyDeviceToHost, s));
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_CUDA, "%s: kernel execution failed: %s", src.who, cudaGetErrorString(e));
+    if (ctx->slots[0].h_status->overflow)
+        return fail(ctx, REGK_ERR_CUDA, "internal error: frame capacity bound exceeded");
+    if (n)
+        cudaEventElapsedTime(&out->kernel_ms, e0, e1);
+    out->total = total;
+    if (dev_out) {
+        out->frame_bytes = (const uint8_t *)db.p;
+        out->frame_off = (const uint64_t *)doff.p;
+        return REGK_OK;
+    }
+    if ((rc = ensure_host(ctx, hb, total + 16)) || (rc = ensure_host(ctx, hoff, (frames + 1) * 8)))
+        return rc;
+    if (total)
+        CK(cudaMemcpyAsync(hb.p, db.p, total, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(hoff.p, doff.p, (frames + 1) * 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    out->frame_bytes = (const uint8_t *)hb.p;
+    out->frame_off = (const uint64_t *)hoff.p;
+    return REGK_OK;
+}
+
+/* regk_parents.cuh on the path stream of the batch finished last (n >= 1 records), into the given buffers: enqueues
+   the table reset, `start` (if any) and the three kernels on the context's stream; p->parent_len / unique_first / n_unique are device
+   pointers into `len` and `unique`. */
+static int enqueue_parent_pass(regk_ctx *ctx, DevBuf &len, DevBuf &slot, DevBuf &table, DevBuf &totals, DevBuf &unique, uint64_t n,
+    cudaEvent_t start, ParentParams *out)
+{
+    cudaStream_t s = ctx->stream;
+    uint64_t slots = 1024;
+    while (slots < 2 * n)
+        slots <<= 1;
+    const uint64_t ntiles = (n + PARENT_TILE - 1) / PARENT_TILE;
+    const size_t totals_bytes = ((ntiles * 4 + 15) & ~(size_t)15) + (ntiles / SUPER + 1) * 8 + 16;
+    int rc;
+    if ((rc = ensure_dev(ctx, len, n * 4)) || (rc = ensure_dev(ctx, slot, n * 4)) || (rc = ensure_dev(ctx, table, slots * 4)) ||
+        (rc = ensure_dev(ctx, totals, totals_bytes)) || (rc = ensure_dev(ctx, unique, n * 8 + 8)))
+        return rc;
+    ParentParams p{};
+    p.n = n;
+    p.path_bytes = ctx->last_path_bytes;
+    p.path_off = ctx->last_path_off;
+    p.parent_len = (uint32_t *)len.p;
+    p.slot_of = (uint32_t *)slot.p;
+    p.owner = (uint32_t *)table.p;
+    p.mask = (uint32_t)(slots - 1);
+    p.tile_total = (uint32_t *)totals.p;
+    p.super_total = (unsigned long long *)((uint8_t *)totals.p + ((ntiles * 4 + 15) & ~(size_t)15));
+    p.unique_first = (unsigned long long *)unique.p;
+    p.n_unique = p.unique_first + n;
+    p.tail_mode = ctx->last_alias ? 0u : (ctx->last_host_off ? 2u : 1u);
+    p.host_stride = ctx->last_host_stride;
+    p.host_off = ctx->last_host_off;
+    CK(cudaMemsetAsync(p.owner, 0, slots * 4, s));
+    CK(cudaMemsetAsync(totals.p, 0, totals_bytes, s));
+    if (start)
+        CK(cudaEventRecord(start, s));                  /* the kernels' time starts here */
+    regk_parent_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p);
+    regk_parent_mark_kernel<<<(unsigned)ntiles, PARENT_TILE, 0, s>>>(p);
+    regk_parent_compact_kernel<<<(unsigned)ntiles, PARENT_TILE, 0, s>>>(p);
+    CK(cudaGetLastError());
+    *out = p;
+    return REGK_OK;
+}
+
 extern "C" {
 
 int regk_abi_version(void)
@@ -717,6 +882,16 @@ void regk_destroy(regk_ctx *ctx)
     for (DevBuf *b : {&ctx->skip_work, &ctx->skip_off_p, &ctx->skip_off_j, &ctx->skip_index, &ctx->skip_bits})
         if (b->p)
             cudaFree(b->p);
+    for (auto &b : ctx->mk)
+        if (b.p)
+            cudaFree(b.p);
+    for (HostBuf *b : {&ctx->h_mk_count, &ctx->h_mk_drec, &ctx->h_mk_dlen, &ctx->h_mk_dbytes, &ctx->h_mk_doff, &ctx->h_mk_depth,
+             &ctx->h_mk_invalid, &ctx->h_mk_fbytes, &ctx->h_mk_foff})
+        if (b->p)
+            cudaFreeHost(b->p);
+    for (auto &ev : ctx->mk_ev)
+        if (ev)
+            cudaEventDestroy(ev);
     for (auto &sl : ctx->slots)
         for (auto &ev : sl.ev)
             if (ev)
@@ -740,7 +915,8 @@ int regk_set_option(regk_ctx *ctx, const char *name, int64_t value)
 {
     if (!ctx || !name)
         return REGK_ERR_INVALID_ARG;
-    static const char *known[] = {"async", "force_generic", "dom_cap", "json_out_cap", "chunk_records", "time_every", "offsets32", nullptr};
+    static const char *known[] = {"async", "force_generic", "dom_cap", "json_out_cap", "chunk_records", "time_every", "offsets32",
+                                  "mkdirp_tight_table", nullptr};
     for (const char **k = known; *k; k++)
         if (!strcmp(*k, name)) {
             ctx->opt[name] = value;
@@ -2125,102 +2301,9 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
     if (!ctx->last_path_off || (has_data && (!ctx->last_json_off || ctx->last_n != ctx->last_json_n)))
         return fail(ctx, REGK_ERR_STATE, "regk_jute_requests: no finished batch with %s on this context",
             has_data ? "both a path and a payload stream" : "a path stream");
-    const uint64_t n = ctx->last_n;
-    const bool multi = o->group != 0;
-    const uint64_t g = multi ? o->group : 1, frames = (n + g - 1) / g;
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->stream;
-    const bool dev_out = o->flags & REGK_OUT_DEVICE;
-    out->n = frames;
-    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
-    /* totals of the two streams: the closing offsets on the device */
-    unsigned long long tot[2] = {0, 0};
-    CK(cudaMemcpyAsync(&tot[0], ctx->last_path_off + n, 8, cudaMemcpyDeviceToHost, s));
-    if (has_data)
-        CK(cudaMemcpyAsync(&tot[1], ctx->last_json_off + n, 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    JuteParams p{};
-    p.n = n;
-    p.op = o->op;
-    p.mid = has_data ? 4u : 0u;
-    p.group = (uint32_t)g;
-    p.multi = multi ? 1u : 0u;
-    /* what follows the data: create - acl vector [OPEN_ACL_UNSAFE] + flags; delete / setData - the expected version */
-    uint8_t tail[48] = {0};
-    if (o->op == REGK_ZK_CREATE) {
-        static const uint8_t acl[27] = {0, 0, 0, 1, 0, 0, 0, 31, 0, 0, 0, 5, 'w', 'o', 'r', 'l', 'd', 0, 0, 0, 6, 'a', 'n', 'y', 'o', 'n', 'e'};
-        memcpy(tail, acl, 27);
-        for (int k = 0; k < 4; k++)
-            tail[27 + k] = (uint8_t)(o->zk_flags >> (24 - 8 * k));
-        p.tail_len = 31;
-    } else {
-        for (int k = 0; k < 4; k++)
-            tail[k] = (uint8_t)((uint32_t)o->version >> (24 - 8 * k));
-        p.tail_len = 4;
-    }
-    static const uint8_t multi_end[9] = {0xFF, 0xFF, 0xFF, 0xFF, 1, 0xFF, 0xFF, 0xFF, 0xFF};   /* MultiHeader {type -1, done, err -1} */
-    memcpy(tail + p.tail_len, multi_end, 9);
-    memcpy(p.tail, tail, sizeof p.tail);
-    p.per_rec = (multi ? JUTE_MULTI_HEAD : 0u) + 4u + p.mid + p.tail_len;
-    const uint64_t total = tot[0] + tot[1] + (uint64_t)p.per_rec * n + (uint64_t)JUTE_FRAME_HEAD * frames +
-        (multi ? (uint64_t)JUTE_MULTI_HEAD * frames : 0);
-    int rc;
-    if ((rc = ensure_dev(ctx, ctx->jute_bytes, total + 32)) || (rc = ensure_dev(ctx, ctx->jute_off, (frames + 1) * 8)))
-        return rc;
-    if ((rc = ensure_dev(ctx, ctx->svc_work, 256)))
-        return rc;
-    CK(cudaMemsetAsync(ctx->svc_work.p, 0, sizeof(DevStatus), s));
-    if (n == 0)
-        CK(cudaMemsetAsync(ctx->jute_off.p, 0, 8, s));
-    cudaEvent_t e0 = ctx->slots[0].ev[0], e1 = ctx->slots[0].ev[1];
-    if (n) {
-        p.path_bytes = ctx->last_path_bytes;
-        p.path_off = ctx->last_path_off;
-        p.json_bytes = has_data ? ctx->last_json_bytes : nullptr;
-        p.json_off = has_data ? ctx->last_json_off : nullptr;
-        p.out_bytes = (uint8_t *)ctx->jute_bytes.p;
-        p.out_off = (unsigned long long *)ctx->jute_off.p;
-        p.out_capacity = total;
-        p.xid_base = o->xid_base;
-        p.status = (DevStatus *)ctx->svc_work.p;
-        /* staging budgets: 9/8 of a tile's mean share of each stream plus slack (tiles beyond it go byte-wise) */
-        p.path_cap = (uint32_t)align16(std::min<uint64_t>(tot[0] * JUTE_TILE / n * 9 / 8 + 1024, 65520));
-        p.json_cap = has_data ? (uint32_t)align16(std::min<uint64_t>(tot[1] * JUTE_TILE / n * 9 / 8 + 1024, 65520)) : 0u;  /* lengths travel as 16 bits */
-        p.path_limit = tot[0] + 16;                 /* every stream buffer of this library has >= 16 bytes of slack */
-        p.json_limit = has_data ? tot[1] + 16 : 0;
-        /* ... + one owner byte and one list entry per 16-byte output block of a tile that fits the staging budgets */
-        const uint32_t max_fixed = p.per_rec + JUTE_FRAME_HEAD + JUTE_MULTI_HEAD;
-        const size_t owner_bytes = 3 * ((p.path_cap + p.json_cap + max_fixed * JUTE_TILE) / 16 + 32);   /* owner u8 + list u16 per block */
-        const size_t smem = 34 * 16 + 16 + JUTE_TILE * JUTE_SLOT + 16 + 48 + 16 + (size_t)p.path_cap + 16 + p.json_cap + 48 + owner_bytes;
-        CK(cudaEventRecord(e0, s));
-        CK(multi ? (has_data ? launch_jute<true, true>(p, smem, ctx->device, s) : launch_jute<true, false>(p, smem, ctx->device, s))
-                 : (has_data ? launch_jute<false, true>(p, smem, ctx->device, s) : launch_jute<false, false>(p, smem, ctx->device, s)));
-        CK(cudaEventRecord(e1, s));
-        out->launches = 1;
-    }
-    CK(cudaMemcpyAsync(ctx->slots[0].h_status, ctx->svc_work.p, sizeof(DevStatus), cudaMemcpyDeviceToHost, s));
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_jute_requests: kernel execution failed: %s", cudaGetErrorString(e));
-    if (ctx->slots[0].h_status->overflow)
-        return fail(ctx, REGK_ERR_CUDA, "internal error: frame capacity bound exceeded");
-    if (n)
-        cudaEventElapsedTime(&out->kernel_ms, e0, e1);
-    out->total = total;
-    if (dev_out) {
-        out->frame_bytes = (const uint8_t *)ctx->jute_bytes.p;
-        out->frame_off = (const uint64_t *)ctx->jute_off.p;
-        return REGK_OK;
-    }
-    if ((rc = ensure_host(ctx, ctx->h_jute_bytes, total + 16)) || (rc = ensure_host(ctx, ctx->h_jute_off, (frames + 1) * 8)))
-        return rc;
-    if (total)
-        CK(cudaMemcpyAsync(ctx->h_jute_bytes.p, ctx->jute_bytes.p, total, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(ctx->h_jute_off.p, ctx->jute_off.p, (frames + 1) * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    out->frame_bytes = (const uint8_t *)ctx->h_jute_bytes.p;
-    out->frame_off = (const uint64_t *)ctx->h_jute_off.p;
-    return REGK_OK;
+    const FrameSrc src{ctx->last_n, ctx->last_path_bytes, ctx->last_path_off, has_data ? ctx->last_json_bytes : nullptr,
+                       has_data ? ctx->last_json_off : nullptr};
+    return frame_requests(ctx, src, o, ctx->jute_bytes, ctx->jute_off, ctx->h_jute_bytes, ctx->h_jute_off, out);
 }
 
 int regk_decode(regk_ctx *ctx, const regk_decode_in *in, regk_decode_out *out)
@@ -2383,43 +2466,17 @@ int regk_parent_dirs(regk_ctx *ctx, uint32_t flags, regk_parents *out)
     out->flags = dev_out ? REGK_OUT_DEVICE : 0;
     if (n == 0)
         return REGK_OK;
-    uint64_t slots = 1024;
-    while (slots < 2 * n)
-        slots <<= 1;
-    const uint64_t ntiles = (n + PARENT_TILE - 1) / PARENT_TILE;
-    const size_t totals_bytes = ((ntiles * 4 + 15) & ~(size_t)15) + (ntiles / SUPER + 1) * 8 + 16;
     int rc;
-    if ((rc = ensure_dev(ctx, ctx->par_len, n * 4)) || (rc = ensure_dev(ctx, ctx->par_slot, n * 4)) ||
-        (rc = ensure_dev(ctx, ctx->par_table, slots * 4)) || (rc = ensure_dev(ctx, ctx->par_totals, totals_bytes)) ||
-        (rc = ensure_dev(ctx, ctx->par_unique, n * 8 + 8)) || (rc = ensure_host(ctx, ctx->h_par_count, 8)))
+    if ((rc = ensure_host(ctx, ctx->h_par_count, 8)))
         return rc;
-    ParentParams p{};
-    p.n = n;
-    p.path_bytes = ctx->last_path_bytes;
-    p.path_off = ctx->last_path_off;
-    p.parent_len = (uint32_t *)ctx->par_len.p;
-    p.slot_of = (uint32_t *)ctx->par_slot.p;
-    p.owner = (uint32_t *)ctx->par_table.p;
-    p.mask = (uint32_t)(slots - 1);
-    p.tile_total = (uint32_t *)ctx->par_totals.p;
-    p.super_total = (unsigned long long *)((uint8_t *)ctx->par_totals.p + ((ntiles * 4 + 15) & ~(size_t)15));
-    p.unique_first = (unsigned long long *)ctx->par_unique.p;
-    p.n_unique = p.unique_first + n;
-    p.tail_mode = ctx->last_alias ? 0u : (ctx->last_host_off ? 2u : 1u);
-    p.host_stride = ctx->last_host_stride;
-    p.host_off = ctx->last_host_off;
     if (!ctx->par_ev[0]) {
         CK(cudaEventCreate(&ctx->par_ev[0]));
         CK(cudaEventCreate(&ctx->par_ev[1]));
     }
     cudaEvent_t e0 = ctx->par_ev[0], e1 = ctx->par_ev[1];
-    CK(cudaMemsetAsync(p.owner, 0, slots * 4, s));
-    CK(cudaMemsetAsync(ctx->par_totals.p, 0, totals_bytes, s));
-    CK(cudaEventRecord(e0, s));
-    regk_parent_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p);
-    regk_parent_mark_kernel<<<(unsigned)ntiles, PARENT_TILE, 0, s>>>(p);
-    regk_parent_compact_kernel<<<(unsigned)ntiles, PARENT_TILE, 0, s>>>(p);
-    CK(cudaGetLastError());
+    ParentParams p{};
+    if ((rc = enqueue_parent_pass(ctx, ctx->par_len, ctx->par_slot, ctx->par_table, ctx->par_totals, ctx->par_unique, n, e0, &p)))
+        return rc;
     CK(cudaEventRecord(e1, s));
     CK(cudaMemcpyAsync(ctx->h_par_count.p, p.n_unique, 8, cudaMemcpyDeviceToHost, s));
     cudaError_t e = cudaStreamSynchronize(s);
@@ -2445,6 +2502,243 @@ int regk_parent_dirs(regk_ctx *ctx, uint32_t flags, regk_parents *out)
     out->parent_len = (const uint32_t *)ctx->h_par_len.p;
     out->unique_first = (const uint64_t *)ctx->h_par_unique.p;
     return REGK_OK;
+}
+
+int regk_mkdirp_dirs(regk_ctx *ctx, uint32_t flags, regk_dirs *out)
+{
+    if (!ctx || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_mkdirp_dirs: NULL argument");
+    memset(out, 0, sizeof *out);
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_mkdirp_dirs: batches are still in flight; finish them first");
+    if (!ctx->last_path_off || !ctx->last_path_bytes)
+        return fail(ctx, REGK_ERR_STATE, "regk_mkdirp_dirs: no finished batch with a path stream on this context");
+    const uint64_t n = ctx->last_n;
+    if (n >= 0xFFFFFFFEull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_mkdirp_dirs: batch too large");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    const bool dev_out = flags & REGK_OUT_DEVICE;
+    ctx->mk_valid = false;
+    DevBuf *mk = ctx->mk;
+    int rc;
+    if ((rc = ensure_host(ctx, ctx->h_mk_count, 64)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_COUNT], 64)))
+        return rc;
+    for (auto &ev : ctx->mk_ev)
+        if (!ev)
+            CK(cudaEventCreate(&ev));
+    unsigned long long *hc = (unsigned long long *)ctx->h_mk_count.p;
+    unsigned long long *dc = (unsigned long long *)mk[regk_ctx::MK_COUNT].p;
+    auto read_counters = [&](const void *src, size_t bytes) -> int {
+        CK(cudaMemcpyAsync(hc, src, bytes, cudaMemcpyDeviceToHost, s));
+        const cudaError_t e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess)
+            return fail(ctx, REGK_ERR_CUDA, "regk_mkdirp_dirs: kernel execution failed: %s", cudaGetErrorString(e));
+        return REGK_OK;
+    };
+    std::vector<uint64_t> depth_off(1, 0);
+    uint64_t n_invalid = 0, n_dirs = 0, bytes = 0;
+    uint32_t launches = 0;
+    float ms[3] = {0, 0, 0};
+    if (n) {
+        /* 1. the distinct immediate directories, on buffers of its own (regk_parent_dirs' results stay as they are) */
+        ParentParams pp{};
+        if ((rc = enqueue_parent_pass(ctx, mk[regk_ctx::MK_PLEN], mk[regk_ctx::MK_PSLOT], mk[regk_ctx::MK_PTABLE],
+                 mk[regk_ctx::MK_PTOTALS], mk[regk_ctx::MK_PUNIQUE], n, ctx->mk_ev[0], &pp)))
+            return rc;
+        launches += 3;
+        CK(cudaEventRecord(ctx->mk_ev[1], s));
+        if ((rc = read_counters(pp.n_unique, 8)))
+            return rc;
+        const uint64_t nu = hc[0];
+        /* workspace for up to nu items per pass: flags, two work lists, two-level totals of two counts */
+        const uint64_t ntiles = (nu + MK_TILE - 1) / MK_TILE, tt = align16(ntiles * 4), st = (ntiles / SUPER + 1) * 8;
+        const size_t totals_bytes = 2 * tt + 2 * st + 16;
+        if ((rc = ensure_dev(ctx, mk[regk_ctx::MK_FLAGS], nu + 16)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_LIST0], nu * 16 + 16)) ||
+            (rc = ensure_dev(ctx, mk[regk_ctx::MK_LIST1], nu * 16 + 16)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_TOTALS], totals_bytes)) ||
+            (rc = ensure_dev(ctx, mk[regk_ctx::MK_INVALID], nu * 8 + 8)))
+            return rc;
+        uint8_t *tb = (uint8_t *)mk[regk_ctx::MK_TOTALS].p;
+        MkdirpParams p{};
+        p.path_bytes = ctx->last_path_bytes;
+        p.path_off = ctx->last_path_off;
+        p.parent_len = pp.parent_len;
+        p.unique_first = pp.unique_first;
+        p.n_unique = nu;
+        p.flags = (uint8_t *)mk[regk_ctx::MK_FLAGS].p;
+        p.tile_a = (uint32_t *)tb;
+        p.tile_b = (uint32_t *)(tb + tt);
+        p.super_a = (unsigned long long *)(tb + 2 * tt);
+        p.super_b = (unsigned long long *)(tb + 2 * tt + st);
+        p.counters = dc;
+        p.invalid = (unsigned long long *)mk[regk_ctx::MK_INVALID].p;
+        uint4 *list[2] = {(uint4 *)mk[regk_ctx::MK_LIST0].p, (uint4 *)mk[regk_ctx::MK_LIST1].p};
+        CK(cudaMemsetAsync(dc, 0, 64, s));
+        /* 2. root / invalid / depth of each; the invalid list and the depth-1 work list */
+        p.m = nu;
+        p.list_out = list[0];
+        CK(cudaMemsetAsync(tb, 0, totals_bytes, s));
+        regk_mkdirp_classify_kernel<<<(unsigned)ntiles, MK_TILE, 0, s>>>(p);
+        regk_mkdirp_split_kernel<false><<<(unsigned)ntiles, MK_TILE, 0, s>>>(p);
+        CK(cudaGetLastError());
+        launches += 2;
+        if ((rc = read_counters(dc, 32)))
+            return rc;
+        n_invalid = hc[0];
+        uint64_t m = hc[1];
+        const uint64_t entries = hc[3];
+        /* 3. the table: 64-bit slots, at most 2/3 full even before duplicates merge; "mkdirp_tight_table" = 1 sizes it
+           to the smallest power of two above the entry count (long probe chains; testing) */
+        uint64_t slots = 1024;
+        if (opt_get(ctx, "mkdirp_tight_table", 0)) {
+            slots = 2;
+            while (slots <= entries)
+                slots <<= 1;
+        } else {
+            while (slots < entries + entries / 2)
+                slots <<= 1;
+        }
+        if (slots > (1ull << 32))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_mkdirp_dirs: %llu directory entries are too many for one table",
+                (unsigned long long)entries);
+        if ((rc = ensure_dev(ctx, mk[regk_ctx::MK_TABLE], slots * 8)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DREC], entries * 8 + 8)) ||
+            (rc = ensure_dev(ctx, mk[regk_ctx::MK_DLEN], entries * 4 + 8)))
+            return rc;
+        p.table = (unsigned long long *)mk[regk_ctx::MK_TABLE].p;
+        p.mask = (uint32_t)(slots - 1);
+        p.dir_rec = (unsigned long long *)mk[regk_ctx::MK_DREC].p;
+        p.dir_len = (uint32_t *)mk[regk_ctx::MK_DLEN].p;
+        CK(cudaMemsetAsync(p.table, 0, slots * 8, s));
+        /* 4. one depth at a time: extend + insert, mark, split; the host reads how many directories and entries remain */
+        for (int cur = 0; m; cur ^= 1) {
+            const uint64_t mt = (m + MK_TILE - 1) / MK_TILE;
+            p.m = m;
+            p.list_in = list[cur];
+            p.list_out = list[cur ^ 1];
+            p.dir_base = n_dirs;
+            CK(cudaMemsetAsync(tb, 0, totals_bytes, s));
+            regk_mkdirp_insert_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(p);
+            regk_mkdirp_mark_kernel<<<(unsigned)mt, MK_TILE, 0, s>>>(p);
+            regk_mkdirp_split_kernel<true><<<(unsigned)mt, MK_TILE, 0, s>>>(p);
+            CK(cudaGetLastError());
+            launches += 3;
+            if ((rc = read_counters(dc, 24)))
+                return rc;
+            n_dirs += hc[0];
+            depth_off.push_back(n_dirs);
+            m = hc[1];
+            bytes = hc[2];
+        }
+        CK(cudaEventRecord(ctx->mk_ev[2], s));
+        /* 5. dir_off and the packed bytes */
+        const uint64_t dt = (n_dirs + MK_TILE - 1) / MK_TILE, dtt = dt * 8, dst = (dt / SUPER + 1) * 8;
+        if ((rc = ensure_dev(ctx, mk[regk_ctx::MK_DBYTES], bytes + 16)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DOFF], (n_dirs + 1) * 8)) ||
+            (rc = ensure_dev(ctx, mk[regk_ctx::MK_TOTALS], dtt + dst + 16)))
+            return rc;
+        if (n_dirs) {
+            MkGatherParams g{};
+            g.n_dirs = n_dirs;
+            g.path_bytes = ctx->last_path_bytes;
+            g.path_off = ctx->last_path_off;
+            g.dir_rec = p.dir_rec;
+            g.dir_len = p.dir_len;
+            g.tile_total = (unsigned long long *)mk[regk_ctx::MK_TOTALS].p;
+            g.super_total = (unsigned long long *)((uint8_t *)mk[regk_ctx::MK_TOTALS].p + dtt);
+            g.dir_bytes = (uint8_t *)mk[regk_ctx::MK_DBYTES].p;
+            g.dir_off = (unsigned long long *)mk[regk_ctx::MK_DOFF].p;
+            CK(cudaMemsetAsync(g.super_total, 0, dst, s));
+            regk_mkdirp_len_kernel<<<(unsigned)dt, MK_TILE, 0, s>>>(g);
+            regk_mkdirp_gather_kernel<<<(unsigned)dt, MK_TILE, 0, s>>>(g);
+            CK(cudaGetLastError());
+            launches += 2;
+        } else {
+            CK(cudaMemsetAsync(mk[regk_ctx::MK_DOFF].p, 0, 8, s));
+        }
+        CK(cudaEventRecord(ctx->mk_ev[3], s));
+        const cudaError_t e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess)
+            return fail(ctx, REGK_ERR_CUDA, "regk_mkdirp_dirs: kernel execution failed: %s", cudaGetErrorString(e));
+        for (int k = 0; k < 3; k++)
+            cudaEventElapsedTime(&ms[k], ctx->mk_ev[k], ctx->mk_ev[k + 1]);
+    } else {
+        if ((rc = ensure_dev(ctx, mk[regk_ctx::MK_DOFF], 8)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DBYTES], 16)) ||
+            (rc = ensure_dev(ctx, mk[regk_ctx::MK_DREC], 8)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DLEN], 8)) ||
+            (rc = ensure_dev(ctx, mk[regk_ctx::MK_INVALID], 8)))
+            return rc;
+        CK(cudaMemsetAsync(mk[regk_ctx::MK_DOFF].p, 0, 8, s));
+    }
+    /* depth_off was counted on the host; the device result gets a copy */
+    const size_t nd1 = depth_off.size();
+    if ((rc = ensure_host(ctx, ctx->h_mk_depth, nd1 * 8)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DEPTH], nd1 * 8)))
+        return rc;
+    memcpy(ctx->h_mk_depth.p, depth_off.data(), nd1 * 8);
+    CK(cudaMemcpyAsync(mk[regk_ctx::MK_DEPTH].p, ctx->h_mk_depth.p, nd1 * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaStreamSynchronize(s));
+    ctx->mk_valid = true;
+    ctx->mk_n_dirs = n_dirs;
+    ctx->mk_bytes = bytes;
+    out->n = n;
+    out->n_dirs = n_dirs;
+    out->n_invalid = n_invalid;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->max_depth = (uint32_t)(nd1 - 1);
+    out->dir_bytes_len = bytes;
+    out->parent_ms = ms[0];
+    out->closure_ms = ms[1];
+    out->gather_ms = ms[2];
+    out->kernel_ms = ms[0] + ms[1] + ms[2];
+    const void *dsrc[6] = {mk[regk_ctx::MK_DREC].p, mk[regk_ctx::MK_DLEN].p, mk[regk_ctx::MK_DEPTH].p, mk[regk_ctx::MK_DBYTES].p,
+                           mk[regk_ctx::MK_DOFF].p, mk[regk_ctx::MK_INVALID].p};
+    if (!dev_out) {
+        HostBuf *hb[6] = {&ctx->h_mk_drec, &ctx->h_mk_dlen, &ctx->h_mk_depth, &ctx->h_mk_dbytes, &ctx->h_mk_doff, &ctx->h_mk_invalid};
+        const size_t sz[6] = {n_dirs * 8, n_dirs * 4, 0, bytes, (n_dirs + 1) * 8, n_invalid * 8};
+        for (int k = 0; k < 6; k++) {
+            if (k == 2)
+                continue;                               /* already on the host */
+            if ((rc = ensure_host(ctx, *hb[k], sz[k] + 16)))
+                return rc;
+            if (sz[k])
+                CK(cudaMemcpyAsync(hb[k]->p, dsrc[k], sz[k], cudaMemcpyDeviceToHost, s));
+            dsrc[k] = hb[k]->p;
+        }
+        dsrc[2] = ctx->h_mk_depth.p;
+        CK(cudaStreamSynchronize(s));
+    }
+    out->dir_rec = (const uint64_t *)dsrc[0];
+    out->dir_len = (const uint32_t *)dsrc[1];
+    out->depth_off = (const uint64_t *)dsrc[2];
+    out->dir_bytes = (const uint8_t *)dsrc[3];
+    out->dir_off = (const uint64_t *)dsrc[4];
+    out->invalid = (const uint64_t *)dsrc[5];
+    return REGK_OK;
+}
+
+int regk_mkdirp_requests(regk_ctx *ctx, int32_t xid_base, uint32_t zk_flags, uint32_t flags, regk_frames *out)
+{
+    if (!ctx || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_mkdirp_requests: NULL argument");
+    memset(out, 0, sizeof *out);
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_mkdirp_requests: batches are still in flight; finish them first");
+    if (!ctx->mk_valid)
+        return fail(ctx, REGK_ERR_STATE, "regk_mkdirp_requests: no directory set on this context; call regk_mkdirp_dirs first");
+    CK(cudaSetDevice(ctx->device));
+    const uint64_t nd = ctx->mk_n_dirs;
+    int rc;
+    /* CreateRequest with an empty data buffer: the payload offsets are all zero */
+    if ((rc = ensure_dev(ctx, ctx->mk[regk_ctx::MK_ZERO], (nd + 1) * 8)))
+        return rc;
+    CK(cudaMemsetAsync(ctx->mk[regk_ctx::MK_ZERO].p, 0, (nd + 1) * 8, ctx->stream));
+    regk_jute_opts o{};
+    o.op = REGK_ZK_CREATE;
+    o.flags = flags;
+    o.xid_base = xid_base;
+    o.zk_flags = zk_flags;
+    FrameSrc src{nd, (const uint8_t *)ctx->mk[regk_ctx::MK_DBYTES].p, (const unsigned long long *)ctx->mk[regk_ctx::MK_DOFF].p,
+                 (const uint8_t *)ctx->mk[regk_ctx::MK_DBYTES].p, (const unsigned long long *)ctx->mk[regk_ctx::MK_ZERO].p};
+    src.who = "regk_mkdirp_requests";
+    return frame_requests(ctx, src, &o, ctx->mk[regk_ctx::MK_FBYTES], ctx->mk[regk_ctx::MK_FOFF], ctx->h_mk_fbytes, ctx->h_mk_foff, out);
 }
 
 int regk_release(regk_ctx *ctx, regk_result *res)

@@ -1290,5 +1290,62 @@ RG_HD bool string_equal(const uint32_t *W, uint64_t a, uint64_t b, uint32_t n)
     return true;
 }
 
+/* ------------------------------------------- the mkdirp set (regk_mkdirp.cuh) -- */
+
+constexpr uint32_t MKDIR_INVALID = 0xFFFFFFFFu;
+constexpr uint32_t MKDIR_HASH_SEED = 0x811C9DC5u;
+
+/* What mkdirp(D) creates for a directory D of L bytes, as its number of components: 0 for "/" (or an empty
+   directory: nothing to create), MKDIR_INVALID when ZooKeeper's path check would reject D - no leading '/', an
+   empty component ("//"), a trailing '/', or a byte in 0x00-0x1F or 0x7F (bytes >= 0x80 and '.' / '..' components
+   are outside the domain fence) - else the number of '/' in D. */
+RG_HD uint32_t mkdir_components(const uint8_t *p, uint32_t L)
+{
+    if (L == 0u)
+        return 0u;
+    if (p[0] != '/')
+        return MKDIR_INVALID;
+    if (L == 1u)
+        return 0u;
+    if (p[L - 1u] == '/')
+        return MKDIR_INVALID;
+    uint32_t depth = 0;
+    uint8_t prev = 0;
+    for (uint32_t i = 0; i < L; i++) {
+        const uint8_t c = p[i];
+        if (c < 0x20u || c == 0x7Fu || (c == '/' && prev == '/'))
+            return MKDIR_INVALID;
+        depth += c == '/' ? 1u : 0u;
+        prev = c;
+    }
+    return depth;
+}
+
+/* One more component of a valid directory of L bytes: the prefix that ends at `pos` (0, or a '/' of the directory)
+   is extended through the next '/' or the end.  Returns the new prefix length; *h carries the running FNV-1a state
+   of the prefix bytes, so that every ancestor's hash costs only its own last component. */
+RG_HD uint32_t mkdir_extend(const uint8_t *p, uint32_t pos, uint32_t L, uint32_t *h)
+{
+    uint32_t s = *h, k = pos;
+    do {
+        s = (s ^ p[k]) * 0x01000193u;
+        k++;
+    } while (k < L && p[k] != '/');
+    *h = s;
+    return k;
+}
+
+/* table slot hash of a prefix of L bytes whose running state is h (murmur3 finaliser) */
+RG_HD uint32_t mkdir_slot_hash(uint32_t h, uint32_t L)
+{
+    h ^= L;
+    h ^= h >> 16;
+    h *= 0x85EBCA6Bu;
+    h ^= h >> 13;
+    h *= 0xC2B2AE35u;
+    h ^= h >> 16;
+    return h;
+}
+
 }  /* namespace regk */
 #endif /* REGK_CORE_CUH */
