@@ -55,6 +55,9 @@ struct regk_ctx {
     std::string err;
     int sm_count = 0;
     int max_smem_optin = 0;
+    /* compose kernels' L2 lookahead: CTAs of one wave by dynamic shared memory (lookahead_tiles); index as in
+       smem_attr_needs_raise (0 alias paths, 1 node paths, 2 payloads) */
+    std::map<size_t, uint32_t> wave_ctas[3];
 
     /* type table */
     std::vector<std::string> types;             /* raw */
@@ -267,6 +270,22 @@ bool smem_attr_needs_raise(int device, int which, size_t bytes)
         return false;
     h = bytes;
     return true;
+}
+
+/* Lookahead distance of a compose kernel (PathParams / JsonParams::lookahead): half a wave, where a wave is how many
+   of its CTAs the GPU holds at once with `smem` bytes of dynamic shared memory.  The tile that far ahead starts about
+   half a CTA lifetime later, when its prefetched metadata has landed in L2.  On an H100, half a wave measured faster
+   than one (DESIGN.md §4). */
+int lookahead_tiles(regk_ctx *ctx, int which, const void *kernel, size_t smem, uint32_t *out)
+{
+    auto it = ctx->wave_ctas[which].find(smem);        /* batches of one workload alternate between a few budgets */
+    if (it == ctx->wave_ctas[which].end()) {
+        int per_sm = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, TILE, smem));
+        it = ctx->wave_ctas[which].emplace(smem, (uint32_t)per_sm * (uint32_t)ctx->sm_count).first;
+    }
+    *out = it->second / 2;
+    return REGK_OK;
 }
 
 }  // namespace
@@ -1025,6 +1044,23 @@ int regk_memcpy_d2h(regk_ctx *ctx, void *dst_host, const void *src_dev, size_t b
     return REGK_OK;
 }
 
+#ifdef REGK_PHASE_STAMPS
+/* development build only (tools/tile_phases.py): from now on thread 0 of every compose CTA of this context's device
+   stores its phase stamps into `dev_buf`, u64[2][tiles][8] (kernel, tile, {start, 4 phases, -, -, SM}); NULL stops */
+int regk_phase_stamps(regk_ctx *ctx, void *dev_buf, uint64_t tiles)
+{
+    if (!ctx)
+        return REGK_ERR_INVALID_ARG;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaStreamSynchronize(ctx->stream));
+    unsigned long long *p = (unsigned long long *)dev_buf;
+    const unsigned long long cap = dev_buf ? tiles : 0;
+    CK(cudaMemcpyToSymbol(regk::g_phase_buf, &p, sizeof(p)));
+    CK(cudaMemcpyToSymbol(regk::g_phase_cap, &cap, sizeof(cap)));
+    return REGK_OK;
+}
+#endif
+
 int regk_sync(regk_ctx *ctx)
 {
     if (!ctx)
@@ -1436,6 +1472,9 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
                 CK(cudaFuncSetAttribute(regk_path_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)path_smem));
             }
         }
+        if ((rc = lookahead_tiles(ctx, alias ? 0 : 1, alias ? (const void *)regk_path_kernel<true, false> : (const void *)regk_path_kernel<false, false>,
+                 path_smem, &pp.lookahead)))
+            return rc;
     }
     JsonParams jp{};
     size_t json_smem = 0;
@@ -1496,6 +1535,8 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
         if (smem_attr_needs_raise(ctx->device, 2, json_smem)) {
             CK(cudaFuncSetAttribute(regk_json_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)json_smem));
         }
+        if ((rc = lookahead_tiles(ctx, 2, (const void *)regk_json_kernel, json_smem, &jp.lookahead)))
+            return rc;
     }
 
     if (pipelined) {

@@ -333,6 +333,67 @@ __device__ __forceinline__ T block_scan(T *warp_sum /* smem[WARPS] */, T v, T *t
 }
 
 /*
+ * ---- L2 lookahead ----
+ * Every compose CTA starts with a chain of dependent round trips: its records' offsets and metadata, then the
+ * bytes they point at.  So the CTA of tile k also asks the memory system to bring the first link of that chain for
+ * tile k + D into L2 (cp.async.bulk.prefetch.L2, SASS UBLKPF): the tile's slices of the per-record arrays
+ * (offsets, type ids, ttls, port flags), at addresses known from the tile index alone.  The payload kernel also
+ * prefetches the second link, its address bytes and port values, between two offsets its lanes load at CTA start;
+ * those offsets are not validated yet, so a reversed or oversized range is dropped and every range is clipped to
+ * the caller's buffer.  D is half a wave of the launch (PathParams / JsonParams::lookahead, from the host's
+ * occupancy figure; 0 = off): tile k + D starts about half a CTA lifetime later, when the prefetch has landed.  The
+ * lanes of the last warp issue it, one array per lane, off the tile's own chain (thread 0, warp 0).
+ *
+ * Measured on an H100 (DESIGN.md §4): prefetching the path kernel's byte ranges (domains, hostnames, which its bulk
+ * copies fetch anyway) made the step slower at every distance from a quarter of a wave to two waves.
+ */
+__device__ __forceinline__ void prefetch_l2(const void *base, uint64_t lo, uint64_t hi, uint64_t limit)
+{
+    hi = min(hi, limit);
+    const uintptr_t a = ((uintptr_t)base + lo + 15u) & ~(uintptr_t)15, b = ((uintptr_t)base + hi) & ~(uintptr_t)15;
+    if (base && hi > lo && b > a)
+        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(a), "r"((uint32_t)(b - a)));
+}
+
+/* elements [r0, r1) of an array of n elements of `esz` bytes (NULL: absent) */
+__device__ __forceinline__ void prefetch_slice(const void *a, uint32_t esz, uint64_t r0, uint64_t r1, uint64_t n)
+{
+    prefetch_l2(a, esz * r0, esz * r1, esz * n);
+}
+
+/* records [r0, r1) of the tile `lookahead` tiles after this CTA's (the caller has checked that it exists) */
+__device__ __forceinline__ void look_tile(uint32_t lookahead, uint64_t n, uint64_t &r0, uint64_t &r1)
+{
+    r0 = ((uint64_t)blockIdx.x + lookahead) * TILE;
+    r1 = min(r0 + TILE, n);
+}
+
+/*
+ * ---- per-CTA phase stamps (development build only: -DREGK_PHASE_STAMPS, tools/tile_phases.py) ----
+ * Thread 0 of every compose CTA stores clock64() at five points of its tile, and the SM it ran on, into
+ * g_phase_buf[kernel][tile][8] (kernel 0: paths, 1: payloads; set by regk_phase_stamps()).
+ */
+#ifdef REGK_PHASE_STAMPS
+__device__ unsigned long long *g_phase_buf;
+__device__ unsigned long long g_phase_cap;
+__device__ __forceinline__ void phase_stamp(uint32_t kernel, uint32_t phase)
+{
+    if (threadIdx.x == 0 && g_phase_buf && blockIdx.x < g_phase_cap) {
+        unsigned long long *e = g_phase_buf + ((unsigned long long)kernel * g_phase_cap + blockIdx.x) * 8u;
+        e[phase] = clock64();
+        if (phase == 0) {
+            uint32_t sm;
+            asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+            e[7] = sm;
+        }
+    }
+}
+#define REGK_PHASE(kernel, phase) phase_stamp(kernel, phase)
+#else
+#define REGK_PHASE(kernel, phase) ((void)0)
+#endif
+
+/*
  * Two-level totals instead of a scan pass: producers add each warp's byte count into tile_total[tile]
  * (u32) and super_total[tile / SUPER] (u64) with atomics; a consumer CTA derives its own exclusive base
  * as  sum(super_total[0 .. tile/SUPER)) + sum(tile_total[SUPER*(tile/SUPER) .. tile))  — at most
@@ -402,6 +463,7 @@ struct JsonParams {
     uint64_t addr_limit, ports_limit;   /* bytes behind addr_bytes / elements behind ports (trusted) */
     uint32_t out_cap;                   /* shared-memory budget of the output image */
     uint32_t force_generic;
+    uint32_t lookahead;                 /* tiles between a CTA and the tile whose inputs it prefetches (0: none) */
     PeerDst peer;                       /* multi-GPU job: the other ranks' whole-job payload buffers */
 };
 
@@ -466,6 +528,40 @@ __device__ __forceinline__ uint32_t json_meta_len(const JsonParams &p, const Jso
     return json_length(tf.f1_len, tf.f2_len, m.al, m.has_ttl, m.ttl, m.has_ports, m.k, port_digits);
 }
 
+/* lookahead, payload metadata of records [r0, r1): lane j < 5 takes one array */
+__device__ __forceinline__ void look_json(const JsonParams &p, uint32_t j, uint64_t r0, uint64_t r1)
+{
+    if (j == 0)
+        prefetch_slice(p.type_id, 1, r0, r1, p.n);
+    else if (j == 1)
+        prefetch_slice(p.addr_off, 4, r0, r1 + 1, p.n + 1);
+    else if (j == 2)
+        prefetch_slice(p.ttl, 4, r0, r1, p.n);
+    else if (j == 3)
+        prefetch_slice(p.ports_off, 4, r0, r1 + 1, p.n + 1);
+    else if (j == 4)
+        prefetch_slice(p.ports_present, 1, r0, r1, p.n);
+}
+
+/* lookahead, payload kernel only: the second link of its chain, the address bytes (lane 5) and port values (lane 6),
+   lie between two entries of the offsets array returned here; the lane loads them at CTA start */
+__device__ __forceinline__ const uint32_t *look_json_bounds(const JsonParams &p, uint32_t j)
+{
+    return j == 5 ? p.addr_off : j == 6 ? p.ports_off : nullptr;
+}
+
+/* b0, b1: the two offsets look_json_bounds named, not validated yet: a reversed range, or one larger than four image
+   budgets, is dropped; the rest is clipped to the buffer */
+__device__ __forceinline__ void look_json_bytes(const JsonParams &p, uint32_t j, uint32_t b0, uint32_t b1)
+{
+    if (b1 < b0 || b1 - b0 > 4u * p.out_cap)
+        return;
+    if (j == 5)
+        prefetch_l2(p.addr_bytes, b0, b1, p.addr_limit);
+    else if (j == 6)
+        prefetch_l2(p.ports, 4ull * b0, 4ull * b1, 4ull * p.ports_limit);
+}
+
 /* ================================================================ paths == */
 
 struct PathParams {
@@ -488,9 +584,24 @@ struct PathParams {
     uint64_t dom_limit, host_limit;     /* bytes behind domain_bytes / host_bytes (trusted, from the caller) */
     uint32_t dom_cap, host_cap, out_cap;        /* shared-memory budgets in bytes */
     uint32_t force_generic;
+    uint32_t lookahead;                 /* tiles between a CTA and the tile whose inputs it prefetches (0: none) */
     const unsigned long long *bias_in;  /* optional, device: added to off_bias (job: path bytes of the ranks before this one) */
     PeerDst peer;                       /* multi-GPU job: the other ranks' whole-job path buffers */
 };
+
+/* lookahead of the path kernel, records [r0, r1): lanes 0-1 take the path offsets, lanes 2-6 the side job's payload
+   metadata */
+template <bool ALIAS>
+__device__ __forceinline__ void look_path(const PathParams &p, const JsonParams &jp, bool side, uint32_t lane, uint64_t r0,
+    uint64_t r1)
+{
+    if (lane == 0)
+        prefetch_slice(p.domain_off, 4, r0, r1 + 1, p.n + 1);
+    else if (!ALIAS && lane == 1)
+        prefetch_slice(p.host_off, 4, r0, r1 + 1, p.n + 1);
+    else if (side && lane >= 2)
+        look_json(jp, lane - 2, r0, r1);
+}
 
 /* closed-form offset of record r's path when no label is empty: path_len = L + 2 + H (alias: L + 1) */
 template <bool ALIAS>
@@ -579,6 +690,7 @@ __global__ void __launch_bounds__(TILE, REGK_MINB_PATH) regk_path_kernel(const P
     __shared__ TilePlan s_plan;
     __shared__ uint8_t *s_pb[REGK_MAX_PEERS - 1];
     __shared__ unsigned long long *s_po[REGK_MAX_PEERS - 1];
+    REGK_PHASE(0, 0);
     const uint32_t npeers = p.peer.n;
     if (npeers)
         peer_tables(p.peer, s_pb, s_po);                        /* published by the plan barrier */
@@ -663,7 +775,13 @@ __global__ void __launch_bounds__(TILE, REGK_MINB_PATH) regk_path_kernel(const P
         exact_base = tile_base_from_totals(p.tile_total, p.super_total, tile);
     if (exact && t == 0)
         *reinterpret_cast<unsigned long long *>(warp_sum) = exact_base;     /* read back after the barrier, before any scan */
+    if (p.lookahead && tile + p.lookahead < gridDim.x && t >= TILE - 32) {
+        uint64_t l0, l1;
+        look_tile(p.lookahead, p.n, l0, l1);
+        look_path<ALIAS>(p, jp, side, t & 31u, l0, l1);
+    }
     __syncthreads();                                            /* plan, mbarrier init (and exact base) published */
+    REGK_PHASE(0, 1);
 
     /* the side job runs while the bulk copies are in flight: its second-hop loads (port values) cost nothing
        here, and its registers are free again before the composing starts */
@@ -718,6 +836,7 @@ __global__ void __launch_bounds__(TILE, REGK_MINB_PATH) regk_path_kernel(const P
                 stage_in(s_host, p.host_bytes, s_plan.HB0, s_plan.HB0 + s_plan.host_span, p.host_limit);
             __syncthreads();
         }
+        REGK_PHASE(0, 2);
         /* cooperative pre-pass: lower-case, dot bitmap, '.' -> '/', fence (vectorised, no divergence) */
         uint32_t *dom_w = reinterpret_cast<uint32_t *>(s_dom);
         const uint32_t *bits_w = reinterpret_cast<const uint32_t *>(s_bits);
@@ -763,10 +882,12 @@ __global__ void __launch_bounds__(TILE, REGK_MINB_PATH) regk_path_kernel(const P
                 sink.tail();                                    /* phase B: shared boundary words */
             fence_proxy_async();
             __syncthreads();
+            REGK_PHASE(0, 3);
             if (npeers)
                 flush_out_job(p.out_bytes, s_pb, npeers, s_out, tile_base, tile_total);
             else
                 flush_out(p.out_bytes, s_out, tile_base, tile_total);
+            REGK_PHASE(0, 4);
         }
     } else {
         /* generic path: compose straight from / to global memory */
@@ -860,6 +981,7 @@ __global__ void __launch_bounds__(TILE, REGK_MINB_JSON) regk_json_kernel(const J
     __shared__ JsonPlan s_plan;
     __shared__ uint8_t *s_pb[REGK_MAX_PEERS - 1];
     __shared__ unsigned long long *s_po[REGK_MAX_PEERS - 1];
+    REGK_PHASE(1, 0);
     const uint32_t npeers = p.peer.n;
     if (npeers)
         peer_tables(p.peer, s_pb, s_po);                        /* published by the scan's barriers */
@@ -891,6 +1013,17 @@ __global__ void __launch_bounds__(TILE, REGK_MINB_JSON) regk_json_kernel(const J
         }
     }
 
+    const bool look = p.lookahead && tile + p.lookahead < gridDim.x && t >= TILE - 32;
+    uint32_t lb0 = 0, lb1 = 0;
+    if (look) {
+        uint64_t l0, l1;
+        look_tile(p.lookahead, p.n, l0, l1);
+        look_json(p, t & 31u, l0, l1);
+        if (const uint32_t *bo = look_json_bounds(p, t & 31u)) {
+            lb0 = bo[l0];
+            lb1 = bo[l1];
+        }
+    }
     const JsonMeta m = json_meta(p, r);
     uint32_t bad = m.bad;
     const uint32_t a0 = m.a0, al = m.al, k = m.k;
@@ -927,9 +1060,13 @@ __global__ void __launch_bounds__(TILE, REGK_MINB_JSON) regk_json_kernel(const J
        the plan and the mbarrier init */
     const TypeFrag tf = reinterpret_cast<const TypeFrag *>(p.frag_blob)[m.tid];
     const uint32_t len = live ? json_meta_len(p, m, tf) : 0;
+    if (look)
+        look_json_bytes(p, t & 31u, lb0, lb1);                 /* the bounds have landed by now */
+    REGK_PHASE(1, 1);
     uint32_t tot;
     const uint32_t local = block_scan<uint32_t>(warp_sum, len, &tot);
     mbar_wait(&s_bar, 0);                                       /* fragment table has landed */
+    REGK_PHASE(1, 2);
     const unsigned long long tile_base = s_plan.tile_base;
     const uint32_t tile_total = s_plan.tile_total;
     const uint32_t flags = s_plan.flags;
@@ -955,10 +1092,12 @@ __global__ void __launch_bounds__(TILE, REGK_MINB_JSON) regk_json_kernel(const J
             sink.tail();                                        /* phase B: shared boundary words */
         fence_proxy_async();
         __syncthreads();
+        REGK_PHASE(1, 3);
         if (npeers)
             flush_out_job(p.out_bytes, s_pb, npeers, s_out, tile_base, tile_total);
         else
             flush_out(p.out_bytes, s_out, tile_base, tile_total);
+        REGK_PHASE(1, 4);
     } else {
         if (t == 0)
             atomicAdd(&p.status->generic_tiles, 1u);
