@@ -499,6 +499,68 @@ typedef struct regk_decode_out {
 
 int         regk_decode(regk_ctx *ctx, const regk_decode_in *in, regk_decode_out *out);
 
+/*
+ * ---- reconcile a batch with a snapshot of the registry (the batch form of the reference's heartbeat check,
+ * lib/zk.js:21-44 and lib/index.js:55-159: stat every node, register again what is missing) ----------------------
+ * Desired = the batch finished last on this context, as for regk_jute_requests: paths AND payloads required; a
+ * skip-mode batch contributes its kept records in order; no batch, a REGK_NO_PATH / REGK_NO_JSON batch, an empty batch
+ * (it leaves no streams), a REGK_JOB_STEP result or a pending batch is REGK_ERR_STATE.
+ * Observed = a snapshot of m nodes (path j, data j) in the layout regk_decode accepts: host streams, or device streams
+ * with REGK_IN_DEVICE (bytes 4-byte aligned, offsets 8-byte aligned); u64 CSR offsets; path_total / json_total are
+ * required for device streams; host_nodes is ignored, REGK_DECODE_LAST is REGK_ERR_INVALID_ARG.  Offsets that are not
+ * monotone or reach past the totals are REGK_ERR_INVALID_ARG naming the smallest bad node (host snapshots are checked
+ * on the host, device snapshots by the first kernel before any byte of that node is read).  A snapshot in which two
+ * nodes have the same path is malformed (a registry cannot hold that): REGK_ERR_INVALID_ARG naming the later node.
+ * The snapshot must cover exactly the namespace the batch owns: every node it holds that the batch does not produce -
+ * directories included - is classed DELETE.
+ * Nodes are keyed by their path bytes, compared byte for byte (a hash only picks a table slot); the class depends on
+ * bytes alone (no ephemeral owners, no versions).  Record i:
+ *   REGK_DELTA_DUP     an earlier record of the batch has the same path (the first occurrence decides); no request
+ *   REGK_DELTA_CREATE  no node has path i
+ *   REGK_DELTA_UPDATE  the node with path i holds data that differs from payload i in length or in a byte
+ *   REGK_DELTA_SAME    the node with path i holds payload i
+ * match[i] = that node's index or UINT64_MAX (DUP records carry their path's match too).  Node j: REGK_DELTA_KEEP if
+ * some record has path j, else REGK_DELTA_DELETE.  create / update / dup list record indices, del snapshot indices,
+ * all ascending.  n and m must be < 2^32 - 1.  flags: REGK_OUT_DEVICE returns device pointers, else pinned host
+ * arrays; valid until the next regk_reconcile call.
+ * The call also gathers the three request sets (create paths + payloads, update paths + payloads, delete paths) into
+ * streams of the library's own, so regk_reconcile_requests needs neither the snapshot nor the batch afterwards; a later
+ * batch does not touch them.  Option "reconcile_tight_table" = 1 sizes both hash tables to the smallest power of two
+ * above their entry count (long probe chains; for testing).
+ */
+#define REGK_DELTA_SAME   0u        /* cls[] */
+#define REGK_DELTA_CREATE 1u
+#define REGK_DELTA_UPDATE 2u
+#define REGK_DELTA_DUP    3u
+#define REGK_DELTA_KEEP   0u        /* obs_cls[] */
+#define REGK_DELTA_DELETE 1u
+
+typedef struct regk_delta {
+    uint64_t n, m;                  /* records of the batch finished last / nodes of the snapshot */
+    uint64_t n_same, n_create, n_update, n_dup, n_delete;
+    uint32_t flags, launches;       /* REGK_OUT_DEVICE */
+    const uint8_t  *cls;            /* [n] REGK_DELTA_SAME / _CREATE / _UPDATE / _DUP */
+    const uint64_t *match;          /* [n] */
+    const uint8_t  *obs_cls;        /* [m] REGK_DELTA_KEEP / _DELETE */
+    const uint64_t *create, *update, *dup;   /* ascending record indices */
+    const uint64_t *del;            /* [n_delete] ascending snapshot indices */
+    float kernel_ms;
+} regk_delta;
+
+int         regk_reconcile(regk_ctx *ctx, const regk_decode_in *snapshot, uint32_t flags, regk_delta *out);
+
+/*
+ * The requests that repair the registry, from the last regk_reconcile call (REGK_ERR_STATE without one), framed
+ * exactly as regk_jute_requests frames a batch: frame k is list entry k (group = 0) or multi transaction k, xid =
+ * xid_base + k; group, version and zk_flags mean what they mean there.
+ *   REGK_ZK_CREATE   the create list: CreateRequest{path i, payload i}
+ *   REGK_ZK_SETDATA  the update list: SetDataRequest{path i, payload i, version}
+ *   REGK_ZK_DELETE   the delete list: DeleteRequest{snapshot path j, version}
+ * Send them in this order: delete, then the creates' parents (regk_mkdirp_dirs / regk_mkdirp_requests), then create,
+ * then setData.  flags: REGK_OUT_DEVICE returns device pointers, else pinned host arrays; valid until the next call.
+ */
+int         regk_reconcile_requests(regk_ctx *ctx, const regk_jute_opts *opts, regk_frames *out);
+
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);
 int64_t     regk_get_option(const regk_ctx *ctx, const char *name);

@@ -163,6 +163,39 @@ class DirSet:
         return [b[int(self.dir_off[k]):int(self.dir_off[k + 1])] for k in range(self.n_dirs)]
 
 
+class CDelta(C.Structure):           # regk_delta
+    _fields_ = [("n", C.c_uint64), ("m", C.c_uint64), ("n_same", C.c_uint64), ("n_create", C.c_uint64),
+                ("n_update", C.c_uint64), ("n_dup", C.c_uint64), ("n_delete", C.c_uint64),
+                ("flags", C.c_uint32), ("launches", C.c_uint32),
+                ("cls", C.c_void_p), ("match", C.c_void_p), ("obs_cls", C.c_void_p),
+                ("create", C.c_void_p), ("update", C.c_void_p), ("dup", C.c_void_p), ("del_", C.c_void_p),
+                ("kernel_ms", C.c_float)]
+
+
+DELTA_SAME, DELTA_CREATE, DELTA_UPDATE, DELTA_DUP = 0, 1, 2, 3       # Delta.cls
+DELTA_KEEP, DELTA_DELETE = 0, 1                                      # Delta.obs_cls
+
+
+class Delta:
+    """Host copy of a regk_delta: how the batch finished last differs from a snapshot of the registry.  cls[i] is
+    DELTA_SAME / _CREATE / _UPDATE / _DUP for record i, match[i] the snapshot node with its path (UINT64_MAX: none),
+    obs_cls[j] DELTA_KEEP / _DELETE for node j; create / update / dup are ascending record indices, delete ascending
+    snapshot indices."""
+
+    def __init__(self, out):
+        n, m = int(out.n), int(out.m)
+        self.n, self.m, self.launches, self.kernel_ms = n, m, int(out.launches), float(out.kernel_ms)
+        self.n_same, self.n_create, self.n_update = int(out.n_same), int(out.n_create), int(out.n_update)
+        self.n_dup, self.n_delete = int(out.n_dup), int(out.n_delete)
+        self.cls = _as_np(out.cls, n, np.uint8).copy()
+        self.match = _as_np(out.match, n, np.uint64).copy()
+        self.obs_cls = _as_np(out.obs_cls, m, np.uint8).copy()
+        self.create = _as_np(out.create, self.n_create, np.uint64).copy()
+        self.update = _as_np(out.update, self.n_update, np.uint64).copy()
+        self.dup = _as_np(out.dup, self.n_dup, np.uint64).copy()
+        self.delete = _as_np(out.del_, self.n_delete, np.uint64).copy()
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -174,7 +207,7 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_sync", "regk_set_option", "regk_get_option", "regk_ipc_export", "regk_ipc_open", "regk_ipc_close",
            "regk_gather_push", "regk_parent_dirs", "regk_job_bind", "regk_service_records",
            "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records", "regk_mkdirp_dirs",
-           "regk_mkdirp_requests"]
+           "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests"]
 
 _lib = None
 
@@ -228,6 +261,8 @@ def load_library():
     lib.regk_skipped_records.argtypes = [vp, u32, C.POINTER(CSkipped)]
     lib.regk_mkdirp_dirs.argtypes = [vp, u32, C.POINTER(CDirs)]
     lib.regk_mkdirp_requests.argtypes = [vp, C.c_int32, u32, u32, C.POINTER(CFrames)]
+    lib.regk_reconcile.argtypes = [vp, C.POINTER(CDecodeIn), u32, C.POINTER(CDelta)]
+    lib.regk_reconcile_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     _lib = lib
     return lib
 
@@ -552,6 +587,33 @@ class Context:
         xid = (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31
         self._check(self._lib.regk_mkdirp_requests(self._h, xid, int(zk_flags), FLAG_OUT_DEVICE if device else 0,
                                                    C.byref(out)))
+        if device:
+            return out
+        n = int(out.n)
+        return (_as_np(out.frame_bytes, int(out.total), np.uint8).copy(), _as_np(out.frame_off, n + 1, np.uint64).copy(),
+                float(out.kernel_ms))
+
+    # -- reconcile the batch finished last with a snapshot of the registry --
+    def reconcile(self, snapshot, device: bool = False):
+        """regk_reconcile: compare the batch finished last with `snapshot` (a batch.Snapshot, host arrays or CUDA
+        tensors) and return a Delta, or the raw CDelta (device pointers) with device=True.  Also gathers the requests
+        that repair the difference for reconcile_requests()."""
+        cin, keep = snapshot.cdecode_in()
+        out = CDelta()
+        rc = self._lib.regk_reconcile(self._h, C.byref(cin), FLAG_OUT_DEVICE if device else 0, C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else Delta(out)
+
+    def reconcile_requests(self, op: int = ZK_CREATE, xid_base: int = 1, zk_flags: int = 1, version: int = -1,
+                           group: int = 0, device: bool = False):
+        """regk_reconcile_requests: the create (ZK_CREATE), setData (ZK_SETDATA) or delete (ZK_DELETE) requests of the
+        last reconcile(), framed as jute_requests() frames a batch.  Returns (frame_bytes, frame_off, kernel_ms), or
+        the raw CFrames with device=True."""
+        xid = (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31
+        o = CJuteOpts(int(op), FLAG_OUT_DEVICE if device else 0, xid, int(zk_flags), int(version), int(group))
+        out = CFrames()
+        self._check(self._lib.regk_reconcile_requests(self._h, C.byref(o), C.byref(out)))
         if device:
             return out
         n = int(out.n)

@@ -235,6 +235,59 @@ class RecordBatch:
         return tot
 
 
+@dataclass
+class Snapshot:
+    """What a registry holds under the namespace a batch owns: m nodes, node j = (path j, data j), as u64 CSR streams
+    (the layout regk_decode accepts).  Either all four arrays are host NumPy arrays (uint8 bytes, uint64 offsets) or
+    all four are CUDA tensors (uint8 bytes, int64 offsets); a device snapshot's streams end at the byte tensors' ends.
+    Input of Context.reconcile()."""
+    path_bytes: object
+    path_off: object
+    json_bytes: object
+    json_off: object
+
+    @classmethod
+    def from_nodes(cls, nodes: Iterable) -> "Snapshot":
+        """[(path, data), ...] -> host Snapshot"""
+        nodes = list(nodes)
+
+        def pack(strings):
+            off = np.zeros(len(strings) + 1, np.uint64)
+            if strings:
+                np.cumsum([len(s) for s in strings], out=off[1:])
+            return np.frombuffer(b"".join(strings), np.uint8).copy(), off
+        pb, po = pack([_b(p) for p, _ in nodes])
+        jb, jo = pack([_b(d) for _, d in nodes])
+        return cls(pb, po, jb, jo)
+
+    @property
+    def device(self) -> bool:
+        return hasattr(self.path_off, "data_ptr")
+
+    @property
+    def m(self) -> int:
+        return (self.path_off.numel() if self.device else len(self.path_off)) - 1
+
+    def cdecode_in(self):
+        """regk_decode_in over the four arrays.  Returns (struct, keepalive)."""
+        from ._native import CDecodeIn
+        import ctypes as C
+        if self.device:
+            arrs = [self.path_bytes, self.path_off, self.json_bytes, self.json_off]
+            if not all(a.is_cuda and a.is_contiguous() for a in arrs):
+                raise ValueError("a device snapshot is four contiguous CUDA tensors")
+            ptr = [a.data_ptr() or None for a in arrs]
+            cin = CDecodeIn(n=self.m, flags=FLAG_IN_DEVICE, path_total=self.path_bytes.numel(),
+                            json_total=self.json_bytes.numel(), path_bytes=ptr[0], path_off=ptr[1], json_bytes=ptr[2],
+                            json_off=ptr[3])
+            return cin, arrs
+        keep = [np.ascontiguousarray(self.path_bytes, np.uint8), np.ascontiguousarray(self.path_off, np.uint64),
+                np.ascontiguousarray(self.json_bytes, np.uint8), np.ascontiguousarray(self.json_off, np.uint64)]
+        p = [a.ctypes.data_as(C.c_void_p) for a in keep]
+        cin = CDecodeIn(n=len(keep[1]) - 1, flags=0, path_bytes=p[0], path_off=p[1], json_bytes=p[2], json_off=p[3])
+        return cin, keep
+
+
 SERVICE_KEYS = ("srvce", "proto", "port", "ttl")      # key ids 0..3 of regk_service_batch.key_order
 
 

@@ -28,6 +28,7 @@
 #include "regk_parents.cuh"
 #include "regk_skip.cuh"
 #include "regk_mkdirp.cuh"
+#include "regk_reconcile.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -122,6 +123,16 @@ struct regk_ctx {
     cudaEvent_t mk_ev[4] = {nullptr, nullptr, nullptr, nullptr};
     bool mk_valid = false;                      /* the set of the last regk_mkdirp_dirs call is in mk[MK_D*] */
     uint64_t mk_n_dirs = 0, mk_bytes = 0;
+    /* regk_reconcile (regk_reconcile.cuh): staged snapshot, tables, outputs, lists, the gathered request streams;
+       regk_reconcile_requests' frames */
+    enum { RC_IN_PB, RC_IN_PO, RC_IN_JB, RC_IN_JO, RC_TOBS, RC_TDES, RC_SLOTO, RC_HASHO, RC_SLOTD, RC_CLS, RC_MATCH, RC_OBSCLS,
+           RC_TOTALS, RC_LIST0, RC_LIST1, RC_LIST2, RC_LIST3, RC_LEN0, RC_LEN1, RC_LEN2, RC_LEN3, RC_LEN4, RC_COUNT, RC_GTOTALS,
+           RC_G0B, RC_G0O, RC_G1B, RC_G1O, RC_G2B, RC_G2O, RC_G3B, RC_G3O, RC_G4B, RC_G4O, RC_FBYTES, RC_FOFF, RC_NBUF };
+    DevBuf rc[RC_NBUF];
+    HostBuf h_rc_count, h_rc_cls, h_rc_match, h_rc_obscls, h_rc_list[4], h_rc_fbytes, h_rc_foff;
+    cudaEvent_t rc_ev[2] = {nullptr, nullptr};
+    bool rc_valid = false;                      /* the request streams of the last regk_reconcile call are in rc[RC_G*] */
+    uint64_t rc_count[4] = {0, 0, 0, 0};        /* create, update, dup, delete */
     std::vector<cudaEvent_t> pipe_events;
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     DevBuf skip_work, skip_in[11], skip_off_p, skip_off_j, skip_index, skip_bits;
@@ -911,6 +922,16 @@ void regk_destroy(regk_ctx *ctx)
     for (auto &ev : ctx->mk_ev)
         if (ev)
             cudaEventDestroy(ev);
+    for (auto &b : ctx->rc)
+        if (b.p)
+            cudaFree(b.p);
+    for (HostBuf *b : {&ctx->h_rc_count, &ctx->h_rc_cls, &ctx->h_rc_match, &ctx->h_rc_obscls, &ctx->h_rc_list[0], &ctx->h_rc_list[1],
+             &ctx->h_rc_list[2], &ctx->h_rc_list[3], &ctx->h_rc_fbytes, &ctx->h_rc_foff})
+        if (b->p)
+            cudaFreeHost(b->p);
+    for (auto &ev : ctx->rc_ev)
+        if (ev)
+            cudaEventDestroy(ev);
     for (auto &sl : ctx->slots)
         for (auto &ev : sl.ev)
             if (ev)
@@ -935,7 +956,7 @@ int regk_set_option(regk_ctx *ctx, const char *name, int64_t value)
     if (!ctx || !name)
         return REGK_ERR_INVALID_ARG;
     static const char *known[] = {"async", "force_generic", "dom_cap", "json_out_cap", "chunk_records", "time_every", "offsets32",
-                                  "mkdirp_tight_table", nullptr};
+                                  "mkdirp_tight_table", "reconcile_tight_table", nullptr};
     for (const char **k = known; *k; k++)
         if (!strcmp(*k, name)) {
             ctx->opt[name] = value;
@@ -2780,6 +2801,278 @@ int regk_mkdirp_requests(regk_ctx *ctx, int32_t xid_base, uint32_t zk_flags, uin
                  (const uint8_t *)ctx->mk[regk_ctx::MK_DBYTES].p, (const unsigned long long *)ctx->mk[regk_ctx::MK_ZERO].p};
     src.who = "regk_mkdirp_requests";
     return frame_requests(ctx, src, &o, ctx->mk[regk_ctx::MK_FBYTES], ctx->mk[regk_ctx::MK_FOFF], ctx->h_mk_fbytes, ctx->h_mk_foff, out);
+}
+
+int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk_delta *out)
+{
+    if (!ctx || !in || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: NULL argument");
+    memset(out, 0, sizeof *out);
+    ctx->rc_valid = false;
+    if (in->flags & REGK_DECODE_LAST)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams");
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_reconcile: batches are still in flight; finish them first");
+    if (!ctx->last_path_off || !ctx->last_json_off || ctx->last_n != ctx->last_json_n)
+        return fail(ctx, REGK_ERR_STATE, "regk_reconcile: no finished batch with both a path and a payload stream on this context "
+                                         "(an empty batch or a REGK_JOB_STEP result leaves none)");
+    const uint64_t n = ctx->last_n, m = in->n;
+    if (n >= 0xFFFFFFFFull || m >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: %llu records and %llu nodes: both must be below 2^32 - 1",
+            (unsigned long long)n, (unsigned long long)m);
+    const bool in_dev = in->flags & REGK_IN_DEVICE, dev_out = flags & REGK_OUT_DEVICE;
+    const uint8_t *pb = in->path_bytes, *jb = in->json_bytes;
+    const uint64_t *po = in->path_off, *jo = in->json_off;
+    uint64_t path_total = m ? in->path_total : 0, json_total = m ? in->json_total : 0;
+    if (m && (!po || !jo))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: a snapshot of %llu nodes needs path and data offsets", (unsigned long long)m);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    DevBuf *rb = ctx->rc;
+    int rc;
+    if (m && !in_dev) {
+        path_total = po[m];
+        json_total = jo[m];
+        /* offsets become memory ranges in the kernels: monotone, each node below 4 GiB, ending at the totals */
+        for (uint64_t j = 0; j < m; j++)
+            if (po[j] > po[j + 1] || jo[j] > jo[j + 1] || po[j + 1] - po[j] > 0xFFFFFFFFull || jo[j + 1] - jo[j] > 0xFFFFFFFFull)
+                return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot offsets are not monotone at node %llu",
+                    (unsigned long long)j);
+        if ((path_total && !pb) || (json_total && !jb))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot offsets without bytes");
+        const void *src[4] = {pb, po, jb, jo};
+        const size_t sz[4] = {(size_t)path_total, (size_t)(m + 1) * 8, (size_t)json_total, (size_t)(m + 1) * 8};
+        for (int k = 0; k < 4; k++) {
+            if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_IN_PB + k], sz[k] + 16)))
+                return rc;
+            if (sz[k])
+                CK(cudaMemcpyAsync(rb[regk_ctx::RC_IN_PB + k].p, src[k], sz[k], cudaMemcpyHostToDevice, s));
+        }
+        pb = (const uint8_t *)rb[regk_ctx::RC_IN_PB].p;
+        po = (const uint64_t *)rb[regk_ctx::RC_IN_PO].p;
+        jb = (const uint8_t *)rb[regk_ctx::RC_IN_JB].p;
+        jo = (const uint64_t *)rb[regk_ctx::RC_IN_JO].p;
+    } else if (m) {
+        if ((path_total && !pb) || (json_total && !jb))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot offsets without bytes");
+        if (((uintptr_t)pb & 3u) || ((uintptr_t)jb & 3u) || ((uintptr_t)po & 7u) || ((uintptr_t)jo & 7u))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: misaligned device snapshot (bytes need 4-byte, offsets 8-byte alignment)");
+    }
+    /* an empty stream is never read; its kernels still get a valid pointer */
+    if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_IN_PB], 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_IN_JB], 16)))
+        return rc;
+    if (!pb)
+        pb = (const uint8_t *)rb[regk_ctx::RC_IN_PB].p;
+    if (!jb)
+        jb = (const uint8_t *)rb[regk_ctx::RC_IN_JB].p;
+    /* the batch's totals */
+    unsigned long long tot[2] = {0, 0};
+    CK(cudaMemcpyAsync(&tot[0], ctx->last_path_off + n, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&tot[1], ctx->last_json_off + n, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    /* tables: at most half full; "reconcile_tight_table" = 1: the smallest power of two above the entries */
+    const bool tight = opt_get(ctx, "reconcile_tight_table", 0) != 0;
+    auto table_slots = [tight](uint64_t entries) {
+        uint64_t slots = tight ? 2 : 1024;
+        while (tight ? slots <= entries : slots < 2 * entries)
+            slots <<= 1;
+        return slots;
+    };
+    const uint64_t so = table_slots(m), sd = table_slots(n);
+    const uint64_t tiles_r = (n + RC_TILE - 1) / RC_TILE, tiles_o = (m + RC_TILE - 1) / RC_TILE;
+    const size_t ttr = align16(tiles_r * 4), str = (tiles_r / SUPER + 1) * 8, tto = align16(tiles_o * 4), sto = (tiles_o / SUPER + 1) * 8;
+    const size_t totals_bytes = 3 * (ttr + str) + tto + sto;
+    const size_t counters_bytes = RC_NCOUNTERS * 8;
+    if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_TOBS], so * 4)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_TDES], sd * 4)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RC_SLOTO], m * 4 + 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_HASHO], m * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RC_SLOTD], n * 4)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_CLS], n + 16)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RC_MATCH], n * 8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_OBSCLS], m + 16)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RC_TOTALS], totals_bytes)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_COUNT], counters_bytes)) ||
+        (rc = ensure_host(ctx, ctx->h_rc_count, counters_bytes)))
+        return rc;
+    for (int l = 0; l < RC_NLISTS; l++)
+        if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_LIST0 + l], (l == RC_LDELETE ? m : n) * 8 + 8)))
+            return rc;
+    for (int k = 0; k < 5; k++)
+        if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_LEN0 + k], (k == 4 ? m : n) * 4 + 8)))
+            return rc;
+    for (auto &ev : ctx->rc_ev)
+        if (!ev)
+            CK(cudaEventCreate(&ev));
+    ReconcileParams p{};
+    p.n = n;
+    p.m = m;
+    p.d_path = ctx->last_path_bytes;
+    p.d_path_off = ctx->last_path_off;
+    p.d_json = ctx->last_json_bytes;
+    p.d_json_off = ctx->last_json_off;
+    p.d_path_limit = tot[0] + 16;                   /* every stream buffer of this library has >= 16 bytes of slack */
+    p.d_json_limit = tot[1] + 16;
+    p.o_path = pb;
+    p.o_path_off = (const unsigned long long *)po;
+    p.o_json = jb;
+    p.o_json_off = (const unsigned long long *)jo;
+    p.o_path_total = path_total;                    /* a caller's device buffers end where they end */
+    p.o_json_total = json_total;
+    p.validate = in_dev ? 1u : 0u;
+    p.mask_o = (uint32_t)(so - 1);
+    p.mask_d = (uint32_t)(sd - 1);
+    p.t_obs = (uint32_t *)rb[regk_ctx::RC_TOBS].p;
+    p.t_des = (uint32_t *)rb[regk_ctx::RC_TDES].p;
+    p.slot_obs = (uint32_t *)rb[regk_ctx::RC_SLOTO].p;
+    p.hash_obs = (uint32_t *)rb[regk_ctx::RC_HASHO].p;
+    p.slot_des = (uint32_t *)rb[regk_ctx::RC_SLOTD].p;
+    p.cls = (uint8_t *)rb[regk_ctx::RC_CLS].p;
+    p.match = (unsigned long long *)rb[regk_ctx::RC_MATCH].p;
+    p.obs_cls = (uint8_t *)rb[regk_ctx::RC_OBSCLS].p;
+    uint8_t *tb = (uint8_t *)rb[regk_ctx::RC_TOTALS].p;
+    for (int l = 0; l < RC_NLISTS; l++) {
+        const bool del = l == RC_LDELETE;
+        p.tile_total[l] = (uint32_t *)(tb + (size_t)l * (ttr + str));
+        p.super_total[l] = (unsigned long long *)(tb + (size_t)l * (ttr + str) + (del ? tto : ttr));
+        p.list[l] = (unsigned long long *)rb[regk_ctx::RC_LIST0 + l].p;
+    }
+    for (int k = 0; k < 5; k++)
+        p.len[k] = (uint32_t *)rb[regk_ctx::RC_LEN0 + k].p;
+    p.counters = (unsigned long long *)rb[regk_ctx::RC_COUNT].p;
+    p.tiles_r = (uint32_t)tiles_r;
+    CK(cudaMemsetAsync(p.t_obs, 0, so * 4, s));
+    CK(cudaMemsetAsync(p.t_des, 0, sd * 4, s));
+    CK(cudaMemsetAsync(tb, 0, totals_bytes, s));
+    CK(cudaMemsetAsync(p.counters, 0, counters_bytes, s));
+    CK(cudaMemsetAsync(p.counters, 0xFF, 16, s));   /* no bad node, no duplicate node */
+    CK(cudaEventRecord(ctx->rc_ev[0], s));
+    uint32_t launches = 0;
+    if (m) {
+        regk_reconcile_insert_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(p);
+        launches++;
+    }
+    regk_reconcile_desired_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p);
+    regk_reconcile_mark_kernel<<<(unsigned)(tiles_r + tiles_o), RC_TILE, 0, s>>>(p);
+    regk_reconcile_compact_kernel<<<(unsigned)(tiles_r + tiles_o), RC_TILE, 0, s>>>(p);
+    CK(cudaGetLastError());
+    launches += 3;
+    unsigned long long *hc = (unsigned long long *)ctx->h_rc_count.p;
+    CK(cudaMemcpyAsync(hc, p.counters, counters_bytes, cudaMemcpyDeviceToHost, s));
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_CUDA, "regk_reconcile: kernel execution failed: %s", cudaGetErrorString(e));
+    if (hc[RC_C_BAD] != ~0ull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot offsets are not monotone or reach past the totals at node %llu",
+            hc[RC_C_BAD]);
+    if (hc[RC_C_DUPNODE] != ~0ull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot node %llu has the path of an earlier node; a registry cannot "
+                                               "hold two nodes with one path", hc[RC_C_DUPNODE]);
+    uint64_t cnt[RC_NLISTS];
+    for (int l = 0; l < RC_NLISTS; l++)
+        cnt[l] = hc[RC_C_COUNT + l];
+    if (n == 0)
+        cnt[RC_LCREATE] = cnt[RC_LUPDATE] = cnt[RC_LDUP] = 0;
+    if (m == 0)
+        cnt[RC_LDELETE] = 0;
+    /* the request sets, packed: create paths, create payloads, update paths, update payloads, delete paths */
+    const int g_list[5] = {RC_LCREATE, RC_LCREATE, RC_LUPDATE, RC_LUPDATE, RC_LDELETE};
+    const uint8_t *g_src[5] = {p.d_path, p.d_json, p.d_path, p.d_json, p.o_path};
+    const unsigned long long *g_off[5] = {p.d_path_off, p.d_json_off, p.d_path_off, p.d_json_off, p.o_path_off};
+    uint64_t gmax = 0;
+    for (int g = 0; g < 5; g++)
+        gmax = std::max<uint64_t>(gmax, cnt[g_list[g]]);
+    const uint64_t gt = (gmax + MK_TILE - 1) / MK_TILE;
+    if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_GTOTALS], gt * 8 + (gt / SUPER + 1) * 8 + 16)))
+        return rc;
+    for (int g = 0; g < 5; g++) {
+        const uint64_t c = cnt[g_list[g]], bytes = hc[RC_C_BYTES + g];
+        DevBuf &gb = rb[regk_ctx::RC_G0B + 2 * g], &go = rb[regk_ctx::RC_G0O + 2 * g];
+        if ((rc = ensure_dev(ctx, gb, bytes + 16)) || (rc = ensure_dev(ctx, go, (c + 1) * 8)))
+            return rc;
+        if (!c) {
+            CK(cudaMemsetAsync(go.p, 0, 8, s));
+            continue;
+        }
+        const uint64_t dt = (c + MK_TILE - 1) / MK_TILE;
+        MkGatherParams gp{};
+        gp.n_dirs = c;
+        gp.path_bytes = g_src[g];
+        gp.path_off = g_off[g];
+        gp.dir_rec = p.list[g_list[g]];
+        gp.dir_len = p.len[g];
+        gp.tile_total = (unsigned long long *)rb[regk_ctx::RC_GTOTALS].p;
+        gp.super_total = gp.tile_total + dt;
+        gp.dir_bytes = (uint8_t *)gb.p;
+        gp.dir_off = (unsigned long long *)go.p;
+        CK(cudaMemsetAsync(gp.super_total, 0, (dt / SUPER + 1) * 8, s));
+        regk_mkdirp_len_kernel<<<(unsigned)dt, MK_TILE, 0, s>>>(gp);
+        regk_mkdirp_gather_kernel<<<(unsigned)dt, MK_TILE, 0, s>>>(gp);
+        CK(cudaGetLastError());
+        launches += 2;
+    }
+    CK(cudaEventRecord(ctx->rc_ev[1], s));
+    e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_CUDA, "regk_reconcile: kernel execution failed: %s", cudaGetErrorString(e));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, ctx->rc_ev[0], ctx->rc_ev[1]);
+    const void *dsrc[7] = {p.cls, p.match, p.obs_cls, p.list[0], p.list[1], p.list[2], p.list[3]};
+    if (!dev_out) {
+        HostBuf *hb[7] = {&ctx->h_rc_cls, &ctx->h_rc_match, &ctx->h_rc_obscls, &ctx->h_rc_list[0], &ctx->h_rc_list[1],
+                          &ctx->h_rc_list[2], &ctx->h_rc_list[3]};
+        const size_t sz[7] = {n, n * 8, m, cnt[0] * 8, cnt[1] * 8, cnt[2] * 8, cnt[3] * 8};
+        for (int k = 0; k < 7; k++) {
+            if ((rc = ensure_host(ctx, *hb[k], sz[k] + 16)))
+                return rc;
+            if (sz[k])
+                CK(cudaMemcpyAsync(hb[k]->p, dsrc[k], sz[k], cudaMemcpyDeviceToHost, s));
+            dsrc[k] = hb[k]->p;
+        }
+        CK(cudaStreamSynchronize(s));
+    }
+    ctx->rc_valid = true;
+    for (int l = 0; l < RC_NLISTS; l++)
+        ctx->rc_count[l] = cnt[l];
+    out->n = n;
+    out->m = m;
+    out->n_create = cnt[RC_LCREATE];
+    out->n_update = cnt[RC_LUPDATE];
+    out->n_dup = cnt[RC_LDUP];
+    out->n_delete = cnt[RC_LDELETE];
+    out->n_same = n - out->n_create - out->n_update - out->n_dup;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->cls = (const uint8_t *)dsrc[0];
+    out->match = (const uint64_t *)dsrc[1];
+    out->obs_cls = (const uint8_t *)dsrc[2];
+    out->create = (const uint64_t *)dsrc[3];
+    out->update = (const uint64_t *)dsrc[4];
+    out->dup = (const uint64_t *)dsrc[5];
+    out->del = (const uint64_t *)dsrc[6];
+    out->kernel_ms = ms;
+    return REGK_OK;
+}
+
+int regk_reconcile_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
+{
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: NULL argument");
+    memset(out, 0, sizeof *out);
+    if (o->op != REGK_ZK_CREATE && o->op != REGK_ZK_DELETE && o->op != REGK_ZK_SETDATA)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: op %u is not create (1), delete (2) or setData (5)", o->op);
+    if (o->group > 65536)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: at most 65536 operations per multi transaction");
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_reconcile_requests: batches are still in flight; finish them first");
+    if (!ctx->rc_valid)
+        return fail(ctx, REGK_ERR_STATE, "regk_reconcile_requests: no reconcile result on this context; call regk_reconcile first");
+    CK(cudaSetDevice(ctx->device));
+    /* gathered streams: create paths / payloads (0, 1), update paths / payloads (2, 3), delete paths (4) */
+    const int g = o->op == REGK_ZK_CREATE ? 0 : o->op == REGK_ZK_SETDATA ? 2 : 4;
+    const uint64_t c = ctx->rc_count[o->op == REGK_ZK_CREATE ? RC_LCREATE : o->op == REGK_ZK_SETDATA ? RC_LUPDATE : RC_LDELETE];
+    DevBuf *rb = ctx->rc;
+    const bool data = g != 4;
+    FrameSrc src{c, (const uint8_t *)rb[regk_ctx::RC_G0B + 2 * g].p, (const unsigned long long *)rb[regk_ctx::RC_G0O + 2 * g].p,
+                 data ? (const uint8_t *)rb[regk_ctx::RC_G0B + 2 * g + 2].p : nullptr,
+                 data ? (const unsigned long long *)rb[regk_ctx::RC_G0O + 2 * g + 2].p : nullptr};
+    src.who = "regk_reconcile_requests";
+    return frame_requests(ctx, src, o, rb[regk_ctx::RC_FBYTES], rb[regk_ctx::RC_FOFF], ctx->h_rc_fbytes, ctx->h_rc_foff, out);
 }
 
 int regk_release(regk_ctx *ctx, regk_result *res)

@@ -1254,6 +1254,27 @@ RG_HD uint32_t string_word(const uint32_t *W, uint64_t o, uint32_t k)
     return funnel_r(W[b], W[b + 1], ((uint32_t)o & 3u) * 8u);
 }
 
+/* one 4-byte group into a running string hash, and the finaliser (murmur3) */
+RG_HD uint32_t hash32_step(uint32_t h, uint32_t w)
+{
+    w *= 0xCC9E2D51u;
+    w = (w << 15) | (w >> 17);
+    w *= 0x1B873593u;
+    h ^= w;
+    h = (h << 13) | (h >> 19);
+    return h * 5u + 0xE6546B64u;
+}
+
+RG_HD uint32_t hash32_final(uint32_t h)
+{
+    h ^= h >> 16;
+    h *= 0x85EBCA6Bu;
+    h ^= h >> 13;
+    h *= 0xC2B2AE35u;
+    h ^= h >> 16;
+    return h;
+}
+
 /* 32-bit hash of the n bytes at byte offset o (murmur3 mixing, word-wise; only picks a table slot) */
 RG_HD uint32_t string_hash32(const uint32_t *W, uint64_t o, uint32_t n)
 {
@@ -1263,19 +1284,9 @@ RG_HD uint32_t string_hash32(const uint32_t *W, uint64_t o, uint32_t n)
         uint32_t w = string_word(W, o, k);
         if (k == nw)
             w &= low_bytes(rem);
-        w *= 0xCC9E2D51u;
-        w = (w << 15) | (w >> 17);
-        w *= 0x1B873593u;
-        h ^= w;
-        h = (h << 13) | (h >> 19);
-        h = h * 5u + 0xE6546B64u;
+        h = hash32_step(h, w);
     }
-    h ^= h >> 16;
-    h *= 0x85EBCA6Bu;
-    h ^= h >> 13;
-    h *= 0xC2B2AE35u;
-    h ^= h >> 16;
-    return h;
+    return hash32_final(h);
 }
 
 /* do the n bytes at byte offsets a and b of W agree? */
@@ -1287,6 +1298,54 @@ RG_HD bool string_equal(const uint32_t *W, uint64_t a, uint64_t b, uint32_t n)
             return false;
     if (rem)
         return ((string_word(W, a, nw) ^ string_word(W, b, nw)) & low_bytes(rem)) == 0u;
+    return true;
+}
+
+/* ---- the same on a buffer with no slack behind it (a caller's device stream ends where it ends) ---- */
+
+/* word b of W, where only bytes [0, limit) of the buffer may be read: bytes at or past `limit` read as 0 */
+RG_HD uint32_t word_clamped(const uint32_t *W, uint64_t b, uint64_t limit)
+{
+    const uint64_t byte0 = b << 2;
+    if (byte0 + 4u <= limit)
+        return W[b];
+    const uint8_t *B = reinterpret_cast<const uint8_t *>(W);
+    uint32_t v = 0;
+    for (uint32_t i = 0; i < 4u && byte0 + i < limit; i++)
+        v |= (uint32_t)B[byte0 + i] << (8u * i);
+    return v;
+}
+
+/* string_word with every read below `limit`: equal to string_word for the bytes of a string that ends by `limit` */
+RG_HD uint32_t string_word_clamped(const uint32_t *W, uint64_t o, uint32_t k, uint64_t limit)
+{
+    const uint64_t b = (o >> 2) + k;
+    return funnel_r(word_clamped(W, b, limit), word_clamped(W, b + 1u, limit), ((uint32_t)o & 3u) * 8u);
+}
+
+/* string_hash32 of the n bytes at o of a buffer readable below `limit`: the same value for the same bytes */
+RG_HD uint32_t string_hash32_clamped(const uint32_t *W, uint64_t o, uint32_t n, uint64_t limit)
+{
+    uint32_t h = 0x9747B28Cu ^ n;
+    const uint32_t nw = n >> 2, rem = n & 3u;
+    for (uint32_t k = 0; k < nw + (rem ? 1u : 0u); k++) {
+        uint32_t w = string_word_clamped(W, o, k, limit);
+        if (k == nw)
+            w &= low_bytes(rem);
+        h = hash32_step(h, w);
+    }
+    return hash32_final(h);
+}
+
+/* do the n bytes at a of buffer A (readable below la) and at b of buffer B (readable below lb) agree? */
+RG_HD bool string_equal2(const uint32_t *A, uint64_t a, uint64_t la, const uint32_t *B, uint64_t b, uint64_t lb, uint32_t n)
+{
+    const uint32_t nw = n >> 2, rem = n & 3u;
+    for (uint32_t k = 0; k < nw; k++)
+        if (string_word_clamped(A, a, k, la) != string_word_clamped(B, b, k, lb))
+            return false;
+    if (rem)
+        return ((string_word_clamped(A, a, nw, la) ^ string_word_clamped(B, b, nw, lb)) & low_bytes(rem)) == 0u;
     return true;
 }
 
