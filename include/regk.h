@@ -514,7 +514,7 @@ int         regk_decode(regk_ctx *ctx, const regk_decode_in *in, regk_decode_out
  * The snapshot must cover exactly the namespace the batch owns: every node it holds that the batch does not produce -
  * directories included - is classed DELETE.
  * Nodes are keyed by their path bytes, compared byte for byte (a hash only picks a table slot); the class depends on
- * bytes alone (no ephemeral owners, no versions).  Record i:
+ * bytes alone (no ephemeral owners, no versions) - regk_reconcile_owned below also weighs each node's Stat.  Record i:
  *   REGK_DELTA_DUP     an earlier record of the batch has the same path (the first occurrence decides); no request
  *   REGK_DELTA_CREATE  no node has path i
  *   REGK_DELTA_UPDATE  the node with path i holds data that differs from payload i in length or in a byte
@@ -557,9 +557,63 @@ int         regk_reconcile(regk_ctx *ctx, const regk_decode_in *snapshot, uint32
  *   REGK_ZK_SETDATA  the update list: SetDataRequest{path i, payload i, version}
  *   REGK_ZK_DELETE   the delete list: DeleteRequest{snapshot path j, version}
  * Send them in this order: delete, then the creates' parents (regk_mkdirp_dirs / regk_mkdirp_requests), then create,
- * then setData.  flags: REGK_OUT_DEVICE returns device pointers, else pinned host arrays; valid until the next call.
+ * then setData, then (after regk_reconcile_owned) replace.  flags: REGK_OUT_DEVICE returns device pointers, else pinned
+ * host arrays; valid until the next call.  The frames come from whichever of regk_reconcile / regk_reconcile_owned last
+ * succeeded.  After regk_reconcile_owned two more options exist:
+ *   REGK_ZK_REPLACE           (op) the replace list: frame q is one multi transaction (group = 0 counts as 1; at most
+ *                             32768 entries, i.e. 65536 operations) - len | xid_base + q | 14 | for each entry (record i):
+ *                             MultiHeader{2, false, -1} DeleteRequest{path i, version} MultiHeader{1, false, -1}
+ *                             CreateRequest{path i, payload i, [OPEN_ACL_UNSAFE], zk_flags} | MultiHeader{-1, true, -1}.
+ *                             Entry r is 65 + 2 P + J bytes, a frame 21 more.  The node is never missing: ZooKeeper applies
+ *                             the delete and the create together or neither.
+ *   REGK_ZK_VERSION_OBSERVED  (flags) every delete, setData and the delete of a replace carries the Stat.version its
+ *                             node had in the snapshot instead of opts->version: the write fails with BADVERSION if the
+ *                             node changed since.  Not with REGK_ZK_CREATE (REGK_ERR_INVALID_ARG).
+ * Both are REGK_ERR_STATE after a plain regk_reconcile.  After regk_reconcile_owned, REGK_ZK_CREATE and REGK_ZK_REPLACE
+ * require opts->zk_flags == the zk_flags the reconcile classified with (REGK_ERR_INVALID_ARG otherwise): a node created
+ * in another mode would be classed REPLACE again by the next reconcile, and the repair would never converge.
  */
+#define REGK_ZK_REPLACE          256u       /* regk_jute_opts.op: not a ZooKeeper OpCode */
+#define REGK_ZK_VERSION_OBSERVED (1u << 9)  /* regk_jute_opts.flags */
+
 int         regk_reconcile_requests(regk_ctx *ctx, const regk_jute_opts *opts, regk_frames *out);
+
+/*
+ * ---- reconcile against node stats: ephemeral owners and versions (the reference re-registers after a session loss by
+ * unlinking every node, waiting 1 s and creating it again, lib/register.js:85-95, :228-239) ----------------------------
+ * As regk_reconcile, with the Stat of every snapshot node, as the caller's client read it (getData / exists replies):
+ * version[j] = Stat.version, ephemeral_owner[j] = Stat.ephemeralOwner (0 = persistent).  The arrays live where the
+ * snapshot's streams do (device arrays with REGK_IN_DEVICE: version 4-byte, ephemeral_owner 8-byte aligned).
+ * want = session when zk_flags == 1 (EPHEMERAL), else 0.  Record i is REGK_DELTA_REPLACE when it is the first record
+ * with its path, node j has that path and ephemeral_owner[j] != want - a stale ephemeral of an earlier session (which
+ * the server would delete when that session expires), another session's ephemeral, or a persistent node where an
+ * ephemeral is wanted (and the reverse).  The payload is not compared then.  Every other class is as in regk_reconcile;
+ * the node of a REPLACE record is KEEP (its delete travels inside the replace frame).
+ * n_same + n_create + n_update + n_dup + n_replace == n.
+ * Edge: a persistent node that has children, where an ephemeral is wanted, is REPLACE too; ZooKeeper then aborts the
+ * multi with NOTEMPTY, as the reference's unlink fails there.  An ephemeral node has no children, so the reverse cannot.
+ * Refused besides regk_reconcile's refusals (REGK_ERR_INVALID_ARG): stat NULL, an array NULL while m > 0, misaligned
+ * device arrays, zk_flags other than 0 or 1 (a sequential or container mode makes a path key meaningless), zk_flags == 1
+ * with session == 0.  The delta's arrays are valid until the next regk_reconcile / regk_reconcile_owned call.
+ */
+typedef struct regk_node_stat {
+    const int32_t *version;         /* [m] Stat.version of snapshot node j (passed through verbatim) */
+    const int64_t *ephemeral_owner; /* [m] Stat.ephemeralOwner of node j; 0 = persistent */
+    int64_t  session;               /* session id the repair will be sent on */
+    uint32_t zk_flags;              /* CreateMode of the batch's nodes: 1 = EPHEMERAL, 0 = persistent; nothing else */
+    uint32_t reserved;
+} regk_node_stat;
+
+#define REGK_DELTA_REPLACE 4u       /* cls[]: only regk_reconcile_owned produces it */
+
+typedef struct regk_delta_owned {
+    regk_delta d;                   /* filled as regk_reconcile fills it; cls[] may hold REGK_DELTA_REPLACE */
+    uint64_t n_replace;
+    const uint64_t *replace;        /* [n_replace] ascending record indices */
+} regk_delta_owned;
+
+int         regk_reconcile_owned(regk_ctx *ctx, const regk_decode_in *snapshot, const regk_node_stat *stat,
+                                 uint32_t flags, regk_delta_owned *out);
 
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);

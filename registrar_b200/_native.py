@@ -95,6 +95,8 @@ class CJuteOpts(C.Structure):        # regk_jute_opts
 
 
 ZK_CREATE, ZK_DELETE, ZK_SETDATA = 1, 2, 5
+ZK_REPLACE = 256                    # reconcile_requests after reconcile_owned: delete + create in one multi transaction
+FLAG_ZK_VERSION_OBSERVED = 1 << 9   # regk_jute_opts.flags: each frame carries its node's Stat.version
 
 
 class CDecodeIn(C.Structure):        # regk_decode_in
@@ -173,6 +175,7 @@ class CDelta(C.Structure):           # regk_delta
 
 
 DELTA_SAME, DELTA_CREATE, DELTA_UPDATE, DELTA_DUP = 0, 1, 2, 3       # Delta.cls
+DELTA_REPLACE = 4                                                    # Delta.cls, reconcile_owned only
 DELTA_KEEP, DELTA_DELETE = 0, 1                                      # Delta.obs_cls
 
 
@@ -180,9 +183,10 @@ class Delta:
     """Host copy of a regk_delta: how the batch finished last differs from a snapshot of the registry.  cls[i] is
     DELTA_SAME / _CREATE / _UPDATE / _DUP for record i, match[i] the snapshot node with its path (UINT64_MAX: none),
     obs_cls[j] DELTA_KEEP / _DELETE for node j; create / update / dup are ascending record indices, delete ascending
-    snapshot indices."""
+    snapshot indices.  From reconcile_owned, cls may also hold DELTA_REPLACE and `replace` lists those records
+    (ascending); a plain reconcile reports n_replace == 0."""
 
-    def __init__(self, out):
+    def __init__(self, out, replace=None, n_replace=0):
         n, m = int(out.n), int(out.m)
         self.n, self.m, self.launches, self.kernel_ms = n, m, int(out.launches), float(out.kernel_ms)
         self.n_same, self.n_create, self.n_update = int(out.n_same), int(out.n_create), int(out.n_update)
@@ -194,6 +198,17 @@ class Delta:
         self.update = _as_np(out.update, self.n_update, np.uint64).copy()
         self.dup = _as_np(out.dup, self.n_dup, np.uint64).copy()
         self.delete = _as_np(out.del_, self.n_delete, np.uint64).copy()
+        self.n_replace = int(n_replace)
+        self.replace = _as_np(replace, self.n_replace, np.uint64).copy()
+
+
+class CNodeStat(C.Structure):        # regk_node_stat
+    _fields_ = [("version", C.c_void_p), ("ephemeral_owner", C.c_void_p), ("session", C.c_int64),
+                ("zk_flags", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class CDeltaOwned(C.Structure):      # regk_delta_owned
+    _fields_ = [("d", CDelta), ("n_replace", C.c_uint64), ("replace", C.c_void_p)]
 
 
 class CSkipped(C.Structure):         # regk_skipped
@@ -207,7 +222,7 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_sync", "regk_set_option", "regk_get_option", "regk_ipc_export", "regk_ipc_open", "regk_ipc_close",
            "regk_gather_push", "regk_parent_dirs", "regk_job_bind", "regk_service_records",
            "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records", "regk_mkdirp_dirs",
-           "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests"]
+           "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned"]
 
 _lib = None
 
@@ -263,6 +278,7 @@ def load_library():
     lib.regk_mkdirp_requests.argtypes = [vp, C.c_int32, u32, u32, C.POINTER(CFrames)]
     lib.regk_reconcile.argtypes = [vp, C.POINTER(CDecodeIn), u32, C.POINTER(CDelta)]
     lib.regk_reconcile_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
+    lib.regk_reconcile_owned.argtypes = [vp, C.POINTER(CDecodeIn), C.POINTER(CNodeStat), u32, C.POINTER(CDeltaOwned)]
     _lib = lib
     return lib
 
@@ -605,13 +621,30 @@ class Context:
         self._check(rc)
         return out if device else Delta(out)
 
+    def reconcile_owned(self, snapshot, session: int, zk_flags: int = 1, device: bool = False):
+        """regk_reconcile_owned: reconcile() that also weighs each node's Stat - `snapshot` must carry `version` and
+        `owner` (Stat.version / Stat.ephemeralOwner per node).  A matched node whose owner is not `session` (zk_flags 1,
+        EPHEMERAL) or not 0 (zk_flags 0, persistent) makes its record DELTA_REPLACE.  Returns a Delta with `replace`,
+        or the raw CDeltaOwned (device pointers) with device=True."""
+        cin, keep = snapshot.cdecode_in()
+        st, skeep = snapshot.cnode_stat(int(session), int(zk_flags))
+        out = CDeltaOwned()
+        rc = self._lib.regk_reconcile_owned(self._h, C.byref(cin), C.byref(st), FLAG_OUT_DEVICE if device else 0,
+                                            C.byref(out))
+        del keep, skeep
+        self._check(rc)
+        return out if device else Delta(out.d, out.replace, out.n_replace)
+
     def reconcile_requests(self, op: int = ZK_CREATE, xid_base: int = 1, zk_flags: int = 1, version: int = -1,
-                           group: int = 0, device: bool = False):
+                           group: int = 0, device: bool = False, observed_version: bool = False):
         """regk_reconcile_requests: the create (ZK_CREATE), setData (ZK_SETDATA) or delete (ZK_DELETE) requests of the
-        last reconcile(), framed as jute_requests() frames a batch.  Returns (frame_bytes, frame_off, kernel_ms), or
-        the raw CFrames with device=True."""
+        last reconcile(), framed as jute_requests() frames a batch; after reconcile_owned() also the replace multi
+        transactions (ZK_REPLACE, group 0 counts as 1), and observed_version=True puts each node's snapshot version
+        into its delete / setData / replace frame instead of `version`.  Returns (frame_bytes, frame_off, kernel_ms),
+        or the raw CFrames with device=True."""
         xid = (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31
-        o = CJuteOpts(int(op), FLAG_OUT_DEVICE if device else 0, xid, int(zk_flags), int(version), int(group))
+        flags = (FLAG_OUT_DEVICE if device else 0) | (FLAG_ZK_VERSION_OBSERVED if observed_version else 0)
+        o = CJuteOpts(int(op), flags, xid, int(zk_flags), int(version), int(group))
         out = CFrames()
         self._check(self._lib.regk_reconcile_requests(self._h, C.byref(o), C.byref(out)))
         if device:

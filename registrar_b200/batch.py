@@ -240,16 +240,27 @@ class Snapshot:
     """What a registry holds under the namespace a batch owns: m nodes, node j = (path j, data j), as u64 CSR streams
     (the layout regk_decode accepts).  Either all four arrays are host NumPy arrays (uint8 bytes, uint64 offsets) or
     all four are CUDA tensors (uint8 bytes, int64 offsets); a device snapshot's streams end at the byte tensors' ends.
-    Input of Context.reconcile()."""
+    `version` / `owner` are each node's Stat.version (int32) and Stat.ephemeralOwner (int64, 0 = persistent), as the
+    caller's client read them, on the same side as the streams; Context.reconcile_owned() needs them,
+    Context.reconcile() ignores them.  Input of Context.reconcile() and Context.reconcile_owned()."""
     path_bytes: object
     path_off: object
     json_bytes: object
     json_off: object
+    version: object = None
+    owner: object = None
 
     @classmethod
     def from_nodes(cls, nodes: Iterable) -> "Snapshot":
-        """[(path, data), ...] -> host Snapshot"""
+        """[(path, data), ...] or [(path, data, version, owner), ...] -> host Snapshot"""
         nodes = list(nodes)
+        stats = None
+        arity = {len(x) for x in nodes}
+        if len(arity) > 1 or not arity <= {2, 4}:
+            raise ValueError("from_nodes takes (path, data) items or (path, data, version, owner) items, not a mix")
+        if arity == {4}:
+            stats = (np.array([x[2] for x in nodes], np.int32), np.array([x[3] for x in nodes], np.int64))
+            nodes = [(x[0], x[1]) for x in nodes]
 
         def pack(strings):
             off = np.zeros(len(strings) + 1, np.uint64)
@@ -258,7 +269,7 @@ class Snapshot:
             return np.frombuffer(b"".join(strings), np.uint8).copy(), off
         pb, po = pack([_b(p) for p, _ in nodes])
         jb, jo = pack([_b(d) for _, d in nodes])
-        return cls(pb, po, jb, jo)
+        return cls(pb, po, jb, jo) if stats is None else cls(pb, po, jb, jo, stats[0], stats[1])
 
     @property
     def device(self) -> bool:
@@ -286,6 +297,36 @@ class Snapshot:
         p = [a.ctypes.data_as(C.c_void_p) for a in keep]
         cin = CDecodeIn(n=len(keep[1]) - 1, flags=0, path_bytes=p[0], path_off=p[1], json_bytes=p[2], json_off=p[3])
         return cin, keep
+
+    def cnode_stat(self, session: int, zk_flags: int):
+        """regk_node_stat over `version` / `owner`.  Returns (struct, keepalive)."""
+        from ._native import CNodeStat
+        import ctypes as C
+        if self.version is None or self.owner is None:
+            raise ValueError("reconcile_owned needs the snapshot's version and owner arrays")
+        m = self.m
+        if self.device:
+            import torch
+            keep = [self.version, self.owner]
+            if not all(a.is_cuda and a.is_contiguous() for a in keep):
+                raise ValueError("a device snapshot's version and owner are contiguous CUDA tensors")
+            if self.version.dtype != torch.int32 or self.owner.dtype != torch.int64:
+                raise ValueError("a device snapshot's version is int32 and its owner int64, not %s / %s"
+                                 % (self.version.dtype, self.owner.dtype))
+            lens = (self.version.numel(), self.owner.numel())
+            ptr = [a.data_ptr() or None for a in keep]
+        else:
+            keep = [np.asarray(self.version), np.asarray(self.owner)]
+            if not all(a.dtype.kind in "iu" for a in keep):
+                raise ValueError("version and owner are integer arrays")
+            if (keep[0] != keep[0].astype(np.int32)).any() or (keep[1] != keep[1].astype(np.int64)).any():
+                raise ValueError("a version outside int32 or an owner outside int64")
+            keep = [np.ascontiguousarray(keep[0], np.int32), np.ascontiguousarray(keep[1], np.int64)]
+            lens = (keep[0].size, keep[1].size)
+            ptr = [a.ctypes.data_as(C.c_void_p) for a in keep]
+        if lens != (m, m):
+            raise ValueError("the snapshot has %d nodes but %d versions and %d owners" % (m, lens[0], lens[1]))
+        return CNodeStat(version=ptr[0], ephemeral_owner=ptr[1], session=session, zk_flags=zk_flags), keep
 
 
 SERVICE_KEYS = ("srvce", "proto", "port", "ttl")      # key ids 0..3 of regk_service_batch.key_order

@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <string>
@@ -123,16 +124,18 @@ struct regk_ctx {
     cudaEvent_t mk_ev[4] = {nullptr, nullptr, nullptr, nullptr};
     bool mk_valid = false;                      /* the set of the last regk_mkdirp_dirs call is in mk[MK_D*] */
     uint64_t mk_n_dirs = 0, mk_bytes = 0;
-    /* regk_reconcile (regk_reconcile.cuh): staged snapshot, tables, outputs, lists, the gathered request streams;
-       regk_reconcile_requests' frames */
-    enum { RC_IN_PB, RC_IN_PO, RC_IN_JB, RC_IN_JO, RC_TOBS, RC_TDES, RC_SLOTO, RC_HASHO, RC_SLOTD, RC_CLS, RC_MATCH, RC_OBSCLS,
-           RC_TOTALS, RC_LIST0, RC_LIST1, RC_LIST2, RC_LIST3, RC_LEN0, RC_LEN1, RC_LEN2, RC_LEN3, RC_LEN4, RC_COUNT, RC_GTOTALS,
-           RC_G0B, RC_G0O, RC_G1B, RC_G1O, RC_G2B, RC_G2O, RC_G3B, RC_G3O, RC_G4B, RC_G4O, RC_FBYTES, RC_FOFF, RC_NBUF };
+    /* regk_reconcile / regk_reconcile_owned (regk_reconcile.cuh): staged snapshot and stats, tables, outputs, lists,
+       versions, the gathered request streams; regk_reconcile_requests' frames */
+    enum { RC_IN_PB, RC_IN_PO, RC_IN_JB, RC_IN_JO, RC_IN_VER, RC_IN_OWN, RC_TOBS, RC_TDES, RC_SLOTO, RC_HASHO, RC_SLOTD, RC_CLS,
+           RC_MATCH, RC_OBSCLS, RC_TOTALS, RC_LIST0, RC_LEN0 = RC_LIST0 + RC_NLISTS, RC_VER0 = RC_LEN0 + RC_NGATHERS,
+           RC_COUNT = RC_VER0 + RC_NVER, RC_GTOTALS, RC_G0B, RC_FBYTES = RC_G0B + 2 * RC_NGATHERS, RC_FOFF, RC_NBUF };
     DevBuf rc[RC_NBUF];
-    HostBuf h_rc_count, h_rc_cls, h_rc_match, h_rc_obscls, h_rc_list[4], h_rc_fbytes, h_rc_foff;
+    HostBuf h_rc_count, h_rc_cls, h_rc_match, h_rc_obscls, h_rc_list[RC_NLISTS], h_rc_fbytes, h_rc_foff;
     cudaEvent_t rc_ev[2] = {nullptr, nullptr};
-    bool rc_valid = false;                      /* the request streams of the last regk_reconcile call are in rc[RC_G*] */
-    uint64_t rc_count[4] = {0, 0, 0, 0};        /* create, update, dup, delete */
+    bool rc_valid = false;                      /* the request streams of the last reconcile call are in rc[RC_G0B + 2 k] */
+    bool rc_owned = false;                      /* ... and it was regk_reconcile_owned: versions in rc[RC_VER*] */
+    uint32_t rc_zk_flags = 0;                   /* the CreateMode regk_reconcile_owned classified with */
+    uint64_t rc_count[RC_NLISTS] = {};          /* create, update, dup, replace, delete */
     std::vector<cudaEvent_t> pipe_events;
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     DevBuf skip_work, skip_in[11], skip_off_p, skip_off_j, skip_index, skip_bits;
@@ -620,13 +623,28 @@ struct FrameSrc {
     const char *who = "regk_jute_requests";
 };
 
-static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts *o, DevBuf &db, DevBuf &doff, HostBuf &hb,
-    HostBuf &hoff, regk_frames *out)
+/* What the framing driver hands a framing kernel: the streams' extents, the output buffers, the staging budgets. */
+struct FrameGeom {
+    uint64_t n, total;
+    uint8_t *out_bytes;
+    unsigned long long *out_off;
+    DevStatus *status;
+    uint32_t path_cap, json_cap;
+    uint64_t path_limit, json_limit;
+    size_t smem;
+};
+
+/* The driver both framing kernels share: read the streams' totals, size and fill the buffers, launch (`launch` fills the
+   kernel's own parameters from the geometry), check the status, copy the frames out.  Frames are multi transactions of
+   `group` entries when `multi`, else one request per entry; every entry carries `per_rec` framing bytes, emits its path
+   `path_times` times, and a tile's framing slots take `slot_bytes` of shared memory. */
+static int frame_drive(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts *o, bool multi, uint64_t group, uint32_t per_rec,
+    uint32_t path_times, size_t slot_bytes, DevBuf &db, DevBuf &doff, HostBuf &hb, HostBuf &hoff, regk_frames *out,
+    const std::function<cudaError_t(const FrameGeom &)> &launch)
 {
     const uint64_t n = src.n;
     const bool has_data = src.json_off != nullptr;
-    const bool multi = o->group != 0;
-    const uint64_t g = multi ? o->group : 1, frames = (n + g - 1) / g;
+    const uint64_t frames = (n + group - 1) / group;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     const bool dev_out = o->flags & REGK_OUT_DEVICE;
@@ -638,30 +656,7 @@ static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_op
     if (has_data)
         CK(cudaMemcpyAsync(&tot[1], src.json_off + n, 8, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    JuteParams p{};
-    p.n = n;
-    p.op = o->op;
-    p.mid = has_data ? 4u : 0u;
-    p.group = (uint32_t)g;
-    p.multi = multi ? 1u : 0u;
-    /* what follows the data: create - acl vector [OPEN_ACL_UNSAFE] + flags; delete / setData - the expected version */
-    uint8_t tail[48] = {0};
-    if (o->op == REGK_ZK_CREATE) {
-        static const uint8_t acl[27] = {0, 0, 0, 1, 0, 0, 0, 31, 0, 0, 0, 5, 'w', 'o', 'r', 'l', 'd', 0, 0, 0, 6, 'a', 'n', 'y', 'o', 'n', 'e'};
-        memcpy(tail, acl, 27);
-        for (int k = 0; k < 4; k++)
-            tail[27 + k] = (uint8_t)(o->zk_flags >> (24 - 8 * k));
-        p.tail_len = 31;
-    } else {
-        for (int k = 0; k < 4; k++)
-            tail[k] = (uint8_t)((uint32_t)o->version >> (24 - 8 * k));
-        p.tail_len = 4;
-    }
-    static const uint8_t multi_end[9] = {0xFF, 0xFF, 0xFF, 0xFF, 1, 0xFF, 0xFF, 0xFF, 0xFF};   /* MultiHeader {type -1, done, err -1} */
-    memcpy(tail + p.tail_len, multi_end, 9);
-    memcpy(p.tail, tail, sizeof p.tail);
-    p.per_rec = (multi ? JUTE_MULTI_HEAD : 0u) + 4u + p.mid + p.tail_len;
-    const uint64_t total = tot[0] + tot[1] + (uint64_t)p.per_rec * n + (uint64_t)JUTE_FRAME_HEAD * frames +
+    const uint64_t total = path_times * tot[0] + tot[1] + (uint64_t)per_rec * n + (uint64_t)JUTE_FRAME_HEAD * frames +
         (multi ? (uint64_t)JUTE_MULTI_HEAD * frames : 0);
     int rc;
     if ((rc = ensure_dev(ctx, db, total + 32)) || (rc = ensure_dev(ctx, doff, (frames + 1) * 8)))
@@ -673,27 +668,23 @@ static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_op
         CK(cudaMemsetAsync(doff.p, 0, 8, s));
     cudaEvent_t e0 = ctx->slots[0].ev[0], e1 = ctx->slots[0].ev[1];
     if (n) {
-        p.path_bytes = src.path_bytes;
-        p.path_off = src.path_off;
-        p.json_bytes = src.json_bytes;
-        p.json_off = src.json_off;
-        p.out_bytes = (uint8_t *)db.p;
-        p.out_off = (unsigned long long *)doff.p;
-        p.out_capacity = total;
-        p.xid_base = o->xid_base;
-        p.status = (DevStatus *)ctx->svc_work.p;
+        FrameGeom g{};
+        g.n = n;
+        g.total = total;
+        g.out_bytes = (uint8_t *)db.p;
+        g.out_off = (unsigned long long *)doff.p;
+        g.status = (DevStatus *)ctx->svc_work.p;
         /* staging budgets: 9/8 of a tile's mean share of each stream plus slack (tiles beyond it go byte-wise) */
-        p.path_cap = (uint32_t)align16(std::min<uint64_t>(tot[0] * JUTE_TILE / n * 9 / 8 + 1024, 65520));
-        p.json_cap = has_data ? (uint32_t)align16(std::min<uint64_t>(tot[1] * JUTE_TILE / n * 9 / 8 + 1024, 65520)) : 0u;  /* lengths travel as 16 bits */
-        p.path_limit = tot[0] + 16;                 /* every stream buffer of this library has >= 16 bytes of slack */
-        p.json_limit = has_data ? tot[1] + 16 : 0;
+        g.path_cap = (uint32_t)align16(std::min<uint64_t>(tot[0] * JUTE_TILE / n * 9 / 8 + 1024, 65520));
+        g.json_cap = has_data ? (uint32_t)align16(std::min<uint64_t>(tot[1] * JUTE_TILE / n * 9 / 8 + 1024, 65520)) : 0u;  /* lengths travel as 16 bits */
+        g.path_limit = tot[0] + 16;                 /* every stream buffer of this library has >= 16 bytes of slack */
+        g.json_limit = has_data ? tot[1] + 16 : 0;
         /* ... + one owner byte and one list entry per 16-byte output block of a tile that fits the staging budgets */
-        const uint32_t max_fixed = p.per_rec + JUTE_FRAME_HEAD + JUTE_MULTI_HEAD;
-        const size_t owner_bytes = 3 * ((p.path_cap + p.json_cap + max_fixed * JUTE_TILE) / 16 + 32);   /* owner u8 + list u16 per block */
-        const size_t smem = 34 * 16 + 16 + JUTE_TILE * JUTE_SLOT + 16 + 48 + 16 + (size_t)p.path_cap + 16 + p.json_cap + 48 + owner_bytes;
+        const uint32_t max_fixed = per_rec + JUTE_FRAME_HEAD + JUTE_MULTI_HEAD;
+        const size_t owner_bytes = 3 * ((path_times * g.path_cap + g.json_cap + max_fixed * JUTE_TILE) / 16 + 32);   /* owner u8 + list u16 per block */
+        g.smem = 34 * 16 + 16 + slot_bytes + 16 + (size_t)g.path_cap + 16 + g.json_cap + 48 + owner_bytes;
         CK(cudaEventRecord(e0, s));
-        CK(multi ? (has_data ? launch_jute<true, true>(p, smem, ctx->device, s) : launch_jute<true, false>(p, smem, ctx->device, s))
-                 : (has_data ? launch_jute<false, true>(p, smem, ctx->device, s) : launch_jute<false, false>(p, smem, ctx->device, s)));
+        CK(launch(g));
         CK(cudaEventRecord(e1, s));
         out->launches = 1;
     }
@@ -720,6 +711,119 @@ static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_op
     out->frame_bytes = (const uint8_t *)hb.p;
     out->frame_off = (const uint64_t *)hoff.p;
     return REGK_OK;
+}
+
+static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts *o, DevBuf &db, DevBuf &doff, HostBuf &hb,
+    HostBuf &hoff, regk_frames *out)
+{
+    const bool has_data = src.json_off != nullptr;
+    const bool multi = o->group != 0;
+    const uint64_t g = multi ? o->group : 1;
+    JuteParams p{};
+    p.n = src.n;
+    p.op = o->op;
+    p.mid = has_data ? 4u : 0u;
+    p.group = (uint32_t)g;
+    p.multi = multi ? 1u : 0u;
+    /* what follows the data: create - acl vector [OPEN_ACL_UNSAFE] + flags; delete / setData - the expected version */
+    uint8_t tail[48] = {0};
+    if (o->op == REGK_ZK_CREATE) {
+        static const uint8_t acl[27] = {0, 0, 0, 1, 0, 0, 0, 31, 0, 0, 0, 5, 'w', 'o', 'r', 'l', 'd', 0, 0, 0, 6, 'a', 'n', 'y', 'o', 'n', 'e'};
+        memcpy(tail, acl, 27);
+        for (int k = 0; k < 4; k++)
+            tail[27 + k] = (uint8_t)(o->zk_flags >> (24 - 8 * k));
+        p.tail_len = 31;
+    } else {
+        for (int k = 0; k < 4; k++)
+            tail[k] = (uint8_t)((uint32_t)o->version >> (24 - 8 * k));
+        p.tail_len = 4;
+    }
+    static const uint8_t multi_end[9] = {0xFF, 0xFF, 0xFF, 0xFF, 1, 0xFF, 0xFF, 0xFF, 0xFF};   /* MultiHeader {type -1, done, err -1} */
+    memcpy(tail + p.tail_len, multi_end, 9);
+    memcpy(p.tail, tail, sizeof p.tail);
+    p.per_rec = (multi ? JUTE_MULTI_HEAD : 0u) + 4u + p.mid + p.tail_len;
+    p.path_bytes = src.path_bytes;
+    p.path_off = src.path_off;
+    p.json_bytes = src.json_bytes;
+    p.json_off = src.json_off;
+    p.xid_base = o->xid_base;
+    /* framing slots, 16 bytes of slack, the constant tail */
+    const size_t slot_bytes = JUTE_TILE * JUTE_SLOT + 16 + 48;
+    return frame_drive(ctx, src, o, multi, g, p.per_rec, 1, slot_bytes, db, doff, hb, hoff, out, [&](const FrameGeom &G) {
+        p.out_bytes = G.out_bytes;
+        p.out_off = G.out_off;
+        p.out_capacity = G.total;
+        p.status = G.status;
+        p.path_cap = G.path_cap;
+        p.json_cap = G.json_cap;
+        p.path_limit = G.path_limit;
+        p.json_limit = G.json_limit;
+        return multi ? (has_data ? launch_jute<true, true>(p, G.smem, ctx->device, ctx->stream)
+                                 : launch_jute<true, false>(p, G.smem, ctx->device, ctx->stream))
+                     : (has_data ? launch_jute<false, true>(p, G.smem, ctx->device, ctx->stream)
+                                 : launch_jute<false, false>(p, G.smem, ctx->device, ctx->stream));
+    });
+}
+
+template <bool MULTI, bool DATA, bool PAIR>
+static cudaError_t launch_jute_entry(const JuteEntryParams &p, size_t smem, int device, cudaStream_t s)
+{
+    static std::mutex mu;
+    static size_t high[64];
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        if (smem > high[device & 63]) {
+            cudaError_t e = cudaFuncSetAttribute(regk_jute_entry_kernel<MULTI, DATA, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 (int)smem);
+            if (e != cudaSuccess)
+                return e;
+            high[device & 63] = smem;
+        }
+    }
+    regk_jute_entry_kernel<MULTI, DATA, PAIR><<<(unsigned)((p.n + JUTE_TILE - 1) / JUTE_TILE), JUTE_THREADS, smem, s>>>(p);
+    return cudaGetLastError();
+}
+
+/* Frames whose entries carry a version of their own (`version`: [n] device array, NULL = o->version for all) or that
+   pair a delete with a create (`pair`: REGK_ZK_REPLACE, always multi transactions) - regk_jute_entry_kernel.  Output
+   and buffers as frame_requests. */
+static int frame_entry_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts *o, const int32_t *version, bool pair,
+    DevBuf &db, DevBuf &doff, HostBuf &hb, HostBuf &hoff, regk_frames *out)
+{
+    const bool has_data = src.json_off != nullptr;
+    const bool multi = pair || o->group != 0;
+    const uint64_t g = o->group ? o->group : 1;
+    JuteEntryParams p{};
+    p.n = src.n;
+    p.op = pair ? (uint32_t)REGK_ZK_DELETE : o->op;
+    p.zk_flags = o->zk_flags;
+    p.version = version;
+    p.version_const = o->version;
+    p.group = (uint32_t)g;
+    /* delete: path length + version; setData: + data length; replace: 17 + P + 4 + J + 31 around the paths and data */
+    p.per_rec = (multi ? JUTE_MULTI_HEAD : 0u) + 4u + (pair ? 17u : 0u) + (has_data ? 4u : 0u) + (pair ? 31u : 4u);
+    p.path_bytes = src.path_bytes;
+    p.path_off = src.path_off;
+    p.json_bytes = src.json_bytes;
+    p.json_off = src.json_off;
+    p.xid_base = o->xid_base;
+    return frame_drive(ctx, src, o, multi, g, p.per_rec, pair ? 2 : 1, JUTE_TILE * JUTE_ESLOT, db, doff, hb, hoff, out,
+        [&](const FrameGeom &G) {
+            p.out_bytes = G.out_bytes;
+            p.out_off = G.out_off;
+            p.out_capacity = G.total;
+            p.status = G.status;
+            p.path_cap = G.path_cap;
+            p.json_cap = G.json_cap;
+            p.path_limit = G.path_limit;
+            p.json_limit = G.json_limit;
+            cudaStream_t s = ctx->stream;
+            return pair ? launch_jute_entry<true, true, true>(p, G.smem, ctx->device, s)
+                : multi ? (has_data ? launch_jute_entry<true, true, false>(p, G.smem, ctx->device, s)
+                                    : launch_jute_entry<true, false, false>(p, G.smem, ctx->device, s))
+                        : (has_data ? launch_jute_entry<false, true, false>(p, G.smem, ctx->device, s)
+                                    : launch_jute_entry<false, false, false>(p, G.smem, ctx->device, s));
+        });
 }
 
 /* regk_parents.cuh on the path stream of the batch finished last (n >= 1 records), into the given buffers: enqueues
@@ -925,10 +1029,12 @@ void regk_destroy(regk_ctx *ctx)
     for (auto &b : ctx->rc)
         if (b.p)
             cudaFree(b.p);
-    for (HostBuf *b : {&ctx->h_rc_count, &ctx->h_rc_cls, &ctx->h_rc_match, &ctx->h_rc_obscls, &ctx->h_rc_list[0], &ctx->h_rc_list[1],
-             &ctx->h_rc_list[2], &ctx->h_rc_list[3], &ctx->h_rc_fbytes, &ctx->h_rc_foff})
+    for (HostBuf *b : {&ctx->h_rc_count, &ctx->h_rc_cls, &ctx->h_rc_match, &ctx->h_rc_obscls, &ctx->h_rc_fbytes, &ctx->h_rc_foff})
         if (b->p)
             cudaFreeHost(b->p);
+    for (auto &b : ctx->h_rc_list)
+        if (b.p)
+            cudaFreeHost(b.p);
     for (auto &ev : ctx->rc_ev)
         if (ev)
             cudaEventDestroy(ev);
@@ -2803,29 +2909,36 @@ int regk_mkdirp_requests(regk_ctx *ctx, int32_t xid_base, uint32_t zk_flags, uin
     return frame_requests(ctx, src, &o, ctx->mk[regk_ctx::MK_FBYTES], ctx->mk[regk_ctx::MK_FOFF], ctx->h_mk_fbytes, ctx->h_mk_foff, out);
 }
 
-int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk_delta *out)
+/* regk_reconcile (st == NULL) and regk_reconcile_owned: one implementation, the same four passes; `rep` / `n_rep` receive
+   the replace list of the owned call */
+static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_node_stat *st, uint32_t flags, regk_delta *out,
+    const uint64_t **rep, uint64_t *n_rep, const char *who)
 {
-    if (!ctx || !in || !out)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: NULL argument");
-    memset(out, 0, sizeof *out);
     ctx->rc_valid = false;
     if (in->flags & REGK_DECODE_LAST)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams");
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams", who);
     if (ctx->pending)
-        return fail(ctx, REGK_ERR_STATE, "regk_reconcile: batches are still in flight; finish them first");
+        return fail(ctx, REGK_ERR_STATE, "%s: batches are still in flight; finish them first", who);
     if (!ctx->last_path_off || !ctx->last_json_off || ctx->last_n != ctx->last_json_n)
-        return fail(ctx, REGK_ERR_STATE, "regk_reconcile: no finished batch with both a path and a payload stream on this context "
-                                         "(an empty batch or a REGK_JOB_STEP result leaves none)");
+        return fail(ctx, REGK_ERR_STATE, "%s: no finished batch with both a path and a payload stream on this context "
+                                         "(an empty batch or a REGK_JOB_STEP result leaves none)", who);
     const uint64_t n = ctx->last_n, m = in->n;
     if (n >= 0xFFFFFFFFull || m >= 0xFFFFFFFFull)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: %llu records and %llu nodes: both must be below 2^32 - 1",
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: %llu records and %llu nodes: both must be below 2^32 - 1", who,
             (unsigned long long)n, (unsigned long long)m);
     const bool in_dev = in->flags & REGK_IN_DEVICE, dev_out = flags & REGK_OUT_DEVICE;
     const uint8_t *pb = in->path_bytes, *jb = in->json_bytes;
     const uint64_t *po = in->path_off, *jo = in->json_off;
     uint64_t path_total = m ? in->path_total : 0, json_total = m ? in->json_total : 0;
     if (m && (!po || !jo))
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: a snapshot of %llu nodes needs path and data offsets", (unsigned long long)m);
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: a snapshot of %llu nodes needs path and data offsets", who, (unsigned long long)m);
+    const int32_t *sver = st ? st->version : nullptr;
+    const int64_t *sown = st ? st->ephemeral_owner : nullptr;
+    if (st && m && (!sver || !sown))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: a snapshot of %llu nodes needs a version and an owner per node", who,
+            (unsigned long long)m);
+    if (st && m && in_dev && (((uintptr_t)sver & 3u) || ((uintptr_t)sown & 7u)))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device stats (version needs 4-byte, ephemeral_owner 8-byte alignment)", who);
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     DevBuf *rb = ctx->rc;
@@ -2836,13 +2949,13 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
         /* offsets become memory ranges in the kernels: monotone, each node below 4 GiB, ending at the totals */
         for (uint64_t j = 0; j < m; j++)
             if (po[j] > po[j + 1] || jo[j] > jo[j + 1] || po[j + 1] - po[j] > 0xFFFFFFFFull || jo[j + 1] - jo[j] > 0xFFFFFFFFull)
-                return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot offsets are not monotone at node %llu",
+                return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets are not monotone at node %llu", who,
                     (unsigned long long)j);
         if ((path_total && !pb) || (json_total && !jb))
-            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot offsets without bytes");
-        const void *src[4] = {pb, po, jb, jo};
-        const size_t sz[4] = {(size_t)path_total, (size_t)(m + 1) * 8, (size_t)json_total, (size_t)(m + 1) * 8};
-        for (int k = 0; k < 4; k++) {
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets without bytes", who);
+        const void *src[6] = {pb, po, jb, jo, sver, sown};
+        const size_t sz[6] = {(size_t)path_total, (size_t)(m + 1) * 8, (size_t)json_total, (size_t)(m + 1) * 8, (size_t)m * 4, (size_t)m * 8};
+        for (int k = 0; k < (st ? 6 : 4); k++) {
             if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_IN_PB + k], sz[k] + 16)))
                 return rc;
             if (sz[k])
@@ -2852,11 +2965,15 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
         po = (const uint64_t *)rb[regk_ctx::RC_IN_PO].p;
         jb = (const uint8_t *)rb[regk_ctx::RC_IN_JB].p;
         jo = (const uint64_t *)rb[regk_ctx::RC_IN_JO].p;
+        if (st) {
+            sver = (const int32_t *)rb[regk_ctx::RC_IN_VER].p;
+            sown = (const int64_t *)rb[regk_ctx::RC_IN_OWN].p;
+        }
     } else if (m) {
         if ((path_total && !pb) || (json_total && !jb))
-            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot offsets without bytes");
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets without bytes", who);
         if (((uintptr_t)pb & 3u) || ((uintptr_t)jb & 3u) || ((uintptr_t)po & 7u) || ((uintptr_t)jo & 7u))
-            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: misaligned device snapshot (bytes need 4-byte, offsets 8-byte alignment)");
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device snapshot (bytes need 4-byte, offsets 8-byte alignment)", who);
     }
     /* an empty stream is never read; its kernels still get a valid pointer */
     if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_IN_PB], 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_IN_JB], 16)))
@@ -2881,7 +2998,7 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
     const uint64_t so = table_slots(m), sd = table_slots(n);
     const uint64_t tiles_r = (n + RC_TILE - 1) / RC_TILE, tiles_o = (m + RC_TILE - 1) / RC_TILE;
     const size_t ttr = align16(tiles_r * 4), str = (tiles_r / SUPER + 1) * 8, tto = align16(tiles_o * 4), sto = (tiles_o / SUPER + 1) * 8;
-    const size_t totals_bytes = 3 * (ttr + str) + tto + sto;
+    const size_t totals_bytes = RC_NREC_LISTS * (ttr + str) + tto + sto;
     const size_t counters_bytes = RC_NCOUNTERS * 8;
     if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_TOBS], so * 4)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_TDES], sd * 4)) ||
         (rc = ensure_dev(ctx, rb[regk_ctx::RC_SLOTO], m * 4 + 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_HASHO], m * 4 + 16)) ||
@@ -2893,8 +3010,11 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
     for (int l = 0; l < RC_NLISTS; l++)
         if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_LIST0 + l], (l == RC_LDELETE ? m : n) * 8 + 8)))
             return rc;
-    for (int k = 0; k < 5; k++)
-        if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_LEN0 + k], (k == 4 ? m : n) * 4 + 8)))
+    for (int k = 0; k < RC_NGATHERS; k++)
+        if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_LEN0 + k], (k == RC_GDELETE ? m : n) * 4 + 8)))
+            return rc;
+    for (int k = 0; st && k < RC_NVER; k++)
+        if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_VER0 + k], (k == RC_VDELETE ? m : n) * 4 + 8)))
             return rc;
     for (auto &ev : ctx->rc_ev)
         if (!ev)
@@ -2915,6 +3035,13 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
     p.o_path_total = path_total;                    /* a caller's device buffers end where they end */
     p.o_json_total = json_total;
     p.validate = in_dev ? 1u : 0u;
+    if (st) {
+        p.o_version = sver;
+        p.o_owner = (const long long *)sown;
+        p.want = st->zk_flags == 1u ? (long long)st->session : 0ll;
+        for (int k = 0; k < RC_NVER; k++)
+            p.ver[k] = (int32_t *)rb[regk_ctx::RC_VER0 + k].p;
+    }
     p.mask_o = (uint32_t)(so - 1);
     p.mask_d = (uint32_t)(sd - 1);
     p.t_obs = (uint32_t *)rb[regk_ctx::RC_TOBS].p;
@@ -2932,7 +3059,7 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
         p.super_total[l] = (unsigned long long *)(tb + (size_t)l * (ttr + str) + (del ? tto : ttr));
         p.list[l] = (unsigned long long *)rb[regk_ctx::RC_LIST0 + l].p;
     }
-    for (int k = 0; k < 5; k++)
+    for (int k = 0; k < RC_NGATHERS; k++)
         p.len[k] = (uint32_t *)rb[regk_ctx::RC_LEN0 + k].p;
     p.counters = (unsigned long long *)rb[regk_ctx::RC_COUNT].p;
     p.tiles_r = (uint32_t)tiles_r;
@@ -2956,33 +3083,35 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
     CK(cudaMemcpyAsync(hc, p.counters, counters_bytes, cudaMemcpyDeviceToHost, s));
     cudaError_t e = cudaStreamSynchronize(s);
     if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_reconcile: kernel execution failed: %s", cudaGetErrorString(e));
+        return fail(ctx, REGK_ERR_CUDA, "%s: kernel execution failed: %s", who, cudaGetErrorString(e));
     if (hc[RC_C_BAD] != ~0ull)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot offsets are not monotone or reach past the totals at node %llu",
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets are not monotone or reach past the totals at node %llu", who,
             hc[RC_C_BAD]);
     if (hc[RC_C_DUPNODE] != ~0ull)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: snapshot node %llu has the path of an earlier node; a registry cannot "
-                                               "hold two nodes with one path", hc[RC_C_DUPNODE]);
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot node %llu has the path of an earlier node; a registry cannot "
+                                               "hold two nodes with one path", who, hc[RC_C_DUPNODE]);
     uint64_t cnt[RC_NLISTS];
     for (int l = 0; l < RC_NLISTS; l++)
         cnt[l] = hc[RC_C_COUNT + l];
     if (n == 0)
-        cnt[RC_LCREATE] = cnt[RC_LUPDATE] = cnt[RC_LDUP] = 0;
+        cnt[RC_LCREATE] = cnt[RC_LUPDATE] = cnt[RC_LDUP] = cnt[RC_LREPLACE] = 0;
     if (m == 0)
         cnt[RC_LDELETE] = 0;
-    /* the request sets, packed: create paths, create payloads, update paths, update payloads, delete paths */
-    const int g_list[5] = {RC_LCREATE, RC_LCREATE, RC_LUPDATE, RC_LUPDATE, RC_LDELETE};
-    const uint8_t *g_src[5] = {p.d_path, p.d_json, p.d_path, p.d_json, p.o_path};
-    const unsigned long long *g_off[5] = {p.d_path_off, p.d_json_off, p.d_path_off, p.d_json_off, p.o_path_off};
+    /* the request sets, packed: create paths, create payloads, update paths, update payloads, delete paths, replace
+       paths, replace payloads */
+    const int g_list[RC_NGATHERS] = {RC_LCREATE, RC_LCREATE, RC_LUPDATE, RC_LUPDATE, RC_LDELETE, RC_LREPLACE, RC_LREPLACE};
+    const uint8_t *g_src[RC_NGATHERS] = {p.d_path, p.d_json, p.d_path, p.d_json, p.o_path, p.d_path, p.d_json};
+    const unsigned long long *g_off[RC_NGATHERS] = {p.d_path_off, p.d_json_off, p.d_path_off, p.d_json_off, p.o_path_off,
+                                                    p.d_path_off, p.d_json_off};
     uint64_t gmax = 0;
-    for (int g = 0; g < 5; g++)
+    for (int g = 0; g < RC_NGATHERS; g++)
         gmax = std::max<uint64_t>(gmax, cnt[g_list[g]]);
     const uint64_t gt = (gmax + MK_TILE - 1) / MK_TILE;
     if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_GTOTALS], gt * 8 + (gt / SUPER + 1) * 8 + 16)))
         return rc;
-    for (int g = 0; g < 5; g++) {
+    for (int g = 0; g < RC_NGATHERS; g++) {
         const uint64_t c = cnt[g_list[g]], bytes = hc[RC_C_BYTES + g];
-        DevBuf &gb = rb[regk_ctx::RC_G0B + 2 * g], &go = rb[regk_ctx::RC_G0O + 2 * g];
+        DevBuf &gb = rb[regk_ctx::RC_G0B + 2 * g], &go = rb[regk_ctx::RC_G0B + 2 * g + 1];
         if ((rc = ensure_dev(ctx, gb, bytes + 16)) || (rc = ensure_dev(ctx, go, (c + 1) * 8)))
             return rc;
         if (!c) {
@@ -3009,15 +3138,21 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
     CK(cudaEventRecord(ctx->rc_ev[1], s));
     e = cudaStreamSynchronize(s);
     if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_reconcile: kernel execution failed: %s", cudaGetErrorString(e));
+        return fail(ctx, REGK_ERR_CUDA, "%s: kernel execution failed: %s", who, cudaGetErrorString(e));
     float ms = 0;
     cudaEventElapsedTime(&ms, ctx->rc_ev[0], ctx->rc_ev[1]);
-    const void *dsrc[7] = {p.cls, p.match, p.obs_cls, p.list[0], p.list[1], p.list[2], p.list[3]};
+    const int NOUT = 3 + RC_NLISTS;                 /* cls, match, obs_cls, then the lists */
+    const void *dsrc[NOUT] = {p.cls, p.match, p.obs_cls};
+    for (int l = 0; l < RC_NLISTS; l++)
+        dsrc[3 + l] = p.list[l];
     if (!dev_out) {
-        HostBuf *hb[7] = {&ctx->h_rc_cls, &ctx->h_rc_match, &ctx->h_rc_obscls, &ctx->h_rc_list[0], &ctx->h_rc_list[1],
-                          &ctx->h_rc_list[2], &ctx->h_rc_list[3]};
-        const size_t sz[7] = {n, n * 8, m, cnt[0] * 8, cnt[1] * 8, cnt[2] * 8, cnt[3] * 8};
-        for (int k = 0; k < 7; k++) {
+        HostBuf *hb[NOUT] = {&ctx->h_rc_cls, &ctx->h_rc_match, &ctx->h_rc_obscls};
+        size_t sz[NOUT] = {n, n * 8, m};
+        for (int l = 0; l < RC_NLISTS; l++) {
+            hb[3 + l] = &ctx->h_rc_list[l];
+            sz[3 + l] = cnt[l] * 8;
+        }
+        for (int k = 0; k < NOUT; k++) {
             if ((rc = ensure_host(ctx, *hb[k], sz[k] + 16)))
                 return rc;
             if (sz[k])
@@ -3027,6 +3162,8 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
         CK(cudaStreamSynchronize(s));
     }
     ctx->rc_valid = true;
+    ctx->rc_owned = st != nullptr;
+    ctx->rc_zk_flags = st ? st->zk_flags : 0u;
     for (int l = 0; l < RC_NLISTS; l++)
         ctx->rc_count[l] = cnt[l];
     out->n = n;
@@ -3035,44 +3172,93 @@ int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk
     out->n_update = cnt[RC_LUPDATE];
     out->n_dup = cnt[RC_LDUP];
     out->n_delete = cnt[RC_LDELETE];
-    out->n_same = n - out->n_create - out->n_update - out->n_dup;
+    out->n_same = n - out->n_create - out->n_update - out->n_dup - cnt[RC_LREPLACE];
     out->flags = dev_out ? REGK_OUT_DEVICE : 0;
     out->launches = launches;
     out->cls = (const uint8_t *)dsrc[0];
     out->match = (const uint64_t *)dsrc[1];
     out->obs_cls = (const uint8_t *)dsrc[2];
-    out->create = (const uint64_t *)dsrc[3];
-    out->update = (const uint64_t *)dsrc[4];
-    out->dup = (const uint64_t *)dsrc[5];
-    out->del = (const uint64_t *)dsrc[6];
+    out->create = (const uint64_t *)dsrc[3 + RC_LCREATE];
+    out->update = (const uint64_t *)dsrc[3 + RC_LUPDATE];
+    out->dup = (const uint64_t *)dsrc[3 + RC_LDUP];
+    out->del = (const uint64_t *)dsrc[3 + RC_LDELETE];
     out->kernel_ms = ms;
+    if (rep) {
+        *rep = (const uint64_t *)dsrc[3 + RC_LREPLACE];
+        *n_rep = cnt[RC_LREPLACE];
+    }
     return REGK_OK;
 }
+
+int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk_delta *out)
+{
+    if (!ctx || !in || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile: NULL argument");
+    memset(out, 0, sizeof *out);
+    return reconcile_run(ctx, in, nullptr, flags, out, nullptr, nullptr, "regk_reconcile");
+}
+
+int regk_reconcile_owned(regk_ctx *ctx, const regk_decode_in *in, const regk_node_stat *st, uint32_t flags, regk_delta_owned *out)
+{
+    if (!ctx || !in || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_owned: NULL argument");
+    memset(out, 0, sizeof *out);
+    ctx->rc_valid = false;
+    if (!st)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_owned: NULL stat; regk_reconcile compares bytes alone");
+    if (st->zk_flags > 1u)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_owned: zk_flags %u is not 0 (persistent) or 1 (EPHEMERAL); a "
+                                               "sequential or container mode makes a path key meaningless", st->zk_flags);
+    if (st->zk_flags == 1u && st->session == 0)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_owned: EPHEMERAL nodes need the session id they are sent on");
+    return reconcile_run(ctx, in, st, flags, &out->d, &out->replace, &out->n_replace, "regk_reconcile_owned");
+}
+
 
 int regk_reconcile_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
 {
     if (!ctx || !o || !out)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: NULL argument");
     memset(out, 0, sizeof *out);
-    if (o->op != REGK_ZK_CREATE && o->op != REGK_ZK_DELETE && o->op != REGK_ZK_SETDATA)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: op %u is not create (1), delete (2) or setData (5)", o->op);
+    const bool replace = o->op == REGK_ZK_REPLACE, observed = o->flags & REGK_ZK_VERSION_OBSERVED;
+    if (o->op != REGK_ZK_CREATE && o->op != REGK_ZK_DELETE && o->op != REGK_ZK_SETDATA && !replace)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: op %u is not create (1), delete (2), setData (5) or "
+                                               "replace (256)", o->op);
+    if (observed && o->op == REGK_ZK_CREATE)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: a CreateRequest carries no version to observe");
     if (o->group > 65536)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: at most 65536 operations per multi transaction");
+    if (replace && o->group > 32768)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: at most 32768 replace entries (65536 operations) per "
+                                               "multi transaction");
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "regk_reconcile_requests: batches are still in flight; finish them first");
     if (!ctx->rc_valid)
         return fail(ctx, REGK_ERR_STATE, "regk_reconcile_requests: no reconcile result on this context; call regk_reconcile first");
+    if ((replace || observed) && !ctx->rc_owned)
+        return fail(ctx, REGK_ERR_STATE, "regk_reconcile_requests: replace frames and observed versions need node stats; the last "
+                                         "reconcile was regk_reconcile, call regk_reconcile_owned");
+    if (ctx->rc_owned && (replace || o->op == REGK_ZK_CREATE) && o->zk_flags != ctx->rc_zk_flags)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: zk_flags %u differs from the CreateMode %u regk_reconcile_owned "
+                                               "classified with; nodes created so would be classed REPLACE again", o->zk_flags,
+                    ctx->rc_zk_flags);
     CK(cudaSetDevice(ctx->device));
-    /* gathered streams: create paths / payloads (0, 1), update paths / payloads (2, 3), delete paths (4) */
-    const int g = o->op == REGK_ZK_CREATE ? 0 : o->op == REGK_ZK_SETDATA ? 2 : 4;
-    const uint64_t c = ctx->rc_count[o->op == REGK_ZK_CREATE ? RC_LCREATE : o->op == REGK_ZK_SETDATA ? RC_LUPDATE : RC_LDELETE];
+    /* gathered streams: create paths / payloads, update paths / payloads, delete paths, replace paths / payloads */
+    const int g = o->op == REGK_ZK_CREATE ? RC_GCREATE : o->op == REGK_ZK_SETDATA ? RC_GUPDATE : replace ? RC_GREPLACE : RC_GDELETE;
+    const int l = o->op == REGK_ZK_CREATE ? RC_LCREATE : o->op == REGK_ZK_SETDATA ? RC_LUPDATE : replace ? RC_LREPLACE : RC_LDELETE;
+    const uint64_t c = ctx->rc_count[l];
     DevBuf *rb = ctx->rc;
-    const bool data = g != 4;
-    FrameSrc src{c, (const uint8_t *)rb[regk_ctx::RC_G0B + 2 * g].p, (const unsigned long long *)rb[regk_ctx::RC_G0O + 2 * g].p,
+    const bool data = g != RC_GDELETE;
+    FrameSrc src{c, (const uint8_t *)rb[regk_ctx::RC_G0B + 2 * g].p, (const unsigned long long *)rb[regk_ctx::RC_G0B + 2 * g + 1].p,
                  data ? (const uint8_t *)rb[regk_ctx::RC_G0B + 2 * g + 2].p : nullptr,
-                 data ? (const unsigned long long *)rb[regk_ctx::RC_G0O + 2 * g + 2].p : nullptr};
+                 data ? (const unsigned long long *)rb[regk_ctx::RC_G0B + 2 * g + 3].p : nullptr};
     src.who = "regk_reconcile_requests";
-    return frame_requests(ctx, src, o, rb[regk_ctx::RC_FBYTES], rb[regk_ctx::RC_FOFF], ctx->h_rc_fbytes, ctx->h_rc_foff, out);
+    if (!replace && !observed)
+        return frame_requests(ctx, src, o, rb[regk_ctx::RC_FBYTES], rb[regk_ctx::RC_FOFF], ctx->h_rc_fbytes, ctx->h_rc_foff, out);
+    const int v = l == RC_LUPDATE ? RC_VUPDATE : l == RC_LREPLACE ? RC_VREPLACE : RC_VDELETE;
+    const int32_t *ver = observed ? (const int32_t *)rb[regk_ctx::RC_VER0 + v].p : nullptr;
+    return frame_entry_requests(ctx, src, o, ver, replace, rb[regk_ctx::RC_FBYTES], rb[regk_ctx::RC_FOFF], ctx->h_rc_fbytes,
+                                ctx->h_rc_foff, out);
 }
 
 int regk_release(regk_ctx *ctx, regk_result *res)

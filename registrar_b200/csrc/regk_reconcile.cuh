@@ -7,6 +7,8 @@
  *                       first create)
  *               CREATE  no node has path i          UPDATE  the node's data differs from payload i
  *               SAME    the node holds payload i byte for byte
+ *               REPLACE (stats present: regk_reconcile_owned) the node's ephemeral owner is not the one wanted; the
+ *                       payload is not compared
  *   match[i]    the node with path i, or ~0 (DUP records carry their path's match too)
  *   obs_cls[j]  KEEP if some record has path j, else DELETE
  *
@@ -15,14 +17,16 @@
  *             smallest bad index and never read); then j + 1 goes into T_o, an open-addressing table of 32-bit slots,
  *             with the protocol of regk_parent_kernel: atomicCAS claims an empty slot, a slot whose node has the same
  *             path keeps the smaller index by atomicMin, any other slot moves on.
- *   desired   one thread per record: probe T_o read-only (match, then the payload comparison), then insert i + 1
- *             into T_d with the same protocol.
+ *   desired   one thread per record: probe T_o read-only (match; with stats, the matched node's owner; then the
+ *             payload comparison), then insert i + 1 into T_d with the same protocol.
  *   mark      records: DUP iff the T_d slot names another record.  Nodes: a node whose T_o slot names another node
  *             is a duplicate path (the call is refused, naming the smallest such index); the others probe T_d for
- *             KEEP / DELETE.  Per-tile counts of the four lists go into two-level totals.
- *   compact   the create / update / dup / delete lists in index order, with the byte lengths the gathers need.
+ *             KEEP / DELETE.  Per-tile counts of the five lists go into two-level totals.
+ *   compact   the create / update / dup / replace / delete lists in index order, with the byte lengths the gathers
+ *             need and, with stats, the Stat.version of each update, replace and delete entry's node.
  * Then regk_mkdirp_len_kernel / regk_mkdirp_gather_kernel pack the request sets (create paths and payloads, update
- * paths and payloads, delete paths) into streams of the library's own, which regk_reconcile_requests frames.
+ * paths and payloads, delete paths, replace paths and payloads) into streams of the library's own, which
+ * regk_reconcile_requests frames.  Without stats (regk_reconcile) the replace list stays empty.
  *
  * The snapshot may be a caller's device buffer with no slack behind its last byte, so every read of its bytes goes
  * through the clamped helpers of regk_core.cuh (string_word_clamped and friends), which never touch a byte at or past
@@ -38,14 +42,17 @@ namespace regk {
 constexpr uint32_t RC_TILE = TILE;              /* items per CTA of the mark / compact passes (128) */
 constexpr uint32_t RC_BAD_SLOT = 0xFFFFFFFFu;   /* slot_obs of a node with bad offsets */
 
-enum : uint8_t { RC_SAME = 0, RC_CREATE = 1, RC_UPDATE = 2, RC_DUP = 3 };     /* cls (include/regk.h REGK_DELTA_*) */
+enum : uint8_t { RC_SAME = 0, RC_CREATE = 1, RC_UPDATE = 2, RC_DUP = 3, RC_REPLACE = 4 };  /* cls (include/regk.h REGK_DELTA_*) */
 enum : uint8_t { RC_KEEP = 0, RC_DELETE = 1 };                               /* obs_cls */
-enum { RC_LCREATE, RC_LUPDATE, RC_LDUP, RC_LDELETE, RC_NLISTS };
+enum { RC_LCREATE, RC_LUPDATE, RC_LDUP, RC_LREPLACE, RC_LDELETE, RC_NLISTS };   /* the record lists first, then the nodes' */
+enum { RC_NREC_LISTS = RC_LDELETE };
+/* the gathers: create paths / payloads, update paths / payloads, delete paths, replace paths / payloads */
+enum { RC_GCREATE = 0, RC_GUPDATE = 2, RC_GDELETE = 4, RC_GREPLACE = 5, RC_NGATHERS = 7 };
+enum { RC_VUPDATE, RC_VDELETE, RC_VREPLACE, RC_NVER };                      /* the lists that carry a version */
 
 /* counters[]: [0] smallest node with bad offsets, [1] smallest node with a duplicate path (both ~0 = none, set by the
-   host), [2 + list] entries of each list, [6 + k] bytes of gather k (create paths, create payloads, update paths,
-   update payloads, delete paths) */
-enum { RC_C_BAD = 0, RC_C_DUPNODE = 1, RC_C_COUNT = 2, RC_C_BYTES = 6, RC_NCOUNTERS = 11 };
+   host), [2 + list] entries of each list, [7 + k] bytes of gather k */
+enum { RC_C_BAD = 0, RC_C_DUPNODE = 1, RC_C_COUNT = 2, RC_C_BYTES = 2 + RC_NLISTS, RC_NCOUNTERS = RC_C_BYTES + RC_NGATHERS };
 
 struct ReconcileParams {
     uint64_t n, m;
@@ -62,6 +69,10 @@ struct ReconcileParams {
     const unsigned long long *o_json_off;
     uint64_t o_path_total, o_json_total;        /* readable bytes: exactly these */
     uint32_t validate;                          /* device snapshot: check the offsets in the insert pass */
+    /* the snapshot's Stat (regk_reconcile_owned), NULL for regk_reconcile */
+    const int32_t *o_version;                   /* [m] */
+    const long long *o_owner;                   /* [m] ephemeral owner, 0 = persistent */
+    long long want;                             /* the owner every matched node must have */
     uint32_t mask_o, mask_d;                    /* slots - 1 of T_o / T_d (powers of two) */
     uint32_t *t_obs;                            /* T_o: node + 1, 0 = empty (zeroed by the host) */
     uint32_t *t_des;                            /* T_d: record + 1 */
@@ -74,7 +85,8 @@ struct ReconcileParams {
     uint32_t *tile_total[RC_NLISTS];            /* records: [ntiles_r], delete: [ntiles_o] */
     unsigned long long *super_total[RC_NLISTS];
     unsigned long long *list[RC_NLISTS];        /* ascending indices */
-    uint32_t *len[5];                           /* per list entry: create path / payload, update path / payload, delete path */
+    uint32_t *len[RC_NGATHERS];                 /* per list entry: the bytes of its path / payload in each gather */
+    int32_t *ver[RC_NVER];                      /* per update / delete / replace entry: its node's version (with stats) */
     unsigned long long *counters;               /* [RC_NCOUNTERS] */
     uint32_t tiles_r;                           /* CTAs of the mark / compact passes that cover records; the rest cover nodes */
 };
@@ -157,7 +169,9 @@ __global__ void __launch_bounds__(256, 4) regk_reconcile_desired_kernel(const Re
             slot = (slot + 1u) & p.mask_o;
         }
     }
-    if (match != ~0ull) {
+    if (match != ~0ull && p.o_owner && p.o_owner[match] != p.want) {
+        c = RC_REPLACE;                                     /* the payload does not matter: the node is created again */
+    } else if (match != ~0ull) {
         const unsigned long long q0 = p.d_json_off[i], k0 = p.o_json_off[match];
         const uint32_t jl = (uint32_t)(p.d_json_off[i + 1] - q0);
         const bool same = rc_obs_len(p.o_json_off, match) == jl &&
@@ -204,7 +218,8 @@ __global__ void __launch_bounds__(RC_TILE) regk_reconcile_mark_kernel(const Reco
                 c = RC_DUP;
                 p.cls[i] = c;
             }
-            f = c == RC_CREATE ? 1u << RC_LCREATE : c == RC_UPDATE ? 1u << RC_LUPDATE : c == RC_DUP ? 1u << RC_LDUP : 0u;
+            f = c == RC_CREATE ? 1u << RC_LCREATE : c == RC_UPDATE ? 1u << RC_LUPDATE : c == RC_DUP ? 1u << RC_LDUP :
+                c == RC_REPLACE ? 1u << RC_LREPLACE : 0u;
         }
     } else if (i < p.m) {
         const uint32_t so = p.slot_obs[i];
@@ -236,7 +251,7 @@ __global__ void __launch_bounds__(RC_TILE) regk_reconcile_mark_kernel(const Reco
     }
     if (rec) {
         #pragma unroll
-        for (int l = RC_LCREATE; l <= RC_LDUP; l++) {
+        for (int l = RC_LCREATE; l < RC_NREC_LISTS; l++) {
             const uint32_t c = __popc(__ballot_sync(0xFFFFFFFFu, (f >> l) & 1u));
             if ((threadIdx.x & 31u) == 0)
                 add_tile_total(p.tile_total[l], p.super_total[l], tile, c);
@@ -248,15 +263,16 @@ __global__ void __launch_bounds__(RC_TILE) regk_reconcile_mark_kernel(const Reco
     }
 }
 
-/* ---- compact: every list in index order, and the byte lengths of its entries ---- */
+/* ---- compact: every list in index order, the byte lengths of its entries and, with stats, their versions ---- */
 __global__ void __launch_bounds__(RC_TILE) regk_reconcile_compact_kernel(const ReconcileParams p)
 {
-    __shared__ uint32_t s_warp[3][RC_TILE / 32];
-    __shared__ unsigned long long s_base[3];
+    constexpr uint32_t NL = RC_NREC_LISTS;                  /* lists of a record CTA (a node CTA has one) */
+    __shared__ uint32_t s_warp[NL][RC_TILE / 32];
+    __shared__ unsigned long long s_base[NL];
     const bool rec = blockIdx.x < p.tiles_r;
     const uint32_t tile = rec ? blockIdx.x : blockIdx.x - p.tiles_r;
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const int l0 = rec ? RC_LCREATE : RC_LDELETE, nl = rec ? 3 : 1;
+    const int l0 = rec ? RC_LCREATE : RC_LDELETE, nl = rec ? (int)NL : 1;
     if (threadIdx.x < 32) {
         for (int l = 0; l < nl; l++) {
             const unsigned long long b = tile_base_from_totals(p.tile_total[l0 + l], p.super_total[l0 + l], tile);
@@ -265,53 +281,62 @@ __global__ void __launch_bounds__(RC_TILE) regk_reconcile_compact_kernel(const R
         }
     }
     const uint64_t i = (uint64_t)tile * RC_TILE + threadIdx.x;
-    uint32_t l = 3;                                         /* which of this CTA's lists the item goes to (3: none) */
+    uint32_t l = NL;                                        /* which of this CTA's lists the item goes to (NL: none) */
     if (rec && i < p.n) {
         const uint8_t c = p.cls[i];
-        l = c == RC_CREATE ? 0u : c == RC_UPDATE ? 1u : c == RC_DUP ? 2u : 3u;
+        l = c == RC_CREATE ? RC_LCREATE : c == RC_UPDATE ? RC_LUPDATE : c == RC_DUP ? RC_LDUP : c == RC_REPLACE ? RC_LREPLACE : NL;
     } else if (!rec && i < p.m && p.obs_cls[i] == RC_DELETE && p.slot_obs[i] != RC_BAD_SLOT) {
         l = 0;
     }
-    uint32_t bal[3], rank = 0;
+    uint32_t bal[NL], rank = 0;
     #pragma unroll
-    for (int k = 0; k < 3; k++) {
+    for (int k = 0; k < (int)NL; k++) {
         bal[k] = __ballot_sync(0xFFFFFFFFu, l == (uint32_t)k);
         if (lane == 0)
             s_warp[k][warp] = __popc(bal[k]);
     }
     __syncthreads();
-    if (l < 3u) {
+    if (l < NL) {
         rank = __popc(bal[l] & ((1u << lane) - 1u));
         for (uint32_t w = 0; w < warp; w++)
             rank += s_warp[l][w];
     }
+    /* the gather of this entry's path (its payload is the next one), and the version list it feeds (-1: none) */
+    const int gq = !rec ? RC_GDELETE : l == RC_LCREATE ? RC_GCREATE : l == RC_LUPDATE ? RC_GUPDATE : l == RC_LREPLACE ? RC_GREPLACE : -1;
+    const int vq = !rec ? RC_VDELETE : l == RC_LUPDATE ? RC_VUPDATE : l == RC_LREPLACE ? RC_VREPLACE : -1;
     uint32_t lens[2] = {0u, 0u};                            /* path and payload bytes of this entry */
-    if (l < 3u) {
+    if (l < NL) {
         const unsigned long long k = s_base[l] + rank;
         p.list[l0 + l][k] = i;
-        if (rec && l < 2u) {
+        if (rec && gq >= 0) {
             lens[0] = (uint32_t)(p.d_path_off[i + 1] - p.d_path_off[i]);
             lens[1] = (uint32_t)(p.d_json_off[i + 1] - p.d_json_off[i]);
-            p.len[2 * l][k] = lens[0];
-            p.len[2 * l + 1][k] = lens[1];
+            p.len[gq][k] = lens[0];
+            p.len[gq + 1][k] = lens[1];
         } else if (!rec) {
             lens[0] = rc_obs_len(p.o_path_off, i);
-            p.len[4][k] = lens[0];
+            p.len[RC_GDELETE][k] = lens[0];
         }
+        if (p.o_version && vq >= 0)
+            p.ver[vq][k] = p.o_version[rec ? p.match[i] : i];
     }
-    /* bytes of each gather: create paths / payloads (l 0), update paths / payloads (l 1), delete paths */
+    /* bytes of each gather; a list no lane of the warp feeds is skipped (the test is warp-uniform) */
     #pragma unroll
-    for (int g = 0; g < 2; g++) {
+    for (int q = 0; q < 3; q++) {
+        const uint32_t lq = q == 0 ? RC_LCREATE : q == 1 ? RC_LUPDATE : RC_LREPLACE;
+        const int gb = q == 0 ? RC_GCREATE : q == 1 ? RC_GUPDATE : RC_GREPLACE;
+        if (rec ? bal[lq] == 0u : (q != 0 || bal[0] == 0u))
+            continue;
         #pragma unroll
         for (int s = 0; s < 2; s++) {
-            if (!rec && (g || s))
+            if (!rec && s)
                 continue;
-            unsigned long long v = (l == (uint32_t)g) ? lens[s] : 0u;
+            unsigned long long v = (l == (rec ? lq : 0u)) ? lens[s] : 0u;
             #pragma unroll
             for (int d = 16; d > 0; d >>= 1)
                 v += __shfl_xor_sync(0xFFFFFFFFu, v, d);
             if (lane == 0 && v)
-                atomicAdd(p.counters + RC_C_BYTES + (rec ? 2 * g + s : 4), v);
+                atomicAdd(p.counters + RC_C_BYTES + (rec ? gb + s : RC_GDELETE), v);
         }
     }
     const uint64_t items = rec ? p.n : p.m;
