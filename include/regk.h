@@ -370,9 +370,14 @@ int         regk_jute_frames(regk_ctx *ctx, uint32_t flags, int32_t xid_base, ui
  * out->n = number of frames, frame_off has n + 1 entries.  version is -1 ("any") unless the caller tracks versions.
  * PARITY UNPINNED like regk_jute_frames: restated from zookeeper.jute / MultiTransactionRecord, tested against an
  * independent restatement (oracle/pyoracle.py), not against a server.
+ *   REGK_ZK_GETDATA  GetDataRequest{path, watch = false}: the heartbeat's read of every node (lib/zk.js:21-44), whose
+ *                    replies regk_read_replies turns into a snapshot.  Frame i = len | xid_base + i (wrapping) | 4 | path
+ *                    length | path | 0, 17 + P_i bytes.  Paths only; group != 0 is REGK_ERR_INVALID_ARG (a multi holds
+ *                    no reads).  A successful call records the batch, xid_base and n for regk_read_replies.
  */
 #define REGK_ZK_CREATE  1u
 #define REGK_ZK_DELETE  2u
+#define REGK_ZK_GETDATA 4u
 #define REGK_ZK_SETDATA 5u
 
 typedef struct regk_jute_opts {
@@ -614,6 +619,54 @@ typedef struct regk_delta_owned {
 
 int         regk_reconcile_owned(regk_ctx *ctx, const regk_decode_in *snapshot, const regk_node_stat *stat,
                                  uint32_t flags, regk_delta_owned *out);
+
+/*
+ * ---- the replies to the getData frames of a batch, as a snapshot (the input half of the heartbeat: lib/zk.js:21-44
+ * stats every node, lib/index.js:131-159; and of re-registration after a session loss, lib/register.js:85-95,
+ * :228-239) -------------------------------------------------------------------------------------------------------------
+ * bytes[0, len) = what the caller read off the session after sending the frames of the last REGK_ZK_GETDATA
+ * regk_jute_requests call, back to back, from the first reply's length word on; host memory, or device memory with
+ * REGK_IN_DEVICE in flags (16-byte aligned).  Frame = int len | ReplyHeader{int xid; long zxid; int err} | body, big
+ * endian; body = GetDataResponse{buffer data (D = -1: null, read as empty); Stat (68 bytes)} when err == 0 (len == 88 +
+ * max(D, 0)), none otherwise (len == 16).  ZooKeeper answers a session's requests in order: the k-th frame that is not
+ * a watch notification (xid -1) or a ping (xid -2) must carry xid == xid_base + k (wrapping) and answers record k.
+ * Notifications and pings met before the n-th reply are skipped and counted; the stream may go on past the n-th reply.
+ * n_found + n_missing + n_error == n.  err[k] = ReplyHeader.err of record k's reply.
+ * snapshot: one node per distinct path among the replies with err == 0 (the first such reply gives it; later ones with
+ * the same path are dropped, as regk_reconcile refuses a snapshot that repeats a path; paths are compared byte for byte,
+ * a hash only picks a table slot).  Node j = record node_rec[j]: its path from the batch, its data from the reply, its
+ * Stat.version and Stat.ephemeralOwner - exactly the input regk_reconcile_owned(ctx, &out->snapshot, {version,
+ * ephemeral_owner, session, zk_flags}, ...) takes.  The snapshot holds the batch's own paths only, so a reconcile against
+ * it lists no DELETE.  A record whose reply is NONODE (-101) gets no node, so reconcile classes it CREATE; so does a
+ * record whose reply carries any other error: do not send the repair while n_error > 0.
+ * err and node_rec are pinned host arrays, or device arrays with REGK_OUT_DEVICE; the snapshot, version and
+ * ephemeral_owner are always device arrays.  All stay valid until the next regk_read_replies call (a later batch does
+ * not touch them).
+ * REGK_ERR_STATE: no REGK_ZK_GETDATA framing since the batch finished last, a batch finished since that framing, or a
+ * pending batch.  REGK_ERR_INVALID_ARG (the message names the byte position and the expected xid): the stream ends
+ * before the n-th reply is complete (and says how many were), len < 16, a negative xid other than -1 / -2, an xid
+ * outside the framed range, a reply out of order or for a record that already has one, a success frame whose length
+ * disagrees with its data length, D < -1, Stat.dataLength != max(D, 0), an error reply with a body; an xid range
+ * [xid_base, xid_base + n) that covers -1 or -2; NULL pointers; a misaligned device stream.
+ * PARITY UNPINNED: the reply layout is restated from zookeeper.jute and tested against an independent restatement.
+ */
+typedef struct regk_replies {
+    uint64_t n;                     /* requests: records of the framed batch */
+    uint64_t m;                     /* snapshot nodes: one per distinct path among replies with err == 0 */
+    uint64_t n_found, n_missing, n_error;   /* replies with err 0 / NONODE (-101) / any other err */
+    uint64_t n_skipped;             /* watch notifications (xid -1) and pings (xid -2) met before the n-th reply */
+    uint64_t consumed;              /* stream bytes up to the end of the n-th reply */
+    uint32_t flags, launches;
+    const int32_t  *err;            /* [n] ReplyHeader.err of record i's reply; REGK_OUT_DEVICE decides host/device */
+    const uint64_t *node_rec;       /* [m] record whose reply gave node j, ascending; same side as err */
+    regk_decode_in  snapshot;       /* ALWAYS device (REGK_IN_DEVICE set): path j = that record's path from the batch,
+                                       data j = the reply's data; aligned as regk_reconcile requires */
+    const int32_t  *version;        /* [m] device: Stat.version */
+    const int64_t  *ephemeral_owner;/* [m] device: Stat.ephemeralOwner */
+    float kernel_ms;
+} regk_replies;
+
+int         regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t flags, regk_replies *out);
 
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);

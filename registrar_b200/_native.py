@@ -95,6 +95,7 @@ class CJuteOpts(C.Structure):        # regk_jute_opts
 
 
 ZK_CREATE, ZK_DELETE, ZK_SETDATA = 1, 2, 5
+ZK_GETDATA = 4                      # jute_requests: GetDataRequest{path, watch = false}; its replies go to read_replies()
 ZK_REPLACE = 256                    # reconcile_requests after reconcile_owned: delete + create in one multi transaction
 FLAG_ZK_VERSION_OBSERVED = 1 << 9   # regk_jute_opts.flags: each frame carries its node's Stat.version
 
@@ -211,6 +212,51 @@ class CDeltaOwned(C.Structure):      # regk_delta_owned
     _fields_ = [("d", CDelta), ("n_replace", C.c_uint64), ("replace", C.c_void_p)]
 
 
+class CReplies(C.Structure):        # regk_replies
+    _fields_ = [("n", C.c_uint64), ("m", C.c_uint64), ("n_found", C.c_uint64), ("n_missing", C.c_uint64),
+                ("n_error", C.c_uint64), ("n_skipped", C.c_uint64), ("consumed", C.c_uint64),
+                ("flags", C.c_uint32), ("launches", C.c_uint32), ("err", C.c_void_p), ("node_rec", C.c_void_p),
+                ("snapshot", CDecodeIn), ("version", C.c_void_p), ("ephemeral_owner", C.c_void_p),
+                ("kernel_ms", C.c_float)]
+
+
+class Replies:
+    """What read_replies() made of the replies to the last getData framing: err[k] is the ReplyHeader.err of record
+    k's reply (0 found, -101 NONODE, other codes), node_rec[j] the record whose reply gave snapshot node j (ascending,
+    one node per distinct path among the found replies), plus n_found / n_missing / n_error / n_skipped and `consumed`
+    (stream bytes up to the end of the n-th reply).  The snapshot itself stays on the device: pass this object to
+    Context.reconcile_owned(replies, session=..., zk_flags=...) as it is, or copy it out with snapshot().  A record whose
+    reply carries an error other than NONODE gets no node either, so reconcile classes it CREATE: do not send the repair
+    while n_error > 0.  The snapshot is valid until the next read_replies() call on the context."""
+
+    def __init__(self, ctx, out):
+        self._ctx, self._out = ctx, out
+        n, m = int(out.n), int(out.m)
+        self.n, self.m, self.launches, self.kernel_ms = n, m, int(out.launches), float(out.kernel_ms)
+        self.n_found, self.n_missing, self.n_error = int(out.n_found), int(out.n_missing), int(out.n_error)
+        self.n_skipped, self.consumed = int(out.n_skipped), int(out.consumed)
+        self.err = _as_np(out.err, n, np.int32).copy()
+        self.node_rec = _as_np(out.node_rec, m, np.uint64).copy()
+
+    def cdecode_in(self):
+        """the device regk_decode_in of the snapshot.  Returns (struct, keepalive)."""
+        return self._out.snapshot, None
+
+    def cnode_stat(self, session: int, zk_flags: int):
+        """regk_node_stat over the snapshot's device version / owner arrays.  Returns (struct, keepalive)."""
+        return CNodeStat(version=self._out.version, ephemeral_owner=self._out.ephemeral_owner, session=session,
+                         zk_flags=zk_flags), None
+
+    def snapshot(self):
+        """host batch.Snapshot copy of the snapshot, with version and owner"""
+        from .batch import Snapshot
+        s, m = self._out.snapshot, self.m
+        d2h = lambda ptr, count, dtype: self._ctx._d2h(ptr, count, dtype)
+        return Snapshot(d2h(s.path_bytes, int(s.path_total), np.uint8), d2h(s.path_off, m + 1, np.uint64),
+                        d2h(s.json_bytes, int(s.json_total), np.uint8), d2h(s.json_off, m + 1, np.uint64),
+                        d2h(self._out.version, m, np.int32), d2h(self._out.ephemeral_owner, m, np.int64))
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -222,7 +268,8 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_sync", "regk_set_option", "regk_get_option", "regk_ipc_export", "regk_ipc_open", "regk_ipc_close",
            "regk_gather_push", "regk_parent_dirs", "regk_job_bind", "regk_service_records",
            "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records", "regk_mkdirp_dirs",
-           "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned"]
+           "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned",
+           "regk_read_replies"]
 
 _lib = None
 
@@ -279,6 +326,7 @@ def load_library():
     lib.regk_reconcile.argtypes = [vp, C.POINTER(CDecodeIn), u32, C.POINTER(CDelta)]
     lib.regk_reconcile_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     lib.regk_reconcile_owned.argtypes = [vp, C.POINTER(CDecodeIn), C.POINTER(CNodeStat), u32, C.POINTER(CDeltaOwned)]
+    lib.regk_read_replies.argtypes = [vp, vp, u64, u32, C.POINTER(CReplies)]
     _lib = lib
     return lib
 
@@ -652,6 +700,37 @@ class Context:
         n = int(out.n)
         return (_as_np(out.frame_bytes, int(out.total), np.uint8).copy(), _as_np(out.frame_off, n + 1, np.uint64).copy(),
                 float(out.kernel_ms))
+
+    # -- the replies to the getData frames of the batch finished last, as a snapshot --
+    def read_replies(self, stream, device: bool = False):
+        """regk_read_replies: `stream` (a NumPy uint8 array, or a contiguous CUDA uint8 tensor) holds the bytes read off
+        the session after sending the frames of the last jute_requests(op=ZK_GETDATA) call, from the first reply's
+        length word on.  Returns a Replies (input of reconcile_owned()), or the raw CReplies (err / node_rec on the
+        device) with device=True.  A record whose reply carries an error other than NONODE gets no snapshot node, so a
+        reconcile classes it CREATE: do not send the repair while n_error > 0."""
+        flags = FLAG_OUT_DEVICE if device else 0
+        if hasattr(stream, "data_ptr"):
+            import torch
+            if not stream.is_cuda or stream.dtype != torch.uint8 or not stream.is_contiguous():
+                raise ValueError("a device stream is a contiguous CUDA uint8 tensor")
+            keep, ptr, n = stream, stream.data_ptr() or None, stream.numel()
+            flags |= FLAG_IN_DEVICE
+        else:
+            keep = np.ascontiguousarray(stream)
+            if keep.dtype != np.uint8 or keep.ndim != 1:
+                raise ValueError("a host stream is a one-dimensional uint8 array")
+            ptr, n = _np_ptr(keep), keep.size
+        out = CReplies()
+        rc = self._lib.regk_read_replies(self._h, ptr, n, flags, C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else Replies(self, out)
+
+    def _d2h(self, ptr, count, dtype):
+        out = np.zeros(count, dtype)
+        if count:
+            self._check(self._lib.regk_memcpy_d2h(self._h, out.ctypes.data_as(C.c_void_p), C.c_void_p(ptr), out.nbytes))
+        return out
 
     # -- multi-GPU reassembly (regk_gather_push over CUDA-IPC mapped peer buffers) --
     def dev_alloc(self, nbytes: int) -> int:

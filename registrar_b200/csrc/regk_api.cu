@@ -30,6 +30,7 @@
 #include "regk_skip.cuh"
 #include "regk_mkdirp.cuh"
 #include "regk_reconcile.cuh"
+#include "regk_replies.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -136,6 +137,20 @@ struct regk_ctx {
     bool rc_owned = false;                      /* ... and it was regk_reconcile_owned: versions in rc[RC_VER*] */
     uint32_t rc_zk_flags = 0;                   /* the CreateMode regk_reconcile_owned classified with */
     uint64_t rc_count[RC_NLISTS] = {};          /* create, update, dup, replace, delete */
+    /* which batch finished last: bumped whenever the streams of the batch finished last change */
+    uint64_t last_gen = 0;
+    /* the last REGK_ZK_GETDATA framing: the batch it framed, xid_base, n (regk_read_replies reads its replies) */
+    bool gd_valid = false;
+    uint64_t gd_gen = 0, gd_n = 0;
+    int32_t gd_xid = 0;
+    /* regk_read_replies (regk_replies.cuh): staged stream, candidates, jump tables, per-record arrays, table, the nodes
+       and the gathered snapshot */
+    enum { RQ_STREAM, RQ_WORD, RQ_TOTALS, RQ_TOTALS2, RQ_TBASE, RQ_CAND, RQ_MARK, RQ_JUMP, RQ_ERRA, RQ_DPOS, RQ_DLEN, RQ_VER, RQ_OWN,
+           RQ_SLOT, RQ_TABLE, RQ_NREC, RQ_NVER, RQ_NOWN, RQ_NPLEN, RQ_NDLEN, RQ_GTOT, RQ_PB, RQ_PO, RQ_JB, RQ_JO, RQ_COUNT,
+           RQ_NBUF };
+    DevBuf rq[RQ_NBUF];
+    HostBuf h_rq_count, h_rq_err, h_rq_node;
+    cudaEvent_t rq_ev[2] = {nullptr, nullptr};
     std::vector<cudaEvent_t> pipe_events;
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     DevBuf skip_work, skip_in[11], skip_off_p, skip_off_j, skip_index, skip_bits;
@@ -727,7 +742,9 @@ static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_op
     p.multi = multi ? 1u : 0u;
     /* what follows the data: create - acl vector [OPEN_ACL_UNSAFE] + flags; delete / setData - the expected version */
     uint8_t tail[48] = {0};
-    if (o->op == REGK_ZK_CREATE) {
+    if (o->op == REGK_ZK_GETDATA) {
+        p.tail_len = 1;                                 /* watch = false */
+    } else if (o->op == REGK_ZK_CREATE) {
         static const uint8_t acl[27] = {0, 0, 0, 1, 0, 0, 0, 31, 0, 0, 0, 5, 'w', 'o', 'r', 'l', 'd', 0, 0, 0, 6, 'a', 'n', 'y', 'o', 'n', 'e'};
         memcpy(tail, acl, 27);
         for (int k = 0; k < 4; k++)
@@ -1036,6 +1053,15 @@ void regk_destroy(regk_ctx *ctx)
         if (b.p)
             cudaFreeHost(b.p);
     for (auto &ev : ctx->rc_ev)
+        if (ev)
+            cudaEventDestroy(ev);
+    for (auto &b : ctx->rq)
+        if (b.p)
+            cudaFree(b.p);
+    for (HostBuf *b : {&ctx->h_rq_count, &ctx->h_rq_err, &ctx->h_rq_node})
+        if (b->p)
+            cudaFreeHost(b->p);
+    for (auto &ev : ctx->rq_ev)
         if (ev)
             cudaEventDestroy(ev);
     for (auto &sl : ctx->slots)
@@ -1702,6 +1728,7 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
             ctx->skip_last.n = n;
         }
         if (rc == REGK_OK) {
+            ctx->last_gen++;
             ctx->last_path_bytes = do_path ? pp.out_bytes : nullptr;
             ctx->last_path_off = do_path ? pp.out_off : nullptr;
             ctx->last_n = do_path ? n : 0;
@@ -2202,6 +2229,7 @@ int regk_finish(regk_ctx *ctx, regk_result *res)
             ctx->skip_last.n = n;
         }
     }
+    ctx->last_gen++;
     ctx->last_path_bytes = st.bad_bits ? nullptr : slot->dev_path_bytes;
     ctx->last_path_off = st.bad_bits ? nullptr : slot->dev_path_off;
     ctx->last_n = (st.bad_bits || !slot->dev_path_off) ? 0 : n;
@@ -2425,6 +2453,7 @@ int regk_service_records(regk_ctx *ctx, const regk_service_batch *b, regk_result
             "service record %llu is outside the supported input domain (REGK_BAD bits 0x%x); no output produced",
             (unsigned long long)res->first_bad, st.bad_bits);
     res->json_total = st.json_total;
+    ctx->last_gen++;
     ctx->last_path_off = nullptr;                   /* the payload buffers were reused */
     ctx->last_json_off = nullptr;
     if (out_dev) {
@@ -2459,11 +2488,16 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
     if (!ctx || !o || !out)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: NULL argument");
     memset(out, 0, sizeof *out);
-    if (o->op != REGK_ZK_CREATE && o->op != REGK_ZK_DELETE && o->op != REGK_ZK_SETDATA)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: op %u is not create (1), delete (2) or setData (5)", o->op);
+    const bool getdata = o->op == REGK_ZK_GETDATA;
+    if (o->op != REGK_ZK_CREATE && o->op != REGK_ZK_DELETE && o->op != REGK_ZK_SETDATA && !getdata)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: op %u is not create (1), delete (2), getData (4) or setData (5)",
+            o->op);
     if (o->group > 65536)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: at most 65536 operations per multi transaction");
-    const bool has_data = o->op != REGK_ZK_DELETE;
+    if (getdata && o->group != 0)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: getData requests cannot go in a multi transaction (group %u)",
+            o->group);
+    const bool has_data = o->op != REGK_ZK_DELETE && !getdata;
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "regk_jute_requests: batches are still in flight; finish them first");
     if (!ctx->last_path_off || (has_data && (!ctx->last_json_off || ctx->last_n != ctx->last_json_n)))
@@ -2471,7 +2505,14 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
             has_data ? "both a path and a payload stream" : "a path stream");
     const FrameSrc src{ctx->last_n, ctx->last_path_bytes, ctx->last_path_off, has_data ? ctx->last_json_bytes : nullptr,
                        has_data ? ctx->last_json_off : nullptr};
-    return frame_requests(ctx, src, o, ctx->jute_bytes, ctx->jute_off, ctx->h_jute_bytes, ctx->h_jute_off, out);
+    const int rc = frame_requests(ctx, src, o, ctx->jute_bytes, ctx->jute_off, ctx->h_jute_bytes, ctx->h_jute_off, out);
+    if (rc == REGK_OK && getdata) {
+        ctx->gd_valid = true;
+        ctx->gd_gen = ctx->last_gen;
+        ctx->gd_xid = o->xid_base;
+        ctx->gd_n = ctx->last_n;
+    }
+    return rc;
 }
 
 int regk_decode(regk_ctx *ctx, const regk_decode_in *in, regk_decode_out *out)
@@ -3259,6 +3300,304 @@ int regk_reconcile_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames 
     const int32_t *ver = observed ? (const int32_t *)rb[regk_ctx::RC_VER0 + v].p : nullptr;
     return frame_entry_requests(ctx, src, o, ver, replace, rb[regk_ctx::RC_FBYTES], rb[regk_ctx::RC_FOFF], ctx->h_rc_fbytes,
                                 ctx->h_rc_foff, out);
+}
+
+static const char *reply_reason(uint32_t code)
+{
+    switch (code) {
+    case RP_TRUNC: return "the stream ends inside the frame";
+    case RP_BAD_LEN: return "a frame length below 16 (no room for a ReplyHeader)";
+    case RP_NEG_XID: return "a negative xid other than -1 (notification) or -2 (ping)";
+    case RP_XID_RANGE: return "an xid outside the framed requests";
+    case RP_ERR_BODY: return "an error reply with a body";
+    case RP_SUCC_LEN: return "a success frame whose length disagrees with its data length";
+    case RP_NEG_DATA: return "a data length below -1";
+    case RP_STAT_LEN: return "Stat.dataLength differs from the data the reply carries";
+    case RP_ORDER: return "a reply out of order, or for a record that already has one";
+    default: return "internal error";
+    }
+}
+
+int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t flags, regk_replies *out)
+{
+    if (!ctx || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: NULL argument");
+    memset(out, 0, sizeof *out);
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_replies: batches are still in flight; finish them first");
+    if (!ctx->gd_valid)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_replies: no getData framing (regk_jute_requests with REGK_ZK_GETDATA) of the "
+                                         "batch finished last");
+    if (ctx->gd_gen != ctx->last_gen || !ctx->last_path_off)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_replies: a batch finished after the getData framing; frame its getData "
+                                         "requests first");
+    if (!bytes && len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: NULL stream of %llu bytes", (unsigned long long)len);
+    const bool in_dev = flags & REGK_IN_DEVICE, dev_out = flags & REGK_OUT_DEVICE;
+    if (in_dev && ((uintptr_t)bytes & 15u))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: misaligned device stream (16-byte alignment needed)");
+    const uint64_t n = ctx->gd_n;
+    const int32_t xb = ctx->gd_xid;
+    for (int32_t reserved : {-1, -2})
+        if ((uint64_t)((uint32_t)reserved - (uint32_t)xb) < n)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: the framed xids [%d, %d + %llu) cover %d, which ZooKeeper "
+                                                   "uses for %s", xb, xb, (unsigned long long)n, reserved,
+                        reserved == -1 ? "watch notifications" : "pings");
+    if (n >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: %llu records: must be below 2^32 - 1", (unsigned long long)n);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    DevBuf *rb = ctx->rq;
+    int rc;
+    for (auto &ev : ctx->rq_ev)
+        if (!ev)
+            CK(cudaEventCreate(&ev));
+    const uint8_t *ds = bytes;
+    if (!in_dev) {
+        if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_STREAM], len + 16)))
+            return rc;
+        if (len)
+            CK(cudaMemcpyAsync(rb[regk_ctx::RQ_STREAM].p, bytes, len, cudaMemcpyHostToDevice, s));
+        ds = (const uint8_t *)rb[regk_ctx::RQ_STREAM].p;
+    }
+    const uint64_t nblk = (len + 15) / 16, tiles_s = (nblk + RP_TILE - 1) / RP_TILE, tiles_r = (n + RP_TILE - 1) / RP_TILE;
+    uint64_t slots = 1024;
+    while (slots < 2 * n)
+        slots <<= 1;
+    /* two-level totals of the candidate pass (the chain and node passes get theirs once the candidates are counted) */
+    const size_t totals_bytes = align16(tiles_s * 4) + (tiles_s / SUPER + 1) * 8;
+    const size_t n8 = n * 8 + 16, n4 = n * 4 + 16;
+    if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_WORD], nblk * 4 + 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_TOTALS], totals_bytes)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_TBASE], tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_ERRA], n4)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_DPOS], n8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_DLEN], n4)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_VER], n4)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_OWN], n8)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_SLOT], n4)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_TABLE], slots * 4)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_COUNT], RQ_NCOUNTERS * 8)) || (rc = ensure_host(ctx, ctx->h_rq_count, RQ_NCOUNTERS * 8)))
+        return rc;
+    RepParams p{};
+    p.s = ds;
+    p.len = len;
+    p.xid_base = xb;
+    p.n = n;
+    p.word = (uint32_t *)rb[regk_ctx::RQ_WORD].p;
+    p.tile_total = (uint32_t *)rb[regk_ctx::RQ_TOTALS].p;
+    p.super_total = (unsigned long long *)((uint8_t *)rb[regk_ctx::RQ_TOTALS].p + align16(tiles_s * 4));
+    p.tile_base = (unsigned long long *)rb[regk_ctx::RQ_TBASE].p;
+    p.err = (int32_t *)rb[regk_ctx::RQ_ERRA].p;
+    p.data_pos = (unsigned long long *)rb[regk_ctx::RQ_DPOS].p;
+    p.dlen = (uint32_t *)rb[regk_ctx::RQ_DLEN].p;
+    p.ver = (int32_t *)rb[regk_ctx::RQ_VER].p;
+    p.own = (long long *)rb[regk_ctx::RQ_OWN].p;
+    p.slot = (uint32_t *)rb[regk_ctx::RQ_SLOT].p;
+    p.d_path = ctx->last_path_bytes;
+    p.d_path_off = ctx->last_path_off;
+    p.table = (uint32_t *)rb[regk_ctx::RQ_TABLE].p;
+    p.mask_t = (uint32_t)(slots - 1);
+    p.counters = (unsigned long long *)rb[regk_ctx::RQ_COUNT].p;
+    unsigned long long *hc = (unsigned long long *)ctx->h_rq_count.p;
+    CK(cudaMemsetAsync(p.counters, 0, RQ_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(p.counters + RQ_ERR, 0xFF, 8, s));
+    CK(cudaMemsetAsync(p.tile_total, 0, totals_bytes, s));
+    CK(cudaEventRecord(ctx->rq_ev[0], s));
+    uint32_t launches = 0;
+    /* 1. candidates: the plausible positions; their count from the CTA totals' upper level */
+    const uint64_t nsup = tiles_s / SUPER + 1;
+    std::vector<unsigned long long> sup(nsup, 0);
+    if (len) {
+        regk_replies_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(p);
+        CK(cudaGetLastError());
+        launches++;
+        CK(cudaMemcpyAsync(sup.data(), p.super_total, nsup * 8, cudaMemcpyDeviceToHost, s));
+    }
+    cudaError_t e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_CUDA, "regk_read_replies: kernel execution failed: %s", cudaGetErrorString(e));
+    uint64_t C = 0;
+    for (unsigned long long v : sup)
+        C += v;
+    if (C >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: %llu plausible frame positions in the stream: must be below "
+                                               "2^32 - 1", (unsigned long long)C);
+    /* 2. positions, successors, the jump tables J_0 .. J_K (2^(K+1) >= C), the chain from position 0 */
+    uint32_t K = 0;
+    while ((1ull << (K + 1)) < C)
+        K++;
+    const size_t tiles_c = (C + RP_TILE - 1) / RP_TILE, tiles2 = std::max<uint64_t>(tiles_c, tiles_r);
+    const size_t totals2_bytes = align16(tiles2 * 4) + (tiles2 / SUPER + 1) * 8;
+    if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_CAND], C * 8 + 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_MARK], C + 16)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_JUMP], (size_t)(K + 1) * C * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_TOTALS2], totals2_bytes)))
+        return rc;
+    p.cand = (unsigned long long *)rb[regk_ctx::RQ_CAND].p;
+    p.marked = (uint8_t *)rb[regk_ctx::RQ_MARK].p;
+    p.C = C;
+    uint32_t *J = (uint32_t *)rb[regk_ctx::RQ_JUMP].p;
+    RepParams p2 = p;                                   /* the chain and node passes' totals */
+    p2.tile_total = (uint32_t *)rb[regk_ctx::RQ_TOTALS2].p;
+    p2.super_total = (unsigned long long *)((uint8_t *)rb[regk_ctx::RQ_TOTALS2].p + align16(tiles2 * 4));
+    const unsigned g256 = (unsigned)((C + 255) / 256);
+    if (C) {
+        regk_replies_compact_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(p);
+        regk_replies_succ_kernel<<<g256, 256, 0, s>>>(p, J);
+        for (uint32_t l = 0; l < K; l++)
+            regk_replies_jump_kernel<<<g256, 256, 0, s>>>(J + (size_t)l * C, J + (size_t)(l + 1) * C, C);
+        CK(cudaMemsetAsync(p.marked, 0, C, s));
+        for (uint32_t l = K + 1; l-- > 0;)
+            regk_replies_mark_kernel<<<g256, 256, 0, s>>>(p, J + (size_t)l * C, l == K ? 1u : 0u);
+        /* 3. the chain's replies: k, the full check, the per-record arrays */
+        CK(cudaMemsetAsync(p2.tile_total, 0, totals2_bytes, s));
+        regk_replies_chain_count_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(p2);
+        regk_replies_chain_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(p2);
+        CK(cudaGetLastError());
+        launches += 2 * K + 6;
+    }
+    CK(cudaMemcpyAsync(hc, p.counters, RQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_CUDA, "regk_read_replies: kernel execution failed: %s", cudaGetErrorString(e));
+    if (hc[RQ_ERR] != ~0ull) {
+        /* the smallest record whose frame fails the full check; the frame starts 24 bytes before its data */
+        const uint64_t k = hc[RQ_ERR] >> 8;
+        const uint32_t code = (uint32_t)(hc[RQ_ERR] & 0xFF);
+        unsigned long long dpos = 0;
+        CK(cudaMemcpyAsync(&dpos, p.data_pos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        const uint64_t pos = dpos - 24;
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: byte %llu: %s; expected the reply to record %llu (xid %d)",
+            (unsigned long long)pos, reply_reason(code), (unsigned long long)k, (int32_t)((uint32_t)xb + (uint32_t)k));
+    }
+    if (hc[RQ_NREP] < n) {
+        /* the chain stops before the n-th reply: the full check where it stops names the reason */
+        uint64_t stop = 0;
+        if (C) {
+            regk_replies_stop_kernel<<<g256, 256, 0, s>>>(p);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(hc + RQ_STOP, p.counters + RQ_STOP, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            stop = hc[RQ_STOP];
+        }
+        const uint64_t done = hc[RQ_NREP];
+        uint8_t head[24] = {0};
+        const uint64_t avail = len - stop, take = std::min<uint64_t>(avail, sizeof head);
+        if (take) {
+            CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+        }
+        ReplyHead h;
+        const uint32_t code = reply_head(head, avail, xb, n, &h);
+        const int32_t want = (int32_t)((uint32_t)xb + (uint32_t)done);
+        if (code == RP_TRUNC)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: byte %llu: the stream ends before the reply to record %llu "
+                                                   "(xid %d) is complete; %llu of %llu replies complete", (unsigned long long)stop,
+                        (unsigned long long)done, want, (unsigned long long)done, (unsigned long long)n);
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: byte %llu: %s (len %d, xid %d); expected the reply to record "
+                                               "%llu (xid %d)", (unsigned long long)stop, code ? reply_reason(code) : "internal error",
+                    h.len, h.xid, (unsigned long long)done, want);
+    }
+    /* 4. the nodes: found records, one per distinct path, in record order */
+    if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_NREC], n8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_NVER], n4)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_NOWN], n8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_NPLEN], n4)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_NDLEN], n4)))
+        return rc;
+    p.node_rec = (unsigned long long *)rb[regk_ctx::RQ_NREC].p;
+    p.node_ver = (int32_t *)rb[regk_ctx::RQ_NVER].p;
+    p.node_own = (long long *)rb[regk_ctx::RQ_NOWN].p;
+    p.node_plen = (uint32_t *)rb[regk_ctx::RQ_NPLEN].p;
+    p.node_dlen = (uint32_t *)rb[regk_ctx::RQ_NDLEN].p;
+    p.tile_total = p2.tile_total;
+    p.super_total = p2.super_total;
+    CK(cudaMemsetAsync(p.table, 0, slots * 4, s));
+    CK(cudaMemsetAsync(p.tile_total, 0, totals2_bytes, s));
+    regk_replies_insert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p);
+    regk_replies_node_count_kernel<<<(unsigned)tiles_r, RP_TILE, 0, s>>>(p);
+    regk_replies_node_kernel<<<(unsigned)tiles_r, RP_TILE, 0, s>>>(p);
+    CK(cudaGetLastError());
+    launches += 3;
+    CK(cudaMemcpyAsync(hc, p.counters, RQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_CUDA, "regk_read_replies: kernel execution failed: %s", cudaGetErrorString(e));
+    const uint64_t m = hc[RQ_M];
+    /* 5. the snapshot's streams: node paths from the batch, node data from the reply stream */
+    const uint64_t gt = (m + MK_TILE - 1) / MK_TILE;
+    if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_GTOT], gt * 8 + (gt / SUPER + 1) * 8 + 16)) ||
+        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_PO], (m + 1) * 8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_JO], (m + 1) * 8)))
+        return rc;
+    uint64_t totals[2] = {0, 0};
+    for (int g = 0; g < 2; g++) {
+        DevBuf &gb = rb[g ? regk_ctx::RQ_JB : regk_ctx::RQ_PB], &go = rb[g ? regk_ctx::RQ_JO : regk_ctx::RQ_PO];
+        MkGatherParams gp{};
+        gp.n_dirs = m;
+        gp.path_bytes = g ? ds : ctx->last_path_bytes;
+        gp.path_off = g ? p.data_pos : ctx->last_path_off;
+        gp.dir_rec = p.node_rec;
+        gp.dir_len = g ? p.node_dlen : p.node_plen;
+        gp.tile_total = (unsigned long long *)rb[regk_ctx::RQ_GTOT].p;
+        gp.super_total = gp.tile_total + gt;
+        gp.dir_off = (unsigned long long *)go.p;
+        if (!m) {
+            if ((rc = ensure_dev(ctx, gb, 16)))
+                return rc;
+            CK(cudaMemsetAsync(go.p, 0, 8, s));
+            continue;
+        }
+        CK(cudaMemsetAsync(gp.super_total, 0, (gt / SUPER + 1) * 8, s));
+        regk_mkdirp_len_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(gp);
+        /* the stream's size: the sum of the upper level of the totals */
+        std::vector<unsigned long long> gs(gt / SUPER + 1);
+        CK(cudaMemcpyAsync(gs.data(), gp.super_total, gs.size() * 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        for (unsigned long long v : gs)
+            totals[g] += v;
+        if ((rc = ensure_dev(ctx, gb, totals[g] + 16)))
+            return rc;
+        gp.dir_bytes = (uint8_t *)gb.p;
+        regk_mkdirp_gather_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(gp);
+        CK(cudaGetLastError());
+        launches += 2;
+    }
+    CK(cudaEventRecord(ctx->rq_ev[1], s));
+    e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_CUDA, "regk_read_replies: kernel execution failed: %s", cudaGetErrorString(e));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, ctx->rq_ev[0], ctx->rq_ev[1]);
+    const int32_t *err_out = p.err;
+    const uint64_t *rec_out = (const uint64_t *)p.node_rec;
+    if (!dev_out) {
+        if ((rc = ensure_host(ctx, ctx->h_rq_err, n * 4 + 16)) || (rc = ensure_host(ctx, ctx->h_rq_node, m * 8 + 16)))
+            return rc;
+        if (n)
+            CK(cudaMemcpyAsync(ctx->h_rq_err.p, p.err, n * 4, cudaMemcpyDeviceToHost, s));
+        if (m)
+            CK(cudaMemcpyAsync(ctx->h_rq_node.p, p.node_rec, m * 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        err_out = (const int32_t *)ctx->h_rq_err.p;
+        rec_out = (const uint64_t *)ctx->h_rq_node.p;
+    }
+    out->n = n;
+    out->m = m;
+    out->n_found = hc[RQ_FOUND];
+    out->n_missing = hc[RQ_MISSING];
+    out->n_error = hc[RQ_ERROR];
+    out->n_skipped = hc[RQ_SKIP];
+    out->consumed = hc[RQ_CONSUMED];
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->err = err_out;
+    out->node_rec = rec_out;
+    out->snapshot.n = m;
+    out->snapshot.flags = REGK_IN_DEVICE;
+    out->snapshot.path_total = totals[0];
+    out->snapshot.json_total = totals[1];
+    out->snapshot.path_bytes = (const uint8_t *)rb[regk_ctx::RQ_PB].p;
+    out->snapshot.path_off = (const uint64_t *)rb[regk_ctx::RQ_PO].p;
+    out->snapshot.json_bytes = (const uint8_t *)rb[regk_ctx::RQ_JB].p;
+    out->snapshot.json_off = (const uint64_t *)rb[regk_ctx::RQ_JO].p;
+    out->version = p.node_ver;
+    out->ephemeral_owner = (const int64_t *)p.node_own;
+    out->kernel_ms = ms;
+    return REGK_OK;
 }
 
 int regk_release(regk_ctx *ctx, regk_result *res)
