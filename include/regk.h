@@ -168,8 +168,15 @@ int         regk_set_stream(regk_ctx *ctx, void *cuda_stream);
  * Record-type table (registration.type values).  Strings are arbitrary UTF-8;
  * JSON escaping (ECMA-262 QuoteJSONString) is applied here, on the host, once.
  * Rejected (REGK_ERR_OUT_OF_DOMAIN): "type", "address", "ttl" (the dynamic key
- * would overwrite a fixed one, register.js:152) and canonical array-index
- * strings ("0", "42": V8 orders integer keys first).
+ * would overwrite a fixed one, register.js:152), "__proto__", canonical
+ * array-index strings ("0", "42": V8 orders integer keys first), and bytes
+ * that are not well-formed UTF-8 (overlong forms, encoded surrogates, code
+ * points above U+10FFFF, truncated sequences, stray continuation bytes): no JS
+ * string has such a UTF-8 form, so the reference could never write them.
+ * Rejected (REGK_ERR_INVALID_ARG): more than 255 types, or a fragment table
+ * over 16 KB (each type takes eight copies of its escaped name plus about 200
+ * bytes: one name of up to about 2000 escaped bytes, or about 80 short names).
+ * A rejected call leaves the previous table in force.
  */
 int         regk_set_types(regk_ctx *ctx, const char *const *types, const uint32_t *lens, uint32_t ntypes);
 

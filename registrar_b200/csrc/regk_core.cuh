@@ -958,8 +958,8 @@ RG_HD void put_frag(const Src &blob, uint32_t off, uint32_t len, Sink &sink)
 
 /*
  * word sink: copy from the variant that matches the sink's byte phase.
- * OVERSHOOT = true copies a fixed MAXW words with no loop and no bounds (garbage lands in the next <= 16
- * bytes, which the caller guarantees belong to the same record and are written later);
+ * OVERSHOOT = true copies a fixed MAXW words with no loop and no bounds (garbage lands in the next
+ * 4 * MAXW - phase - len bytes, which the caller guarantees belong to the same record and are written later);
  * OVERSHOOT = false stores exactly the completed words.
  */
 template <bool OVERSHOOT, uint32_t MAXW, class Src>
@@ -1040,8 +1040,9 @@ RG_HD void put_frag(const Src &blob, uint32_t off, uint32_t len, WordSink &sink)
         put_frag_w<false, 1>(blob, off, len, sink);
 }
 
-/* The opening fragment {"type":"T","address":" : at least 24 more bytes of the record always follow it
- * (address, quote, second fragment, address, "}}), so up to 37 bytes it is copied as 10 unconditional words. */
+/* The opening fragment {"type":"T","address":" : at least 22 more bytes of the record always follow it
+ * (address, quote, second fragment, address, "}}), so up to 37 bytes it is copied as 10 unconditional words;
+ * their overshoot is largest, 40 - 22 = 18 bytes, for the empty type name at byte phase 0. */
 template <class Src, class Sink>
 RG_HD void put_frag_first(const Src &blob, uint32_t off, uint32_t len, Sink &sink)
 {

@@ -66,6 +66,47 @@ inline bool is_array_index(const std::string &s)
     return v < 4294967295ull;
 }
 
+/* Well-formed UTF-8 (Unicode table 3-7): no overlong form, no encoded surrogate D800-DFFF, nothing above
+   U+10FFFF, no truncated sequence and no stray continuation byte.  Only such bytes are the UTF-8 form of a JS
+   string, so only they can be a type the reference writes; the composers copy bytes >= 0x80 unchanged. */
+inline bool utf8_well_formed(const std::string &s)
+{
+    const size_t n = s.size();
+    size_t i = 0;
+    while (i < n) {
+        const unsigned c = (unsigned char)s[i];
+        if (c < 0x80) {
+            i++;
+            continue;
+        }
+        size_t len;
+        unsigned lo = 0x80, hi = 0xBF;                      /* range of the second byte */
+        if (c >= 0xC2 && c <= 0xDF) {
+            len = 2;
+        } else if (c >= 0xE0 && c <= 0xEF) {
+            len = 3;
+            lo = c == 0xE0 ? 0xA0 : 0x80;                   /* E0 80..9F: overlong */
+            hi = c == 0xED ? 0x9F : 0xBF;                   /* ED A0..BF: surrogates */
+        } else if (c >= 0xF0 && c <= 0xF4) {
+            len = 4;
+            lo = c == 0xF0 ? 0x90 : 0x80;                   /* F0 80..8F: overlong */
+            hi = c == 0xF4 ? 0x8F : 0xBF;                   /* F4 90..BF: above U+10FFFF */
+        } else {
+            return false;                                   /* continuation byte, C0 / C1, F5..FF */
+        }
+        if (n - i < len)
+            return false;
+        const unsigned c1 = (unsigned char)s[i + 1];
+        if (c1 < lo || c1 > hi)
+            return false;
+        for (size_t k = 2; k < len; k++)
+            if (((unsigned char)s[i + k] & 0xC0) != 0x80)
+                return false;
+        i += len;
+    }
+    return true;
+}
+
 constexpr size_t TYPE_BLOB_MAX = 16384;
 
 /* Returns 0 on success, 1 = out-of-domain type name, 2 = table too large; *err gets the reason. */
@@ -84,6 +125,10 @@ inline int build_type_blob(const std::vector<std::string> &types, std::vector<ui
            object's prototype instead of creating an own property, so JSON.stringify drops the nested object. */
         if (t == "type" || t == "address" || t == "ttl" || t == "__proto__" || is_array_index(t)) {
             *err = "type '" + t + "' collides with a fixed key, is an array index or is __proto__";
+            return 1;
+        }
+        if (!utf8_well_formed(t)) {
+            *err = "type " + std::to_string(i) + " is not well-formed UTF-8";
             return 1;
         }
         const std::string q = json_escape(t);
