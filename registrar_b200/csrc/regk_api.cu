@@ -15,8 +15,10 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/regk.h"
@@ -39,27 +41,76 @@ namespace {
 
 thread_local std::string g_create_error;
 
-struct DevBuf {
+/* Memory the context owns (ensure_dev / ensure_host grow it), freed with its owner. */
+template <cudaError_t (*Free)(void *)>
+struct Buf {
     void *p = nullptr;
     size_t cap = 0;
+    Buf() = default;
+    Buf(Buf &&o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    Buf &operator=(Buf &&o) noexcept
+    {
+        std::swap(p, o.p);
+        std::swap(cap, o.cap);
+        return *this;
+    }
+    ~Buf() { release(); }
+    cudaError_t release()
+    {
+        const cudaError_t e = p ? Free(p) : cudaSuccess;
+        p = nullptr;
+        cap = 0;
+        return e;
+    }
+};
+using DevBuf = Buf<cudaFree>;
+using HostBuf = Buf<cudaFreeHost>;
+
+/* A CUDA event or stream the context owns, created on first use (ensure_event / ensure_stream). */
+template <typename T, cudaError_t (*Destroy)(T)>
+struct Handle {
+    T h = nullptr;
+    Handle() = default;
+    Handle(Handle &&o) noexcept : h(std::exchange(o.h, nullptr)) {}
+    Handle &operator=(Handle &&o) noexcept
+    {
+        std::swap(h, o.h);
+        return *this;
+    }
+    ~Handle()
+    {
+        if (h)
+            Destroy(h);
+    }
+    operator T() const { return h; }
+};
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+
+/* Request frames and their offsets, on the device and in pinned host memory (regk_frames). */
+struct FrameBufs {
+    DevBuf bytes, off;
+    HostBuf h_bytes, h_off;
 };
 
-struct HostBuf {
-    void *p = nullptr;
-    size_t cap = 0;
+/* A parent pass (regk_parents.cuh): parent length and table slot per record, the table, tile totals, the distinct
+   parents and their count. */
+struct ParentPass {
+    DevBuf len, slot, table, totals, unique;
 };
 
 }  // namespace
 
 struct regk_ctx {
+    ~regk_ctx();
     int device = 0;
-    cudaStream_t own_stream = nullptr;
-    cudaStream_t stream = nullptr;              /* the stream work is enqueued on */
+    Stream own_stream;
+    cudaStream_t stream = nullptr;              /* the stream work is enqueued on: own_stream or the caller's */
     std::string err;
     int sm_count = 0;
     int max_smem_optin = 0;
-    /* compose kernels' L2 lookahead: CTAs of one wave by dynamic shared memory (lookahead_tiles); index as in
-       smem_attr_needs_raise (0 alias paths, 1 node paths, 2 payloads) */
+    /* compose kernels' L2 lookahead: CTAs of one wave by dynamic shared memory (lookahead_tiles); 0 alias paths,
+       1 node paths, 2 payloads */
     std::map<size_t, uint32_t> wave_ctas[3];
 
     /* type table */
@@ -68,24 +119,23 @@ struct regk_ctx {
     DevBuf blob_dev;
     uint32_t max_type_q = 0;                    /* longest escaped type */
 
-    /* device staging of host batches */
-    DevBuf in[11];
-    /* outputs */
-    DevBuf path_bytes, path_off, json_bytes, json_off, off32_p, off32_j;
-    HostBuf h_path_bytes, h_path_off, h_json_bytes, h_json_off, h_running;
-    cudaStream_t s_h2d = nullptr, s_d2h = nullptr;          /* host pipelining (run_pipelined, two-deep async) */
-    /* "async" host batches alternate between two complete sets of staging, device outputs and pinned result
-       buffers: batch k+1's H2D and kernels overlap batch k's D2H (issued when k+1 is submitted or k is
-       finished, whichever comes first - the copy sizes are only known once k's kernels are done) */
+    /* A batch's device staging of host inputs, device outputs and pinned results.  sync_set serves every batch but
+       "async" host batches (a job step uses none of it: its inputs and outputs are the caller's); the skip-mode redo
+       and regk_service_records write into its device outputs too.  "async" host batches alternate between the two of hset: batch
+       k+1's H2D and kernels overlap batch k's D2H (issued when k+1 is submitted or k is finished, whichever comes
+       first - the copy sizes are only known once k's kernels are done). */
     struct HostSet {
         DevBuf in[11];
         DevBuf path_bytes, path_off, json_bytes, json_off, off32_p, off32_j;
         HostBuf h_path_bytes, h_path_off, h_json_bytes, h_json_off;
-        cudaEvent_t e_in = nullptr, e_out = nullptr;
+        Event e_in, e_out;                      /* async sets: staging copied in, results copied out */
     };
-    HostSet hset[2];
+    HostSet sync_set, hset[2];
     uint64_t hseq = 0;
-    uint32_t *h_gather_flag = nullptr;          /* pinned: 1 = regk_gather_push found the whole-job buffers too small,
+    bool is_async(const HostSet *hs) const { return hs != &sync_set; }
+    HostBuf h_running;                          /* run_pipelined: each chunk's running payload total */
+    Stream s_h2d, s_d2h;                        /* host pipelining (run_pipelined, two-deep async) */
+    HostBuf h_gather_flag;                      /* uint32: 1 = regk_gather_push found the whole-job buffers too small,
                                                    2 = a peer exchange of a job step timed out */
     /* multi-GPU job (regk_job_bind): description, exchange sequence number, per-slot bases {path base, path all,
        rec base, n all, payload base, payload all, -, -} on the device and their pinned host copies */
@@ -97,92 +147,111 @@ struct regk_ctx {
     bool job_bound = false;
     unsigned long long job_seq = 0;
     DevBuf job_bases;
-    unsigned long long *h_job_bases = nullptr;
-    /* device copy of the path stream of the batch finished last (regk_parent_dirs works on it) */
-    const uint8_t *last_path_bytes = nullptr;
-    const unsigned long long *last_path_off = nullptr;
-    uint64_t last_n = 0;
-    /* ... and of its payload stream (regk_jute_frames / regk_decode work on both) */
-    const uint8_t *last_json_bytes = nullptr;
-    const unsigned long long *last_json_off = nullptr;
-    uint64_t last_json_n = 0;
-    DevBuf jute_bytes, jute_off;
-    HostBuf h_jute_bytes, h_jute_off;
-    DevBuf dec_in[4], dec_rec, dec_dom, dec_ports;
-    HostBuf h_dec_rec, h_dec_dom, h_dec_ports;
-    const uint32_t *last_host_off = nullptr;
-    uint32_t last_host_stride = 0;
-    bool last_alias = false;
-    DevBuf svc_in[7], svc_work;                 /* regk_service_records: staged inputs, status + tile totals */
-    DevBuf par_len, par_slot, par_table, par_totals, par_unique;
-    cudaEvent_t par_ev[2] = {nullptr, nullptr};
-    HostBuf h_par_len, h_par_unique, h_par_count;
+    HostBuf h_job_bases;                        /* pinned copies of job_bases, NSLOTS * 8 entries */
+    /* the device streams of the batch finished last: regk_parent_dirs, regk_mkdirp_dirs, regk_jute_requests,
+       regk_decode, the reconcile calls and regk_read_replies work on them; written by set_last only */
+    struct LastBatch {
+        const uint8_t *path_bytes = nullptr;
+        const unsigned long long *path_off = nullptr;
+        uint64_t n = 0;                         /* records of the path stream, 0 without one */
+        const uint8_t *json_bytes = nullptr;
+        const unsigned long long *json_off = nullptr;
+        uint64_t json_n = 0;                    /* ... and of the payload stream */
+        const uint32_t *host_off = nullptr;     /* how its paths end: hostname lengths (NULL: fixed stride) */
+        uint32_t host_stride = 0;
+        bool alias = false;
+        uint64_t gen = 0;                       /* bumped whenever the fields above change */
+    } last;
+    FrameBufs frames;                           /* regk_jute_requests */
+    /* regk_decode: staged streams, records, domain image and ports */
+    struct Decode {
+        DevBuf in[4], rec, dom, ports;
+        HostBuf h_rec, h_dom, h_ports;
+    } dec;
+    /* regk_service_records: staged inputs, status + tile totals (the framing calls borrow it for their status) */
+    struct Service {
+        DevBuf in[7], work;
+    } svc;
+    /* regk_parent_dirs */
+    struct Parents {
+        ParentPass pass;
+        HostBuf h_len, h_unique, h_count;
+        Event ev[2];
+    } par;
     /* regk_mkdirp_dirs (regk_mkdirp.cuh): its own parent pass, work lists, table, the set; regk_mkdirp_requests */
-    enum { MK_PLEN, MK_PSLOT, MK_PTABLE, MK_PTOTALS, MK_PUNIQUE, MK_FLAGS, MK_LIST0, MK_LIST1, MK_TOTALS, MK_TABLE,
-           MK_COUNT, MK_DREC, MK_DLEN, MK_DBYTES, MK_DOFF, MK_DEPTH, MK_INVALID, MK_ZERO, MK_FBYTES, MK_FOFF, MK_NBUF };
-    DevBuf mk[MK_NBUF];
-    HostBuf h_mk_count, h_mk_drec, h_mk_dlen, h_mk_dbytes, h_mk_doff, h_mk_depth, h_mk_invalid, h_mk_fbytes, h_mk_foff;
-    cudaEvent_t mk_ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    bool mk_valid = false;                      /* the set of the last regk_mkdirp_dirs call is in mk[MK_D*] */
-    uint64_t mk_n_dirs = 0, mk_bytes = 0;
+    struct Mkdirp {
+        ParentPass pass;
+        DevBuf flags, list[2], totals, table, count, drec, dlen, dbytes, doff, depth, invalid, zero;
+        HostBuf h_count, h_drec, h_dlen, h_dbytes, h_doff, h_depth, h_invalid;
+        Event ev[4];
+        FrameBufs frames;
+        bool valid = false;                     /* the set of the last regk_mkdirp_dirs call is in drec .. invalid */
+        uint64_t n_dirs = 0, bytes = 0;
+    } mk;
     /* regk_reconcile / regk_reconcile_owned (regk_reconcile.cuh): staged snapshot and stats, tables, outputs, lists,
        versions, the gathered request streams; regk_reconcile_requests' frames */
-    enum { RC_IN_PB, RC_IN_PO, RC_IN_JB, RC_IN_JO, RC_IN_VER, RC_IN_OWN, RC_TOBS, RC_TDES, RC_SLOTO, RC_HASHO, RC_SLOTD, RC_CLS,
-           RC_MATCH, RC_OBSCLS, RC_TOTALS, RC_LIST0, RC_LEN0 = RC_LIST0 + RC_NLISTS, RC_VER0 = RC_LEN0 + RC_NGATHERS,
-           RC_COUNT = RC_VER0 + RC_NVER, RC_GTOTALS, RC_G0B, RC_FBYTES = RC_G0B + 2 * RC_NGATHERS, RC_FOFF, RC_NBUF };
-    DevBuf rc[RC_NBUF];
-    HostBuf h_rc_count, h_rc_cls, h_rc_match, h_rc_obscls, h_rc_list[RC_NLISTS], h_rc_fbytes, h_rc_foff;
-    cudaEvent_t rc_ev[2] = {nullptr, nullptr};
-    bool rc_valid = false;                      /* the request streams of the last reconcile call are in rc[RC_G0B + 2 k] */
-    bool rc_owned = false;                      /* ... and it was regk_reconcile_owned: versions in rc[RC_VER*] */
-    uint32_t rc_zk_flags = 0;                   /* the CreateMode regk_reconcile_owned classified with */
-    uint64_t rc_count[RC_NLISTS] = {};          /* create, update, dup, replace, delete */
-    /* which batch finished last: bumped whenever the streams of the batch finished last change */
-    uint64_t last_gen = 0;
+    struct Reconcile {
+        DevBuf in[6];                           /* path bytes, path offsets, data bytes, data offsets, versions, owners */
+        DevBuf t_obs, t_des, slot_obs, hash_obs, slot_des, cls, match, obs_cls, totals, count, gtotals;
+        DevBuf list[RC_NLISTS], len[RC_NGATHERS], ver[RC_NVER];
+        struct {
+            DevBuf bytes, off;
+        } gather[RC_NGATHERS];
+        HostBuf h_count, h_cls, h_match, h_obs_cls, h_list[RC_NLISTS];
+        Event ev[2];
+        FrameBufs frames;
+        bool valid = false;                     /* the request streams of the last reconcile call are in gather */
+        bool owned = false;                     /* ... and it was regk_reconcile_owned: versions in ver */
+        uint32_t zk_flags = 0;                  /* the CreateMode regk_reconcile_owned classified with */
+        uint64_t n_list[RC_NLISTS] = {};        /* entries of each list: create, update, dup, replace, delete */
+    } rc;
     /* the last REGK_ZK_GETDATA framing: the batch it framed, xid_base, n (regk_read_replies reads its replies) */
     bool gd_valid = false;
     uint64_t gd_gen = 0, gd_n = 0;
     int32_t gd_xid = 0;
     /* regk_read_replies (regk_replies.cuh): staged stream, candidates, jump tables, per-record arrays, table, the nodes
        and the gathered snapshot */
-    enum { RQ_STREAM, RQ_WORD, RQ_TOTALS, RQ_TOTALS2, RQ_TBASE, RQ_CAND, RQ_MARK, RQ_JUMP, RQ_ERRA, RQ_DPOS, RQ_DLEN, RQ_VER, RQ_OWN,
-           RQ_SLOT, RQ_TABLE, RQ_NREC, RQ_NVER, RQ_NOWN, RQ_NPLEN, RQ_NDLEN, RQ_GTOT, RQ_PB, RQ_PO, RQ_JB, RQ_JO, RQ_COUNT,
-           RQ_NBUF };
-    DevBuf rq[RQ_NBUF];
-    HostBuf h_rq_count, h_rq_err, h_rq_node;
-    cudaEvent_t rq_ev[2] = {nullptr, nullptr};
-    std::vector<cudaEvent_t> pipe_events;
+    struct Replies {
+        DevBuf stream, word, totals, totals2, tile_base, cand, mark, jump, err, data_pos, dlen, ver, own, slot, table;
+        DevBuf node_rec, node_ver, node_own, node_plen, node_dlen, gtotals, count;
+        DevBuf snap_bytes[2], snap_off[2];      /* the snapshot's path and data streams */
+        HostBuf h_count, h_err, h_node;
+        Event ev[2];
+    } rq;
+    std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
-    DevBuf skip_work, skip_in[11], skip_off_p, skip_off_j, skip_index, skip_bits;
-    HostBuf h_skip_status, h_skip_index, h_skip_bits;
-    struct SkipLast {
-        bool valid = false;                     /* the batch finished last was a skip-mode batch */
-        uint64_t n = 0, n_skipped = 0;
-        uint32_t bad_bits = 0;
-    } skip_last;
+    struct Skip {
+        DevBuf work, in[11], off_p, off_j, index, bits;
+        HostBuf h_status, h_index, h_bits;
+        struct Last {
+            bool valid = false;                 /* the batch finished last was a skip-mode batch */
+            uint64_t n = 0, n_skipped = 0;
+            uint32_t bad_bits = 0;
+        } last;
+    } skip;
     /* workspace: DevStatus | two-level byte totals of both halves (stream-ordered reuse; host pipelining) */
     DevBuf work;
     /* device-resident batches rotate through a ring of workspaces that a side stream re-zeroes (and copies
        the status out of) after each use, so the main stream carries nothing but the two kernels */
     static constexpr int NWORK = 4;
     DevBuf work_ring[NWORK];
-    cudaEvent_t ws_clean[NWORK] = {nullptr, nullptr, nullptr, nullptr};
+    Event ws_clean[NWORK];
     size_t ws_clean_bytes[NWORK] = {0, 0, 0, 0};
-    cudaStream_t s_side = nullptr;
+    Stream s_side;
     uint64_t ws_seq = 0;
 
     /* in-flight batches: events + pinned status per slot.  Outputs are single-buffered: with the
        "async" option several batches may be enqueued back to back (benchmark loops), each one
        overwriting the previous batch's outputs in stream order. */
     struct Slot {
-        cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};     /* [5]: after a job step's closing exchange */
+        Event ev[6];                            /* [5]: after a job step's closing exchange */
         PathParams path_params{};               /* kept for the exact-offset redo (empty labels) */
         size_t path_smem = 0;
         bool path_alias = false, did_path = false;
         DevStatus *d_status = nullptr;
         DevStatus *h_status = nullptr;          /* pinned */
         int ring = -1;                          /* workspace ring entry used by this batch */
-        int hset = -1;                          /* async host batch: which HostSet it lives in */
+        HostSet *set = nullptr;                 /* where its staging, outputs and host results live */
         bool d2h_issued = false;
         bool timed = true;                      /* ev[0..2] were recorded for this batch */
         const uint8_t *dev_path_bytes = nullptr;        /* where this batch's path stream lives on the device */
@@ -207,12 +276,23 @@ struct regk_ctx {
     };
     static constexpr int NSLOTS = 64;
     Slot slots[NSLOTS];
-    DevStatus *h_status_block = nullptr;        /* pinned, NSLOTS entries */
+    HostBuf h_status_block;                     /* DevStatus[NSLOTS] */
     uint64_t seq = 0;
     int pending = 0;
 
     std::map<std::string, int64_t> opt;
 };
+
+/* Work still enqueued on the context's streams may use its memory: wait for it before the members go.  Errors are
+   ignored - this also runs at interpreter exit, while the CUDA runtime unloads.  A caller's stream is waited for,
+   never destroyed. */
+regk_ctx::~regk_ctx()
+{
+    cudaSetDevice(device);
+    for (cudaStream_t s : {stream, (cudaStream_t)s_h2d, (cudaStream_t)s_d2h, (cudaStream_t)s_side})
+        if (s)
+            cudaStreamSynchronize(s);
+}
 
 namespace {
 
@@ -243,10 +323,7 @@ int ensure_dev(regk_ctx *ctx, DevBuf &b, size_t bytes)
     bytes = (bytes + 255) & ~(size_t)255;
     if (bytes <= b.cap)
         return REGK_OK;
-    if (b.p)
-        CK(cudaFree(b.p));
-    b.p = nullptr;
-    b.cap = 0;
+    CK(b.release());
     size_t want = bytes + bytes / 8;            /* a little slack so slowly growing batches do not thrash */
     cudaError_t e = cudaMalloc(&b.p, want);
     if (e != cudaSuccess) {
@@ -265,14 +342,56 @@ int ensure_host(regk_ctx *ctx, HostBuf &b, size_t bytes)
     bytes = (bytes + 4095) & ~(size_t)4095;
     if (bytes <= b.cap)
         return REGK_OK;
-    if (b.p)
-        CK(cudaFreeHost(b.p));
-    b.p = nullptr;
-    b.cap = 0;
+    CK(b.release());
     cudaError_t e = cudaMallocHost(&b.p, bytes);
     if (e != cudaSuccess)
         return fail(ctx, REGK_ERR_NOMEM, "cudaMallocHost(%zu) failed: %s", bytes, cudaGetErrorString(e));
     b.cap = bytes;
+    return REGK_OK;
+}
+
+int ensure_event(regk_ctx *ctx, Event &ev, unsigned flags = cudaEventDefault)
+{
+    if (!ev.h)
+        CK(cudaEventCreateWithFlags(&ev.h, flags));
+    return REGK_OK;
+}
+
+int ensure_stream(regk_ctx *ctx, Stream &s)
+{
+    if (!s.h)
+        CK(cudaStreamCreateWithFlags(&s.h, cudaStreamNonBlocking));
+    return REGK_OK;
+}
+
+/* `bytes` of a host array into `b` (grown to bytes + 16), enqueued on s */
+int stage_in(regk_ctx *ctx, DevBuf &b, const void *host, size_t bytes, cudaStream_t s)
+{
+    const int rc = ensure_dev(ctx, b, bytes + 16);
+    if (rc)
+        return rc;
+    if (bytes)
+        CK(cudaMemcpyAsync(b.p, host, bytes, cudaMemcpyHostToDevice, s));
+    return REGK_OK;
+}
+
+/* `bytes` of device memory into the pinned buffer `b` (grown to bytes + 16), enqueued on s */
+int to_host(regk_ctx *ctx, HostBuf &b, const void *dev, size_t bytes, cudaStream_t s)
+{
+    const int rc = ensure_host(ctx, b, bytes + 16);
+    if (rc)
+        return rc;
+    if (bytes)
+        CK(cudaMemcpyAsync(b.p, dev, bytes, cudaMemcpyDeviceToHost, s));
+    return REGK_OK;
+}
+
+/* wait for the work enqueued on s; a fault fails the call as "<who>: kernel execution failed" */
+int sync_or_fail(regk_ctx *ctx, cudaStream_t s, const char *who)
+{
+    const cudaError_t e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_CUDA, "%s: kernel execution failed: %s", who, cudaGetErrorString(e));
     return REGK_OK;
 }
 
@@ -287,18 +406,38 @@ size_t align16(size_t v)
     return (v + 15) & ~(size_t)15;
 }
 
-/* cudaFuncAttributeMaxDynamicSharedMemorySize is per function and device, shared by every context of the
-   process: raise it monotonically and remember the high-water mark (which: 0 alias paths, 1 node paths, 2 payloads) */
-bool smem_attr_needs_raise(int device, int which, size_t bytes)
+/* cudaFuncAttributeMaxDynamicSharedMemorySize is per function and device, shared by every context of the process:
+   raise it monotonically, and only when it grows (setting it is not free) */
+int set_smem_limit(regk_ctx *ctx, const void *kernel, size_t bytes)
 {
     static std::mutex mu;
-    static size_t high[64][4];
+    static std::map<std::pair<int, const void *>, size_t> high;
     std::lock_guard<std::mutex> lock(mu);
-    size_t &h = high[device & 63][which];
+    size_t &h = high[{ctx->device, kernel}];
     if (bytes <= h)
-        return false;
+        return REGK_OK;
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     h = bytes;
-    return true;
+    return REGK_OK;
+}
+
+/* The batch finished last is now the one whose device streams are given (NULL: not produced); n is its size. */
+void set_last(regk_ctx *ctx, const uint8_t *path_bytes, const unsigned long long *path_off, const uint8_t *json_bytes,
+    const unsigned long long *json_off, uint64_t n, const uint32_t *host_off, uint32_t host_stride, bool alias)
+{
+    ctx->last = {path_bytes, path_off, path_off ? n : 0, json_bytes, json_off, json_off ? n : 0, host_off, host_stride, alias,
+                 ctx->last.gen + 1};
+}
+
+/* the pinned flag of regk_gather_push and the job exchanges, zeroed when first made */
+int ensure_gather_flag(regk_ctx *ctx)
+{
+    if (ctx->h_gather_flag.p)
+        return REGK_OK;
+    const int rc = ensure_host(ctx, ctx->h_gather_flag, sizeof(uint32_t));
+    if (rc == REGK_OK)
+        *(uint32_t *)ctx->h_gather_flag.p = 0;
+    return rc;
 }
 
 /* Lookahead distance of a compose kernel (PathParams / JsonParams::lookahead): half a wave, where a wave is how many
@@ -378,8 +517,8 @@ static bool chunk_bounds_ok(const regk_batch *b, uint64_t chunk, bool do_path, b
            (!do_json || (ok(b->addr_off) && ok(b->ports_off)));
 }
 
-static int run_pipelined(regk_ctx *ctx, const regk_batch *b, regk_result *res, const PathParams &pp0, size_t path_smem,
-    const JsonParams &jp0, size_t json_smem, const HostPipe &hp)
+static int run_pipelined(regk_ctx *ctx, regk_ctx::HostSet &hs, const regk_batch *b, regk_result *res, const PathParams &pp0,
+    size_t path_smem, const JsonParams &jp0, size_t json_smem, const HostPipe &hp)
 {
     const uint64_t n = b->n;
     const bool alias = b->flags & REGK_NODE_ALIAS;
@@ -387,17 +526,14 @@ static int run_pipelined(regk_ctx *ctx, const regk_batch *b, regk_result *res, c
     const uint32_t stride = b->host_stride;
     cudaStream_t s = ctx->stream;
     int rc;
-    if (!ctx->s_h2d) {
-        CK(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
-        CK(cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking));
-    }
-    while (ctx->pipe_events.size() < 3 * hp.nchunks + 2) {
-        cudaEvent_t e;
-        CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        ctx->pipe_events.push_back(e);
-    }
-    if ((rc = ensure_host(ctx, ctx->h_path_bytes, hp.path_cap)) || (rc = ensure_host(ctx, ctx->h_path_off, (n + 1) * 8)) ||
-        (rc = ensure_host(ctx, ctx->h_json_bytes, hp.json_cap)) || (rc = ensure_host(ctx, ctx->h_json_off, (n + 1) * 8)) ||
+    if ((rc = ensure_stream(ctx, ctx->s_h2d)) || (rc = ensure_stream(ctx, ctx->s_d2h)))
+        return rc;
+    ctx->pipe_events.resize(std::max<size_t>(ctx->pipe_events.size(), 3 * hp.nchunks + 2));
+    for (Event &ev : ctx->pipe_events)
+        if ((rc = ensure_event(ctx, ev, cudaEventDisableTiming)))
+            return rc;
+    if ((rc = ensure_host(ctx, hs.h_path_bytes, hp.path_cap)) || (rc = ensure_host(ctx, hs.h_path_off, (n + 1) * 8)) ||
+        (rc = ensure_host(ctx, hs.h_json_bytes, hp.json_cap)) || (rc = ensure_host(ctx, hs.h_json_off, (n + 1) * 8)) ||
         (rc = ensure_host(ctx, ctx->h_running, (hp.nchunks + 2) * 8)))
         return rc;
     unsigned long long *h_running = (unsigned long long *)ctx->h_running.p;
@@ -526,17 +662,17 @@ static int run_pipelined(regk_ctx *ctx, const regk_batch *b, regk_result *res, c
         if (do_path) {
             const uint64_t lo = path_cf(r0), hi = std::min<uint64_t>(path_cf(r1), hp.path_cap);
             if (hi > lo)
-                CK(cudaMemcpyAsync((uint8_t *)ctx->h_path_bytes.p + lo, (uint8_t *)ctx->path_bytes.p + lo, hi - lo,
+                CK(cudaMemcpyAsync((uint8_t *)hs.h_path_bytes.p + lo, (uint8_t *)hs.path_bytes.p + lo, hi - lo,
                     cudaMemcpyDeviceToHost, ctx->s_d2h));
-            CK(cudaMemcpyAsync((uint64_t *)ctx->h_path_off.p + r0, (uint64_t *)ctx->path_off.p + r0, (r1 - r0 + (last ? 1 : 0)) * 8,
+            CK(cudaMemcpyAsync((uint64_t *)hs.h_path_off.p + r0, (uint64_t *)hs.path_off.p + r0, (r1 - r0 + (last ? 1 : 0)) * 8,
                 cudaMemcpyDeviceToHost, ctx->s_d2h));
         }
         if (do_json) {
             const uint64_t lo = h_running[c], hi = std::min<uint64_t>(h_running[c + 1], hp.json_cap);
             if (hi > lo)
-                CK(cudaMemcpyAsync((uint8_t *)ctx->h_json_bytes.p + lo, (uint8_t *)ctx->json_bytes.p + lo, hi - lo,
+                CK(cudaMemcpyAsync((uint8_t *)hs.h_json_bytes.p + lo, (uint8_t *)hs.json_bytes.p + lo, hi - lo,
                     cudaMemcpyDeviceToHost, ctx->s_d2h));
-            CK(cudaMemcpyAsync((uint64_t *)ctx->h_json_off.p + r0, (uint64_t *)ctx->json_off.p + r0, (r1 - r0 + (last ? 1 : 0)) * 8,
+            CK(cudaMemcpyAsync((uint64_t *)hs.h_json_off.p + r0, (uint64_t *)hs.json_off.p + r0, (r1 - r0 + (last ? 1 : 0)) * 8,
                 cudaMemcpyDeviceToHost, ctx->s_d2h));
         }
     }
@@ -559,10 +695,10 @@ static int run_pipelined(regk_ctx *ctx, const regk_batch *b, regk_result *res, c
         return REGK_ERR_STATE + 100;            /* caller re-runs the batch through the exact-capable path */
     res->path_total = st.path_total;
     res->json_total = st.json_total;
-    res->path_bytes = (uint8_t *)ctx->h_path_bytes.p;
-    res->path_off = (uint64_t *)ctx->h_path_off.p;
-    res->json_bytes = (uint8_t *)ctx->h_json_bytes.p;
-    res->json_off = (uint64_t *)ctx->h_json_off.p;
+    res->path_bytes = (uint8_t *)hs.h_path_bytes.p;
+    res->path_off = (uint64_t *)hs.h_path_off.p;
+    res->json_bytes = (uint8_t *)hs.h_json_bytes.p;
+    res->json_off = (uint64_t *)hs.h_json_off.p;
     if (!do_path)
         memset(res->path_off, 0, (n + 1) * 8);
     if (!do_json)
@@ -570,26 +706,18 @@ static int run_pipelined(regk_ctx *ctx, const regk_batch *b, regk_result *res, c
     return REGK_OK;
 }
 
-/*
- * D2H of an async host batch into its set's pinned result buffers, on the D2H stream.  Called once the
- * batch's status has reached the host (its kernels are done), so the exact byte counts are known; a batch
- * that failed the fence or still needs the exact-offset redo is left to regk_finish.
- */
-static int issue_d2h(regk_ctx *ctx, regk_ctx::Slot &slot)
+/* D2H of a host batch's results into its set's pinned buffers, enqueued on sd once the batch's status has reached the
+   host (its kernels are done), so the exact byte counts are known. */
+static int enqueue_d2h(regk_ctx *ctx, regk_ctx::Slot &slot, cudaStream_t sd)
 {
     const DevStatus st = *slot.h_status;
-    regk_ctx::HostSet &hs = ctx->hset[slot.hset];
-    if (st.bad_bits || st.overflow)
-        return REGK_OK;
-    if (st.needs_exact && slot.did_path)
-        return REGK_OK;
+    regk_ctx::HostSet &hs = *slot.set;
     const uint64_t n = slot.n;
     const bool do_path = !(slot.flags & REGK_NO_PATH), do_json = !(slot.flags & REGK_NO_JSON);
     int rc;
     if ((rc = ensure_host(ctx, hs.h_path_bytes, st.path_total + 16)) || (rc = ensure_host(ctx, hs.h_path_off, (n + 1) * 8)) ||
         (rc = ensure_host(ctx, hs.h_json_bytes, st.json_total + 16)) || (rc = ensure_host(ctx, hs.h_json_off, (n + 1) * 8)))
         return rc;
-    cudaStream_t sd = ctx->s_d2h;
     slot.off32 = slot.off32 && st.path_total < (1ull << 32) && st.json_total < (1ull << 32);   /* else: 64-bit after all */
     const size_t ow = slot.off32 ? 4 : 8;
     if (n && do_path) {
@@ -604,27 +732,50 @@ static int issue_d2h(regk_ctx *ctx, regk_ctx::Slot &slot)
     } else {
         memset(hs.h_json_off.p, 0, (n + 1) * 8);
     }
-    CK(cudaEventRecord(hs.e_out, sd));
+    return REGK_OK;
+}
+
+/* The D2H of an async host batch, on the D2H stream; a batch that failed the fence or still needs the exact-offset
+   redo is left to regk_finish. */
+static int issue_d2h(regk_ctx *ctx, regk_ctx::Slot &slot)
+{
+    const DevStatus st = *slot.h_status;
+    if (st.bad_bits || st.overflow)
+        return REGK_OK;
+    if (st.needs_exact && slot.did_path)
+        return REGK_OK;
+    const int rc = enqueue_d2h(ctx, slot, ctx->s_d2h);
+    if (rc)
+        return rc;
+    CK(cudaEventRecord(slot.set->e_out, ctx->s_d2h));
     slot.d2h_issued = true;
     return REGK_OK;
 }
 
-template <bool MULTI, bool DATA>
-static cudaError_t launch_jute(const JuteParams &p, size_t smem, int device, cudaStream_t s)
+/* a host batch's results as regk_finish hands them out: the pinned buffers of its set */
+static void host_results(regk_result *res, const regk_ctx::HostSet &hs, bool off32)
 {
-    static std::mutex mu;
-    static size_t high[64];
-    {
-        std::lock_guard<std::mutex> lock(mu);
-        if (smem > high[device & 63]) {
-            cudaError_t e = cudaFuncSetAttribute(regk_jute_kernel<MULTI, DATA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess)
-                return e;
-            high[device & 63] = smem;
-        }
+    res->flags = 0;
+    res->path_bytes = (uint8_t *)hs.h_path_bytes.p;
+    res->json_bytes = (uint8_t *)hs.h_json_bytes.p;
+    if (off32) {
+        res->path_off32 = (uint32_t *)hs.h_path_off.p;
+        res->json_off32 = (uint32_t *)hs.h_json_off.p;
+    } else {
+        res->path_off = (uint64_t *)hs.h_path_off.p;
+        res->json_off = (uint64_t *)hs.h_json_off.p;
     }
-    regk_jute_kernel<MULTI, DATA><<<(unsigned)((p.n + JUTE_TILE - 1) / JUTE_TILE), JUTE_THREADS, smem, s>>>(p);
-    return cudaGetLastError();
+}
+
+template <bool MULTI, bool DATA>
+static int launch_jute(regk_ctx *ctx, const JuteParams &p, size_t smem)
+{
+    const int rc = set_smem_limit(ctx, (const void *)regk_jute_kernel<MULTI, DATA>, smem);
+    if (rc)
+        return rc;
+    regk_jute_kernel<MULTI, DATA><<<(unsigned)((p.n + JUTE_TILE - 1) / JUTE_TILE), JUTE_THREADS, smem, ctx->stream>>>(p);
+    CK(cudaGetLastError());
+    return REGK_OK;
 }
 
 /* The request frames of one (path, payload) stream pair on the device - regk_jute_requests on the batch finished last,
@@ -654,9 +805,9 @@ struct FrameGeom {
    `group` entries when `multi`, else one request per entry; every entry carries `per_rec` framing bytes, emits its path
    `path_times` times, and a tile's framing slots take `slot_bytes` of shared memory. */
 static int frame_drive(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts *o, bool multi, uint64_t group, uint32_t per_rec,
-    uint32_t path_times, size_t slot_bytes, DevBuf &db, DevBuf &doff, HostBuf &hb, HostBuf &hoff, regk_frames *out,
-    const std::function<cudaError_t(const FrameGeom &)> &launch)
+    uint32_t path_times, size_t slot_bytes, FrameBufs &fb, regk_frames *out, const std::function<int(const FrameGeom &)> &launch)
 {
+    DevBuf &db = fb.bytes, &doff = fb.off;
     const uint64_t n = src.n;
     const bool has_data = src.json_off != nullptr;
     const uint64_t frames = (n + group - 1) / group;
@@ -676,9 +827,9 @@ static int frame_drive(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts 
     int rc;
     if ((rc = ensure_dev(ctx, db, total + 32)) || (rc = ensure_dev(ctx, doff, (frames + 1) * 8)))
         return rc;
-    if ((rc = ensure_dev(ctx, ctx->svc_work, 256)))
+    if ((rc = ensure_dev(ctx, ctx->svc.work, 256)))
         return rc;
-    CK(cudaMemsetAsync(ctx->svc_work.p, 0, sizeof(DevStatus), s));
+    CK(cudaMemsetAsync(ctx->svc.work.p, 0, sizeof(DevStatus), s));
     if (n == 0)
         CK(cudaMemsetAsync(doff.p, 0, 8, s));
     cudaEvent_t e0 = ctx->slots[0].ev[0], e1 = ctx->slots[0].ev[1];
@@ -688,7 +839,7 @@ static int frame_drive(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts 
         g.total = total;
         g.out_bytes = (uint8_t *)db.p;
         g.out_off = (unsigned long long *)doff.p;
-        g.status = (DevStatus *)ctx->svc_work.p;
+        g.status = (DevStatus *)ctx->svc.work.p;
         /* staging budgets: 9/8 of a tile's mean share of each stream plus slack (tiles beyond it go byte-wise) */
         g.path_cap = (uint32_t)align16(std::min<uint64_t>(tot[0] * JUTE_TILE / n * 9 / 8 + 1024, 65520));
         g.json_cap = has_data ? (uint32_t)align16(std::min<uint64_t>(tot[1] * JUTE_TILE / n * 9 / 8 + 1024, 65520)) : 0u;  /* lengths travel as 16 bits */
@@ -699,14 +850,14 @@ static int frame_drive(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts 
         const size_t owner_bytes = 3 * ((path_times * g.path_cap + g.json_cap + max_fixed * JUTE_TILE) / 16 + 32);   /* owner u8 + list u16 per block */
         g.smem = 34 * 16 + 16 + slot_bytes + 16 + (size_t)g.path_cap + 16 + g.json_cap + 48 + owner_bytes;
         CK(cudaEventRecord(e0, s));
-        CK(launch(g));
+        if ((rc = launch(g)))
+            return rc;
         CK(cudaEventRecord(e1, s));
         out->launches = 1;
     }
-    CK(cudaMemcpyAsync(ctx->slots[0].h_status, ctx->svc_work.p, sizeof(DevStatus), cudaMemcpyDeviceToHost, s));
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "%s: kernel execution failed: %s", src.who, cudaGetErrorString(e));
+    CK(cudaMemcpyAsync(ctx->slots[0].h_status, ctx->svc.work.p, sizeof(DevStatus), cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, src.who)))
+        return rc;
     if (ctx->slots[0].h_status->overflow)
         return fail(ctx, REGK_ERR_CUDA, "internal error: frame capacity bound exceeded");
     if (n)
@@ -717,19 +868,15 @@ static int frame_drive(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts 
         out->frame_off = (const uint64_t *)doff.p;
         return REGK_OK;
     }
-    if ((rc = ensure_host(ctx, hb, total + 16)) || (rc = ensure_host(ctx, hoff, (frames + 1) * 8)))
+    if ((rc = to_host(ctx, fb.h_bytes, db.p, total, s)) || (rc = to_host(ctx, fb.h_off, doff.p, (frames + 1) * 8, s)))
         return rc;
-    if (total)
-        CK(cudaMemcpyAsync(hb.p, db.p, total, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(hoff.p, doff.p, (frames + 1) * 8, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    out->frame_bytes = (const uint8_t *)hb.p;
-    out->frame_off = (const uint64_t *)hoff.p;
+    out->frame_bytes = (const uint8_t *)fb.h_bytes.p;
+    out->frame_off = (const uint64_t *)fb.h_off.p;
     return REGK_OK;
 }
 
-static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts *o, DevBuf &db, DevBuf &doff, HostBuf &hb,
-    HostBuf &hoff, regk_frames *out)
+static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts *o, FrameBufs &fb, regk_frames *out)
 {
     const bool has_data = src.json_off != nullptr;
     const bool multi = o->group != 0;
@@ -766,7 +913,7 @@ static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_op
     p.xid_base = o->xid_base;
     /* framing slots, 16 bytes of slack, the constant tail */
     const size_t slot_bytes = JUTE_TILE * JUTE_SLOT + 16 + 48;
-    return frame_drive(ctx, src, o, multi, g, p.per_rec, 1, slot_bytes, db, doff, hb, hoff, out, [&](const FrameGeom &G) {
+    return frame_drive(ctx, src, o, multi, g, p.per_rec, 1, slot_bytes, fb, out, [&](const FrameGeom &G) {
         p.out_bytes = G.out_bytes;
         p.out_off = G.out_off;
         p.out_capacity = G.total;
@@ -775,37 +922,27 @@ static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_op
         p.json_cap = G.json_cap;
         p.path_limit = G.path_limit;
         p.json_limit = G.json_limit;
-        return multi ? (has_data ? launch_jute<true, true>(p, G.smem, ctx->device, ctx->stream)
-                                 : launch_jute<true, false>(p, G.smem, ctx->device, ctx->stream))
-                     : (has_data ? launch_jute<false, true>(p, G.smem, ctx->device, ctx->stream)
-                                 : launch_jute<false, false>(p, G.smem, ctx->device, ctx->stream));
+        return multi ? (has_data ? launch_jute<true, true>(ctx, p, G.smem) : launch_jute<true, false>(ctx, p, G.smem))
+                     : (has_data ? launch_jute<false, true>(ctx, p, G.smem) : launch_jute<false, false>(ctx, p, G.smem));
     });
 }
 
 template <bool MULTI, bool DATA, bool PAIR>
-static cudaError_t launch_jute_entry(const JuteEntryParams &p, size_t smem, int device, cudaStream_t s)
+static int launch_jute_entry(regk_ctx *ctx, const JuteEntryParams &p, size_t smem)
 {
-    static std::mutex mu;
-    static size_t high[64];
-    {
-        std::lock_guard<std::mutex> lock(mu);
-        if (smem > high[device & 63]) {
-            cudaError_t e = cudaFuncSetAttribute(regk_jute_entry_kernel<MULTI, DATA, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                 (int)smem);
-            if (e != cudaSuccess)
-                return e;
-            high[device & 63] = smem;
-        }
-    }
-    regk_jute_entry_kernel<MULTI, DATA, PAIR><<<(unsigned)((p.n + JUTE_TILE - 1) / JUTE_TILE), JUTE_THREADS, smem, s>>>(p);
-    return cudaGetLastError();
+    const int rc = set_smem_limit(ctx, (const void *)regk_jute_entry_kernel<MULTI, DATA, PAIR>, smem);
+    if (rc)
+        return rc;
+    regk_jute_entry_kernel<MULTI, DATA, PAIR><<<(unsigned)((p.n + JUTE_TILE - 1) / JUTE_TILE), JUTE_THREADS, smem, ctx->stream>>>(p);
+    CK(cudaGetLastError());
+    return REGK_OK;
 }
 
 /* Frames whose entries carry a version of their own (`version`: [n] device array, NULL = o->version for all) or that
    pair a delete with a create (`pair`: REGK_ZK_REPLACE, always multi transactions) - regk_jute_entry_kernel.  Output
    and buffers as frame_requests. */
 static int frame_entry_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_opts *o, const int32_t *version, bool pair,
-    DevBuf &db, DevBuf &doff, HostBuf &hb, HostBuf &hoff, regk_frames *out)
+    FrameBufs &fb, regk_frames *out)
 {
     const bool has_data = src.json_off != nullptr;
     const bool multi = pair || o->group != 0;
@@ -824,32 +961,28 @@ static int frame_entry_requests(regk_ctx *ctx, const FrameSrc &src, const regk_j
     p.json_bytes = src.json_bytes;
     p.json_off = src.json_off;
     p.xid_base = o->xid_base;
-    return frame_drive(ctx, src, o, multi, g, p.per_rec, pair ? 2 : 1, JUTE_TILE * JUTE_ESLOT, db, doff, hb, hoff, out,
-        [&](const FrameGeom &G) {
-            p.out_bytes = G.out_bytes;
-            p.out_off = G.out_off;
-            p.out_capacity = G.total;
-            p.status = G.status;
-            p.path_cap = G.path_cap;
-            p.json_cap = G.json_cap;
-            p.path_limit = G.path_limit;
-            p.json_limit = G.json_limit;
-            cudaStream_t s = ctx->stream;
-            return pair ? launch_jute_entry<true, true, true>(p, G.smem, ctx->device, s)
-                : multi ? (has_data ? launch_jute_entry<true, true, false>(p, G.smem, ctx->device, s)
-                                    : launch_jute_entry<true, false, false>(p, G.smem, ctx->device, s))
-                        : (has_data ? launch_jute_entry<false, true, false>(p, G.smem, ctx->device, s)
-                                    : launch_jute_entry<false, false, false>(p, G.smem, ctx->device, s));
-        });
+    return frame_drive(ctx, src, o, multi, g, p.per_rec, pair ? 2 : 1, JUTE_TILE * JUTE_ESLOT, fb, out, [&](const FrameGeom &G) {
+        p.out_bytes = G.out_bytes;
+        p.out_off = G.out_off;
+        p.out_capacity = G.total;
+        p.status = G.status;
+        p.path_cap = G.path_cap;
+        p.json_cap = G.json_cap;
+        p.path_limit = G.path_limit;
+        p.json_limit = G.json_limit;
+        return pair ? launch_jute_entry<true, true, true>(ctx, p, G.smem)
+            : multi ? (has_data ? launch_jute_entry<true, true, false>(ctx, p, G.smem) : launch_jute_entry<true, false, false>(ctx, p, G.smem))
+                    : (has_data ? launch_jute_entry<false, true, false>(ctx, p, G.smem) : launch_jute_entry<false, false, false>(ctx, p, G.smem));
+    });
 }
 
 /* regk_parents.cuh on the path stream of the batch finished last (n >= 1 records), into the given buffers: enqueues
    the table reset, `start` (if any) and the three kernels on the context's stream; p->parent_len / unique_first / n_unique are device
    pointers into `len` and `unique`. */
-static int enqueue_parent_pass(regk_ctx *ctx, DevBuf &len, DevBuf &slot, DevBuf &table, DevBuf &totals, DevBuf &unique, uint64_t n,
-    cudaEvent_t start, ParentParams *out)
+static int enqueue_parent_pass(regk_ctx *ctx, ParentPass &b, uint64_t n, cudaEvent_t start, ParentParams *out)
 {
     cudaStream_t s = ctx->stream;
+    DevBuf &len = b.len, &slot = b.slot, &table = b.table, &totals = b.totals, &unique = b.unique;
     uint64_t slots = 1024;
     while (slots < 2 * n)
         slots <<= 1;
@@ -861,8 +994,8 @@ static int enqueue_parent_pass(regk_ctx *ctx, DevBuf &len, DevBuf &slot, DevBuf 
         return rc;
     ParentParams p{};
     p.n = n;
-    p.path_bytes = ctx->last_path_bytes;
-    p.path_off = ctx->last_path_off;
+    p.path_bytes = ctx->last.path_bytes;
+    p.path_off = ctx->last.path_off;
     p.parent_len = (uint32_t *)len.p;
     p.slot_of = (uint32_t *)slot.p;
     p.owner = (uint32_t *)table.p;
@@ -871,9 +1004,9 @@ static int enqueue_parent_pass(regk_ctx *ctx, DevBuf &len, DevBuf &slot, DevBuf 
     p.super_total = (unsigned long long *)((uint8_t *)totals.p + ((ntiles * 4 + 15) & ~(size_t)15));
     p.unique_first = (unsigned long long *)unique.p;
     p.n_unique = p.unique_first + n;
-    p.tail_mode = ctx->last_alias ? 0u : (ctx->last_host_off ? 2u : 1u);
-    p.host_stride = ctx->last_host_stride;
-    p.host_off = ctx->last_host_off;
+    p.tail_mode = ctx->last.alias ? 0u : (ctx->last.host_off ? 2u : 1u);
+    p.host_stride = ctx->last.host_stride;
+    p.host_off = ctx->last.host_off;
     CK(cudaMemsetAsync(p.owner, 0, slots * 4, s));
     CK(cudaMemsetAsync(totals.p, 0, totals_bytes, s));
     if (start)
@@ -900,7 +1033,7 @@ const char *regk_last_error(const regk_ctx *ctx)
 
 int regk_create(int device, regk_ctx **out)
 {
-    regk_ctx *ctx = nullptr;
+    regk_ctx *const ctx = nullptr;              /* errors before the context exists go to regk_last_error(NULL) */
     if (!out)
         return fail(nullptr, REGK_ERR_INVALID_ARG, "regk_create: out is NULL");
     *out = nullptr;
@@ -911,165 +1044,33 @@ int regk_create(int device, regk_ctx **out)
             e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0");
     if (device < 0 || device >= ndev)
         return fail(nullptr, REGK_ERR_INVALID_ARG, "regk_create: device %d out of range (0..%d)", device, ndev - 1);
-    ctx = new regk_ctx();
-    ctx->device = device;
-#define CKC(call)                                                                               \
-    do {                                                                                        \
-        cudaError_t e_ = (call);                                                                \
-        if (e_ != cudaSuccess) {                                                                \
-            int rc_ = fail(nullptr, REGK_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(e_)); \
-            delete ctx;                                                                         \
-            return rc_;                                                                         \
-        }                                                                                       \
-    } while (0)
-    CKC(cudaSetDevice(device));
+    auto c = std::make_unique<regk_ctx>();
+    c->device = device;
+    CK(cudaSetDevice(device));
     cudaDeviceProp prop;
-    CKC(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) {   /* sm_90a code runs on compute capability 9.0 only */
-        int rc = fail(nullptr, REGK_ERR_CUDA, "regk_create: device %d is sm_%d%d; this build targets sm_90a (H100)",
+    CK(cudaGetDeviceProperties(&prop, device));
+    if (prop.major != 9 || prop.minor != 0)     /* sm_90a code runs on compute capability 9.0 only */
+        return fail(nullptr, REGK_ERR_CUDA, "regk_create: device %d is sm_%d%d; this build targets sm_90a (H100)",
             device, prop.major, prop.minor);
-        delete ctx;
+    c->sm_count = prop.multiProcessorCount;
+    c->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
+    int rc;
+    if ((rc = ensure_stream(ctx, c->own_stream)) || (rc = ensure_host(ctx, c->h_status_block, sizeof(DevStatus) * regk_ctx::NSLOTS)))
         return rc;
-    }
-    ctx->sm_count = prop.multiProcessorCount;
-    ctx->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
-    CKC(cudaStreamCreateWithFlags(&ctx->own_stream, cudaStreamNonBlocking));
-    ctx->stream = ctx->own_stream;
-    CKC(cudaMallocHost((void **)&ctx->h_status_block, sizeof(DevStatus) * regk_ctx::NSLOTS));
-    memset(ctx->h_status_block, 0, sizeof(DevStatus) * regk_ctx::NSLOTS);
+    c->stream = c->own_stream;
+    memset(c->h_status_block.p, 0, sizeof(DevStatus) * regk_ctx::NSLOTS);
     for (int i = 0; i < regk_ctx::NSLOTS; i++) {
-        for (auto &ev : ctx->slots[i].ev)
-            CKC(cudaEventCreate(&ev));
-        ctx->slots[i].h_status = ctx->h_status_block + i;
+        for (Event &ev : c->slots[i].ev)
+            if ((rc = ensure_event(ctx, ev)))
+                return rc;
+        c->slots[i].h_status = (DevStatus *)c->h_status_block.p + i;
     }
-#undef CKC
-    *out = ctx;
+    *out = c.release();
     return REGK_OK;
 }
 
 void regk_destroy(regk_ctx *ctx)
 {
-    if (!ctx)
-        return;
-    cudaSetDevice(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-    for (auto &b : ctx->in)
-        if (b.p)
-            cudaFree(b.p);
-    for (DevBuf *b : {&ctx->blob_dev, &ctx->path_bytes, &ctx->path_off, &ctx->json_bytes, &ctx->json_off, &ctx->work, &ctx->off32_p,
-             &ctx->off32_j})
-        if (b->p)
-            cudaFree(b->p);
-    for (cudaEvent_t e : ctx->pipe_events)
-        cudaEventDestroy(e);
-    if (ctx->s_h2d)
-        cudaStreamSynchronize(ctx->s_h2d);
-    if (ctx->s_d2h)
-        cudaStreamSynchronize(ctx->s_d2h);
-    for (auto &hs : ctx->hset) {
-        for (auto &b : hs.in)
-            if (b.p)
-                cudaFree(b.p);
-        for (DevBuf *b : {&hs.path_bytes, &hs.path_off, &hs.json_bytes, &hs.json_off, &hs.off32_p, &hs.off32_j})
-            if (b->p)
-                cudaFree(b->p);
-        for (HostBuf *b : {&hs.h_path_bytes, &hs.h_path_off, &hs.h_json_bytes, &hs.h_json_off})
-            if (b->p)
-                cudaFreeHost(b->p);
-        if (hs.e_in)
-            cudaEventDestroy(hs.e_in);
-        if (hs.e_out)
-            cudaEventDestroy(hs.e_out);
-    }
-    for (auto &e : ctx->ws_clean)
-        if (e)
-            cudaEventDestroy(e);
-    for (auto &wb : ctx->work_ring)
-        if (wb.p)
-            cudaFree(wb.p);
-    if (ctx->s_side)
-        cudaStreamDestroy(ctx->s_side);
-    if (ctx->s_h2d)
-        cudaStreamDestroy(ctx->s_h2d);
-    if (ctx->s_d2h)
-        cudaStreamDestroy(ctx->s_d2h);
-    for (HostBuf *b : {&ctx->h_path_bytes, &ctx->h_path_off, &ctx->h_json_bytes, &ctx->h_json_off, &ctx->h_running})
-        if (b->p)
-            cudaFreeHost(b->p);
-    if (ctx->h_status_block)
-        cudaFreeHost(ctx->h_status_block);
-    if (ctx->h_gather_flag)
-        cudaFreeHost(ctx->h_gather_flag);
-    if (ctx->h_job_bases)
-        cudaFreeHost(ctx->h_job_bases);
-    if (ctx->job_bases.p)
-        cudaFree(ctx->job_bases.p);
-    for (auto &b : ctx->dec_in)
-        if (b.p)
-            cudaFree(b.p);
-    for (DevBuf *b : {&ctx->dec_rec, &ctx->dec_dom, &ctx->dec_ports})
-        if (b->p)
-            cudaFree(b->p);
-    for (HostBuf *b : {&ctx->h_jute_bytes, &ctx->h_jute_off, &ctx->h_dec_rec, &ctx->h_dec_dom, &ctx->h_dec_ports})
-        if (b->p)
-            cudaFreeHost(b->p);
-    for (DevBuf *b : {&ctx->par_len, &ctx->par_slot, &ctx->par_table, &ctx->par_totals, &ctx->par_unique, &ctx->svc_work,
-             &ctx->jute_bytes, &ctx->jute_off})
-        if (b->p)
-            cudaFree(b->p);
-    for (auto &b : ctx->svc_in)
-        if (b.p)
-            cudaFree(b.p);
-    for (auto &ev : ctx->par_ev)
-        if (ev)
-            cudaEventDestroy(ev);
-    for (HostBuf *b : {&ctx->h_par_len, &ctx->h_par_unique, &ctx->h_par_count, &ctx->h_skip_status, &ctx->h_skip_index,
-             &ctx->h_skip_bits})
-        if (b->p)
-            cudaFreeHost(b->p);
-    for (auto &b : ctx->skip_in)
-        if (b.p)
-            cudaFree(b.p);
-    for (DevBuf *b : {&ctx->skip_work, &ctx->skip_off_p, &ctx->skip_off_j, &ctx->skip_index, &ctx->skip_bits})
-        if (b->p)
-            cudaFree(b->p);
-    for (auto &b : ctx->mk)
-        if (b.p)
-            cudaFree(b.p);
-    for (HostBuf *b : {&ctx->h_mk_count, &ctx->h_mk_drec, &ctx->h_mk_dlen, &ctx->h_mk_dbytes, &ctx->h_mk_doff, &ctx->h_mk_depth,
-             &ctx->h_mk_invalid, &ctx->h_mk_fbytes, &ctx->h_mk_foff})
-        if (b->p)
-            cudaFreeHost(b->p);
-    for (auto &ev : ctx->mk_ev)
-        if (ev)
-            cudaEventDestroy(ev);
-    for (auto &b : ctx->rc)
-        if (b.p)
-            cudaFree(b.p);
-    for (HostBuf *b : {&ctx->h_rc_count, &ctx->h_rc_cls, &ctx->h_rc_match, &ctx->h_rc_obscls, &ctx->h_rc_fbytes, &ctx->h_rc_foff})
-        if (b->p)
-            cudaFreeHost(b->p);
-    for (auto &b : ctx->h_rc_list)
-        if (b.p)
-            cudaFreeHost(b.p);
-    for (auto &ev : ctx->rc_ev)
-        if (ev)
-            cudaEventDestroy(ev);
-    for (auto &b : ctx->rq)
-        if (b.p)
-            cudaFree(b.p);
-    for (HostBuf *b : {&ctx->h_rq_count, &ctx->h_rq_err, &ctx->h_rq_node})
-        if (b->p)
-            cudaFreeHost(b->p);
-    for (auto &ev : ctx->rq_ev)
-        if (ev)
-            cudaEventDestroy(ev);
-    for (auto &sl : ctx->slots)
-        for (auto &ev : sl.ev)
-            if (ev)
-                cudaEventDestroy(ev);
-    if (ctx->own_stream)
-        cudaStreamDestroy(ctx->own_stream);
     delete ctx;
 }
 
@@ -1220,8 +1221,9 @@ int regk_sync(regk_ctx *ctx)
         return REGK_ERR_INVALID_ARG;
     CK(cudaSetDevice(ctx->device));
     CK(cudaStreamSynchronize(ctx->stream));
-    if (ctx->h_gather_flag && *ctx->h_gather_flag) {
-        *ctx->h_gather_flag = 0;
+    uint32_t *flag = (uint32_t *)ctx->h_gather_flag.p;
+    if (flag && *flag) {
+        *flag = 0;
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_gather_push: the totals table exceeds the whole-job buffers or disagrees with the shard; nothing was stored");
     }
     return REGK_OK;
@@ -1276,10 +1278,9 @@ int regk_gather_push(regk_ctx *ctx, const regk_result *shard, const regk_gather 
             (((uintptr_t)g->path_bytes[q] | (uintptr_t)g->json_bytes[q]) & 15) || (((uintptr_t)g->path_off[q] | (uintptr_t)g->json_off[q]) & 7))
             return fail(ctx, REGK_ERR_INVALID_ARG, "regk_gather_push: buffer of rank %u missing or misaligned", q);
     CK(cudaSetDevice(ctx->device));
-    if (!ctx->h_gather_flag) {
-        CK(cudaMallocHost((void **)&ctx->h_gather_flag, sizeof(uint32_t)));
-        *ctx->h_gather_flag = 0;
-    }
+    int rc = ensure_gather_flag(ctx);
+    if (rc)
+        return rc;
     GatherParams p{};
     p.world = g->world;
     p.rank = g->rank;
@@ -1301,7 +1302,7 @@ int regk_gather_push(regk_ctx *ctx, const regk_result *shard, const regk_gather 
     p.json_cap = g->json_cap;
     p.my_path_total = shard->path_total;
     p.my_json_total = shard->json_total;
-    p.flag = ctx->h_gather_flag;
+    p.flag = (uint32_t *)ctx->h_gather_flag.p;
     regk_gather_push_kernel<<<(unsigned)ctx->sm_count * 8, 256, 0, ctx->stream>>>(p);
     CK(cudaGetLastError());
     return REGK_OK;
@@ -1326,15 +1327,10 @@ int regk_job_bind(regk_ctx *ctx, const regk_job *job)
             (((uintptr_t)job->path_off[q] | (uintptr_t)job->json_off[q] | (uintptr_t)job->mailbox[q]) & 7))
             return fail(ctx, REGK_ERR_INVALID_ARG, "regk_job_bind: buffer of rank %u missing or misaligned", q);
     CK(cudaSetDevice(ctx->device));
-    int rc = ensure_dev(ctx, ctx->job_bases, (size_t)regk_ctx::NSLOTS * 64);
-    if (rc)
+    int rc;
+    if ((rc = ensure_dev(ctx, ctx->job_bases, (size_t)regk_ctx::NSLOTS * 64)) ||
+        (rc = ensure_host(ctx, ctx->h_job_bases, (size_t)regk_ctx::NSLOTS * 64)) || (rc = ensure_gather_flag(ctx)))
         return rc;
-    if (!ctx->h_job_bases)
-        CK(cudaMallocHost((void **)&ctx->h_job_bases, (size_t)regk_ctx::NSLOTS * 64));
-    if (!ctx->h_gather_flag) {
-        CK(cudaMallocHost((void **)&ctx->h_gather_flag, sizeof(uint32_t)));
-        *ctx->h_gather_flag = 0;
-    }
     ctx->job = *job;
     ctx->job_bound = true;
     return REGK_OK;
@@ -1358,7 +1354,7 @@ static int launch_exchange(regk_ctx *ctx, unsigned long long v0, unsigned long l
     e.bases = bases;
     e.close0 = close0;
     e.close1 = nullptr;
-    e.host_flag = ctx->h_gather_flag;
+    e.host_flag = (uint32_t *)ctx->h_gather_flag.p;
     e.timeout_ns = (j.timeout_ms ? j.timeout_ms : 10000ull) * 1000000ull;
     regk_peer_exchange_kernel<<<1, 32, 0, ctx->stream>>>(e);
     CK(cudaGetLastError());
@@ -1454,24 +1450,18 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
     const bool pipelined = !in_dev && !out_dev && !async && chunk_records && n >= 2 * chunk_records &&
         !opt_get(ctx, "force_generic", 0) && chunk_bounds_ok(b, chunk_records, do_path, do_json, alias);
     /* Host buffers in and out with the "async" option: two batches may be in flight, each in its own HostSet. */
-    regk_ctx::HostSet *hs = (!in_dev && !out_dev && async && n) ? &ctx->hset[ctx->hseq & 1] : nullptr;
-    if (hs) {
+    const bool two_deep = !in_dev && !out_dev && async && n;
+    regk_ctx::HostSet &hs = two_deep ? ctx->hset[ctx->hseq & 1] : ctx->sync_set;
+    int rc;
+    if (two_deep) {
         for (const auto &sl : ctx->slots)
-            if (sl.in_use && sl.hset == (int)(ctx->hseq & 1))
+            if (sl.in_use && sl.set == &hs)
                 return fail(ctx, REGK_ERR_STATE,
                     "regk_register_batch: at most two host batches may be in flight; call regk_finish on the older one");
-        if (!ctx->s_h2d) {
-            CK(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
-            CK(cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking));
-        }
-        if (!hs->e_in) {
-            CK(cudaEventCreateWithFlags(&hs->e_in, cudaEventDisableTiming));
-            CK(cudaEventCreateWithFlags(&hs->e_out, cudaEventDisableTiming));
-        }
+        if ((rc = ensure_stream(ctx, ctx->s_h2d)) || (rc = ensure_stream(ctx, ctx->s_d2h)) ||
+            (rc = ensure_event(ctx, hs.e_in, cudaEventDisableTiming)) || (rc = ensure_event(ctx, hs.e_out, cudaEventDisableTiming)))
+            return rc;
     }
-    DevBuf *stage = hs ? hs->in : ctx->in;
-    DevBuf &o_path_bytes = hs ? hs->path_bytes : ctx->path_bytes, &o_path_off = hs ? hs->path_off : ctx->path_off,
-           &o_json_bytes = hs ? hs->json_bytes : ctx->json_bytes, &o_json_off = hs ? hs->json_off : ctx->json_off;
 
     /* ---- inputs on the device ---- */
     const void *src[11] = {b->domain_bytes, b->domain_off, b->host_bytes, b->host_off, b->type_id, b->addr_bytes,
@@ -1490,35 +1480,33 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
                 return fail(ctx, REGK_ERR_INVALID_ARG, "regk_register_batch: device array %d is not 16-byte aligned", i);
             dev[i] = src[i];
         } else {
-            int rc = ensure_dev(ctx, stage[i], sz[i] + 16);
+            rc = pipelined ? ensure_dev(ctx, hs.in[i], sz[i] + 16)         /* run_pipelined copies it chunk by chunk */
+                           : stage_in(ctx, hs.in[i], src[i], sz[i], two_deep ? ctx->s_h2d : s);
             if (rc)
                 return rc;
-            if (sz[i] && !pipelined)
-                CK(cudaMemcpyAsync(stage[i].p, src[i], sz[i], cudaMemcpyHostToDevice, hs ? ctx->s_h2d : s));
-            dev[i] = stage[i].p;
+            dev[i] = hs.in[i].p;
         }
     }
-    if (hs) {
+    if (two_deep) {
         /* this set's staging was last read by the kernels of the batch two submissions back, which has been
            finished (checked above); the kernels below wait for the copies */
-        CK(cudaEventRecord(hs->e_in, ctx->s_h2d));
-        CK(cudaStreamWaitEvent(s, hs->e_in, 0));
+        CK(cudaEventRecord(hs.e_in, ctx->s_h2d));
+        CK(cudaStreamWaitEvent(s, hs.e_in, 0));
     }
 
     /* ---- outputs (capacity = exact upper bounds, see DESIGN.md) ---- */
     const uint64_t path_cap = do_path ? dom_len + host_len + 2 * n + 16 : 16;
     const uint64_t json_cap = do_json ? n * (uint64_t)(38 + 2 * ctx->max_type_q + 4 + 18 + 11) + 2 * addr_len +
         11 * ports_len + 16 : 16;
-    int rc;
-    if (!job && ((rc = ensure_dev(ctx, o_path_bytes, path_cap)) || (rc = ensure_dev(ctx, o_path_off, (n + 1) * 8)) ||
-        (rc = ensure_dev(ctx, o_json_bytes, json_cap)) || (rc = ensure_dev(ctx, o_json_off, (n + 1) * 8))))
+    if (!job && ((rc = ensure_dev(ctx, hs.path_bytes, path_cap)) || (rc = ensure_dev(ctx, hs.path_off, (n + 1) * 8)) ||
+        (rc = ensure_dev(ctx, hs.json_bytes, json_cap)) || (rc = ensure_dev(ctx, hs.json_off, (n + 1) * 8))))
         return rc;
     /* job step: the outputs are the rank's own whole-job buffers, every position job-absolute */
     const regk_job &J = ctx->job;
-    uint8_t *const out_path_bytes = job ? (uint8_t *)J.path_bytes[J.rank] : (uint8_t *)o_path_bytes.p;
-    unsigned long long *const out_path_off = job ? (unsigned long long *)J.path_off[J.rank] + J.rec_base : (unsigned long long *)o_path_off.p;
-    uint8_t *const out_json_bytes = job ? (uint8_t *)J.json_bytes[J.rank] : (uint8_t *)o_json_bytes.p;
-    unsigned long long *const out_json_off = job ? (unsigned long long *)J.json_off[J.rank] + J.rec_base : (unsigned long long *)o_json_off.p;
+    uint8_t *const out_path_bytes = job ? (uint8_t *)J.path_bytes[J.rank] : (uint8_t *)hs.path_bytes.p;
+    unsigned long long *const out_path_off = job ? (unsigned long long *)J.path_off[J.rank] + J.rec_base : (unsigned long long *)hs.path_off.p;
+    uint8_t *const out_json_bytes = job ? (uint8_t *)J.json_bytes[J.rank] : (uint8_t *)hs.json_bytes.p;
+    unsigned long long *const out_json_off = job ? (unsigned long long *)J.json_off[J.rank] + J.rec_base : (unsigned long long *)hs.json_off.p;
     const uint64_t out_path_cap = job ? J.path_cap : path_cap, out_json_cap = job ? J.json_cap : json_cap;
     unsigned long long *const d_bases = job ? (unsigned long long *)ctx->job_bases.p + 8 * (ctx->seq % regk_ctx::NSLOTS) : nullptr;
 
@@ -1542,11 +1530,8 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
         CK(cudaMemsetAsync(wk, 0, work_bytes, s));
     } else {
         ring = (int)(ctx->ws_seq++ % regk_ctx::NWORK);
-        if (!ctx->s_side) {
-            CK(cudaStreamCreateWithFlags(&ctx->s_side, cudaStreamNonBlocking));
-            for (auto &e : ctx->ws_clean)
-                CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        }
+        if ((rc = ensure_stream(ctx, ctx->s_side)) || (rc = ensure_event(ctx, ctx->ws_clean[ring], cudaEventDisableTiming)))
+            return rc;
         const size_t cap_before = ctx->work_ring[ring].cap;
         if ((rc = ensure_dev(ctx, ctx->work_ring[ring], work_bytes)))
             return rc;
@@ -1568,8 +1553,8 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
     DevStatus *d_status = (DevStatus *)wk;
 
     if (n == 0 && !job) {
-        CK(cudaMemsetAsync(o_path_off.p, 0, 8, s));
-        CK(cudaMemsetAsync(o_json_off.p, 0, 8, s));
+        CK(cudaMemsetAsync(hs.path_off.p, 0, 8, s));
+        CK(cudaMemsetAsync(hs.json_off.p, 0, 8, s));
     }
     const uint32_t force_generic = (uint32_t)opt_get(ctx, "force_generic", 0);
 
@@ -1616,17 +1601,11 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
         pp.dom_cap = dom_cap;
         pp.host_cap = host_cap;
         pp.out_cap = out_cap;
-        if (smem_attr_needs_raise(ctx->device, alias ? 0 : 1, path_smem)) {    /* not free: only when it grows */
-            if (alias) {
-                CK(cudaFuncSetAttribute(regk_path_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)path_smem));
-                CK(cudaFuncSetAttribute(regk_path_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)path_smem));
-            } else {
-                CK(cudaFuncSetAttribute(regk_path_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)path_smem));
-                CK(cudaFuncSetAttribute(regk_path_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)path_smem));
-            }
-        }
-        if ((rc = lookahead_tiles(ctx, alias ? 0 : 1, alias ? (const void *)regk_path_kernel<true, false> : (const void *)regk_path_kernel<false, false>,
-                 path_smem, &pp.lookahead)))
+        /* the exact-offset redo (regk_finish) launches the exact variant with the same budget */
+        const void *kernel = alias ? (const void *)regk_path_kernel<true, false> : (const void *)regk_path_kernel<false, false>;
+        const void *exact = alias ? (const void *)regk_path_kernel<true, true> : (const void *)regk_path_kernel<false, true>;
+        if ((rc = set_smem_limit(ctx, kernel, path_smem)) || (rc = set_smem_limit(ctx, exact, path_smem)) ||
+            (rc = lookahead_tiles(ctx, alias ? 0 : 1, kernel, path_smem, &pp.lookahead)))
             return rc;
     }
     JsonParams jp{};
@@ -1685,10 +1664,8 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
         json_smem = (size_t)jp.blob_bytes + out_cap + 32;
         if (json_smem > (size_t)ctx->max_smem_optin)
             return fail(ctx, REGK_ERR_INVALID_ARG, "json kernel needs %zu B of shared memory (> %d)", json_smem, ctx->max_smem_optin);
-        if (smem_attr_needs_raise(ctx->device, 2, json_smem)) {
-            CK(cudaFuncSetAttribute(regk_json_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)json_smem));
-        }
-        if ((rc = lookahead_tiles(ctx, 2, (const void *)regk_json_kernel, json_smem, &jp.lookahead)))
+        if ((rc = set_smem_limit(ctx, (const void *)regk_json_kernel, json_smem)) ||
+            (rc = lookahead_tiles(ctx, 2, (const void *)regk_json_kernel, json_smem, &jp.lookahead)))
             return rc;
     }
 
@@ -1702,15 +1679,15 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
         hp.json_cap = json_cap;
         for (int i = 0; i < 11; i++) {
             hp.src[i] = src[i];
-            hp.dev[i] = need[i] && src[i] ? ctx->in[i].p : nullptr;
+            hp.dev[i] = need[i] && src[i] ? hs.in[i].p : nullptr;
         }
-        rc = run_pipelined(ctx, b, res, pp, path_smem, jp, json_smem, hp);
-        ctx->skip_last = regk_ctx::SkipLast{};
+        slot.set = &hs;
+        rc = run_pipelined(ctx, *slot.set, b, res, pp, path_smem, jp, json_smem, hp);
+        ctx->skip.last = {};
         if (rc == REGK_ERR_OUT_OF_DOMAIN && (b->flags & REGK_SKIP_BAD) && !(res->bad_bits & REGK_BAD_TOO_LARGE)) {
-            /* the whole batch is staged in ctx->in: redo it from there like a dirty batch in regk_finish */
+            /* the whole batch is staged in its set: redo it from there like a dirty batch in regk_finish */
             slot.n = n;
             slot.flags = b->flags;
-            slot.hset = -1;
             slot.off32 = false;                 /* the pipelined route returns 64-bit offsets */
             slot.timed = false;
             slot.launches = res->launches;
@@ -1724,27 +1701,18 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
             return finish_skip(ctx, &slot, st, res);
         }
         if (rc == REGK_OK && (b->flags & REGK_SKIP_BAD)) {
-            ctx->skip_last.valid = true;
-            ctx->skip_last.n = n;
+            ctx->skip.last.valid = true;
+            ctx->skip.last.n = n;
         }
-        if (rc == REGK_OK) {
-            ctx->last_gen++;
-            ctx->last_path_bytes = do_path ? pp.out_bytes : nullptr;
-            ctx->last_path_off = do_path ? pp.out_off : nullptr;
-            ctx->last_n = do_path ? n : 0;
-            ctx->last_json_bytes = do_json ? jp.out_bytes : nullptr;
-            ctx->last_json_off = do_json ? jp.out_off : nullptr;
-            ctx->last_json_n = do_json ? n : 0;
-            ctx->last_host_off = pp.host_off;
-            ctx->last_host_stride = pp.host_stride;
-            ctx->last_alias = alias;
-        }
+        if (rc == REGK_OK)
+            set_last(ctx, do_path ? pp.out_bytes : nullptr, do_path ? pp.out_off : nullptr, do_json ? jp.out_bytes : nullptr,
+                do_json ? jp.out_off : nullptr, n, pp.host_off, pp.host_stride, alias);
         if (rc != REGK_ERR_STATE + 100)         /* anything but "needs the exact redo" */
             return rc;
         /* some domain has empty labels: run the whole batch again through the regular (exact-capable) path */
         for (int i = 0; i < 11; i++)
             if (dev[i] && sz[i])
-                CK(cudaMemcpyAsync(ctx->in[i].p, src[i], sz[i], cudaMemcpyHostToDevice, s));
+                CK(cudaMemcpyAsync(hs.in[i].p, src[i], sz[i], cudaMemcpyHostToDevice, s));
         CK(cudaMemsetAsync(wk, 0, work_bytes, s));
     }
 
@@ -1813,9 +1781,9 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
     }
     slot.off32 = !out_dev && !job && n && opt_get(ctx, "offsets32", 0) != 0;
     if (slot.off32) {
-        if (do_path && (rc = narrow_offsets(ctx, o_path_off.p, hs ? hs->off32_p : ctx->off32_p, n, s)))
+        if (do_path && (rc = narrow_offsets(ctx, hs.path_off.p, hs.off32_p, n, s)))
             return rc;
-        if (do_json && (rc = narrow_offsets(ctx, o_json_off.p, hs ? hs->off32_j : ctx->off32_j, n, s)))
+        if (do_json && (rc = narrow_offsets(ctx, hs.json_off.p, hs.off32_j, n, s)))
             return rc;
     }
     CK(cudaEventRecord(slot.ev[3], s));
@@ -1831,7 +1799,8 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
         CK(cudaStreamWaitEvent(ctx->s_side, job ? slot.ev[5] : slot.ev[3], 0));
         CK(cudaMemcpyAsync(slot.h_status, d_status, sizeof(DevStatus), cudaMemcpyDeviceToHost, ctx->s_side));
         if (job)
-            CK(cudaMemcpyAsync(ctx->h_job_bases + 8 * (ctx->seq % regk_ctx::NSLOTS), d_bases, 64, cudaMemcpyDeviceToHost, ctx->s_side));
+            CK(cudaMemcpyAsync((unsigned long long *)ctx->h_job_bases.p + 8 * (ctx->seq % regk_ctx::NSLOTS), d_bases, 64,
+                cudaMemcpyDeviceToHost, ctx->s_side));
         CK(cudaEventRecord(slot.ev[4], ctx->s_side));
         CK(cudaMemsetAsync(wk, 0, work_bytes, ctx->s_side));
         CK(cudaEventRecord(ctx->ws_clean[ring], ctx->s_side));
@@ -1843,7 +1812,7 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
         slot.ring = -1;
     }
 
-    slot.hset = hs ? (int)(hs - ctx->hset) : -1;
+    slot.set = &hs;
     slot.job = job;
     slot.d2h_issued = false;
     slot.in_use = true;
@@ -1860,12 +1829,12 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
     res->flags = out_dev ? REGK_OUT_DEVICE : 0;
     res->launches = launches;
     res->opaque = &slot;
-    if (hs) {
+    if (two_deep) {
         /* the other set's batch, if still open: its kernels ran ahead of this batch's copies - start its D2H now
            so that it overlaps this batch's H2D */
         ctx->hseq++;
         for (auto &sl : ctx->slots)
-            if (&sl != &slot && sl.in_use && sl.hset >= 0 && !sl.d2h_issued) {
+            if (&sl != &slot && sl.in_use && ctx->is_async(sl.set) && !sl.d2h_issued) {
                 cudaError_t e = cudaEventSynchronize(sl.ev[4]);
                 if (e != cudaSuccess)
                     return fail(ctx, REGK_ERR_CUDA, "kernel execution failed: %s", cudaGetErrorString(e));
@@ -1880,8 +1849,8 @@ int regk_register_batch(regk_ctx *ctx, const regk_batch *b, regk_result *res)
 
 /*
  * Skip mode, dirty batch (regk_skip.cuh): the first pass found out-of-domain records and no REGK_BAD_TOO_LARGE.
- * Fence pass -> compaction of the kept records into ctx->skip_in -> that batch through regk_register_batch as an
- * ordinary device batch (its outputs, in ctx->path_bytes / json_bytes, are the result's streams and what the
+ * Fence pass -> compaction of the kept records into ctx->skip.in -> that batch through regk_register_batch as an
+ * ordinary device batch (its outputs, in sync_set.path_bytes / json_bytes, are the result's streams and what the
  * downstream calls on the batch finished last see) -> offsets expanded to all n records.  Timings describe the
  * first pass, as for the exact-offset redo; launches count every kernel of the call.
  */
@@ -1894,9 +1863,9 @@ static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &fir
     const bool out_dev = flags & REGK_OUT_DEVICE;
     if (ctx->pending) {
         /* the redo writes the device outputs and reads this batch's inputs: only other host-set batches may be open */
-        bool ok = slot->hset >= 0;
+        bool ok = ctx->is_async(slot->set);
         for (const auto &sl : ctx->slots)
-            if (sl.in_use && sl.hset < 0)
+            if (sl.in_use && !ctx->is_async(sl.set))
                 ok = false;
         if (!ok)
             return fail(ctx, REGK_ERR_STATE,
@@ -1915,9 +1884,9 @@ static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &fir
     const size_t tt_bytes = align16(ntiles * 4), st_bytes = nsuper * 8;
     const size_t bits_off = 128 + SKIP_Q * (tt_bytes + st_bytes);
     static_assert(sizeof(SkipStatus) <= 128, "SkipStatus");
-    if ((rc = ensure_dev(ctx, ctx->skip_work, bits_off + align16(n) + 16)) || (rc = ensure_host(ctx, ctx->h_skip_status, sizeof(SkipStatus))))
+    if ((rc = ensure_dev(ctx, ctx->skip.work, bits_off + align16(n) + 16)) || (rc = ensure_host(ctx, ctx->skip.h_status, sizeof(SkipStatus))))
         return rc;
-    uint8_t *wk = (uint8_t *)ctx->skip_work.p;
+    uint8_t *wk = (uint8_t *)ctx->skip.work.p;
     CK(cudaMemsetAsync(wk, 0, bits_off, s));
     SkipParams sp{};
     sp.n = n;
@@ -1945,11 +1914,11 @@ static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &fir
     sp.bits = wk + bits_off;
     regk_fence_kernel<<<(unsigned)ntiles, TILE, 0, s>>>(sp);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(ctx->h_skip_status.p, sp.status, sizeof(SkipStatus), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(ctx->skip.h_status.p, sp.status, sizeof(SkipStatus), cudaMemcpyDeviceToHost, s));
     cudaError_t e = cudaStreamSynchronize(s);
     if (e != cudaSuccess)
         return fail(ctx, REGK_ERR_CUDA, "skip-mode fence pass failed: %s", cudaGetErrorString(e));
-    const SkipStatus fs = *(const SkipStatus *)ctx->h_skip_status.p;
+    const SkipStatus fs = *(const SkipStatus *)ctx->skip.h_status.p;
     if (fs.bad_bits != first.bad_bits || fs.first_bad != first.first_bad)
         return fail(ctx, REGK_ERR_CUDA,
             "internal error: the skip-mode fence (bits 0x%x, first record %llu) disagrees with the compose kernels (0x%x, %llu)",
@@ -1966,11 +1935,11 @@ static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &fir
         cin[i] = nullptr;
         if (!slot->dev_in[i])
             continue;
-        if ((rc = ensure_dev(ctx, ctx->skip_in[i], csz[i] + 16)))
+        if ((rc = ensure_dev(ctx, ctx->skip.in[i], csz[i] + 16)))
             return rc;
-        cin[i] = ctx->skip_in[i].p;
+        cin[i] = ctx->skip.in[i].p;
     }
-    if ((rc = ensure_dev(ctx, ctx->skip_index, nskip * 8 + 16)) || (rc = ensure_dev(ctx, ctx->skip_bits, nskip + 16)))
+    if ((rc = ensure_dev(ctx, ctx->skip.index, nskip * 8 + 16)) || (rc = ensure_dev(ctx, ctx->skip.bits, nskip + 16)))
         return rc;
     sp.c_domain_bytes = (uint8_t *)cin[0];
     sp.c_domain_off = (uint32_t *)cin[1];
@@ -1983,8 +1952,8 @@ static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &fir
     sp.c_ports_off = (uint32_t *)cin[8];
     sp.c_ports = (uint32_t *)cin[9];
     sp.c_ports_present = (uint8_t *)cin[10];
-    sp.skip_index = (unsigned long long *)ctx->skip_index.p;
-    sp.skip_bits = (uint8_t *)ctx->skip_bits.p;
+    sp.skip_index = (unsigned long long *)ctx->skip.index.p;
+    sp.skip_bits = (uint8_t *)ctx->skip.bits.p;
     regk_compact_kernel<<<(unsigned)ntiles, TILE, 0, s>>>(sp);
     CK(cudaGetLastError());
 
@@ -2035,7 +2004,7 @@ static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &fir
         return rc;
 
     /* ---- 3. offsets of all n records ---- */
-    if ((rc = ensure_dev(ctx, ctx->skip_off_p, (n + 1) * 8)) || (rc = ensure_dev(ctx, ctx->skip_off_j, (n + 1) * 8)))
+    if ((rc = ensure_dev(ctx, ctx->skip.off_p, (n + 1) * 8)) || (rc = ensure_dev(ctx, ctx->skip.off_j, (n + 1) * 8)))
         return rc;
     ExpandParams ep{};
     ep.n = n;
@@ -2044,18 +2013,19 @@ static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &fir
     ep.super_total = sp.super_total[SKIP_REC];
     ep.c_path_off = do_path ? (const unsigned long long *)cres.path_off : nullptr;
     ep.c_json_off = do_json ? (const unsigned long long *)cres.json_off : nullptr;
-    ep.path_off = (unsigned long long *)ctx->skip_off_p.p;
-    ep.json_off = (unsigned long long *)ctx->skip_off_j.p;
+    ep.path_off = (unsigned long long *)ctx->skip.off_p.p;
+    ep.json_off = (unsigned long long *)ctx->skip.off_j.p;
     regk_expand_kernel<<<(unsigned)(n / TILE + 1), TILE, 0, s>>>(ep);
     CK(cudaGetLastError());
     if (!do_path)
-        CK(cudaMemsetAsync(ctx->skip_off_p.p, 0, (n + 1) * 8, s));
+        CK(cudaMemsetAsync(ctx->skip.off_p.p, 0, (n + 1) * 8, s));
     if (!do_json)
-        CK(cudaMemsetAsync(ctx->skip_off_j.p, 0, (n + 1) * 8, s));
+        CK(cudaMemsetAsync(ctx->skip.off_j.p, 0, (n + 1) * 8, s));
     uint32_t launches = slot->launches + 3 + cres.launches;
+    regk_ctx::HostSet &hs = *slot->set;
     const bool off32 = slot->off32 && !out_dev && cres.path_total < (1ull << 32) && cres.json_total < (1ull << 32);
     if (off32) {
-        if ((rc = narrow_offsets(ctx, ctx->skip_off_p.p, ctx->off32_p, n, s)) || (rc = narrow_offsets(ctx, ctx->skip_off_j.p, ctx->off32_j, n, s)))
+        if ((rc = narrow_offsets(ctx, ctx->skip.off_p.p, hs.off32_p, n, s)) || (rc = narrow_offsets(ctx, ctx->skip.off_j.p, hs.off32_j, n, s)))
             return rc;
         launches += 2;
     }
@@ -2075,50 +2045,38 @@ static int finish_skip(regk_ctx *ctx, regk_ctx::Slot *slot, const DevStatus &fir
     if (out_dev) {
         res->flags = REGK_OUT_DEVICE;
         res->path_bytes = cres.path_bytes;
-        res->path_off = (uint64_t *)ctx->skip_off_p.p;
+        res->path_off = (uint64_t *)ctx->skip.off_p.p;
         res->json_bytes = cres.json_bytes;
-        res->json_off = (uint64_t *)ctx->skip_off_j.p;
+        res->json_off = (uint64_t *)ctx->skip.off_j.p;
         e = cudaStreamSynchronize(s);
         if (e != cudaSuccess)
             return fail(ctx, REGK_ERR_CUDA, "skip-mode offset expansion failed: %s", cudaGetErrorString(e));
     } else {
-        regk_ctx::HostSet *hs = slot->hset >= 0 ? &ctx->hset[slot->hset] : nullptr;
-        HostBuf &hpb = hs ? hs->h_path_bytes : ctx->h_path_bytes, &hpo = hs ? hs->h_path_off : ctx->h_path_off,
-                &hjb = hs ? hs->h_json_bytes : ctx->h_json_bytes, &hjo = hs ? hs->h_json_off : ctx->h_json_off;
-        if ((rc = ensure_host(ctx, hpb, cres.path_total + 16)) || (rc = ensure_host(ctx, hpo, (n + 1) * 8)) ||
-            (rc = ensure_host(ctx, hjb, cres.json_total + 16)) || (rc = ensure_host(ctx, hjo, (n + 1) * 8)))
+        if ((rc = ensure_host(ctx, hs.h_path_bytes, cres.path_total + 16)) || (rc = ensure_host(ctx, hs.h_path_off, (n + 1) * 8)) ||
+            (rc = ensure_host(ctx, hs.h_json_bytes, cres.json_total + 16)) || (rc = ensure_host(ctx, hs.h_json_off, (n + 1) * 8)))
             return rc;
         const size_t ow = off32 ? 4 : 8;
         if (do_path) {
-            CK(cudaMemcpyAsync(hpb.p, cres.path_bytes, cres.path_total, cudaMemcpyDeviceToHost, s));
-            CK(cudaMemcpyAsync(hpo.p, off32 ? ctx->off32_p.p : ctx->skip_off_p.p, (n + 1) * ow, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(hs.h_path_bytes.p, cres.path_bytes, cres.path_total, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(hs.h_path_off.p, off32 ? hs.off32_p.p : ctx->skip.off_p.p, (n + 1) * ow, cudaMemcpyDeviceToHost, s));
         } else {
-            memset(hpo.p, 0, (n + 1) * 8);
+            memset(hs.h_path_off.p, 0, (n + 1) * 8);
         }
         if (do_json) {
-            CK(cudaMemcpyAsync(hjb.p, cres.json_bytes, cres.json_total, cudaMemcpyDeviceToHost, s));
-            CK(cudaMemcpyAsync(hjo.p, off32 ? ctx->off32_j.p : ctx->skip_off_j.p, (n + 1) * ow, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(hs.h_json_bytes.p, cres.json_bytes, cres.json_total, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(hs.h_json_off.p, off32 ? hs.off32_j.p : ctx->skip.off_j.p, (n + 1) * ow, cudaMemcpyDeviceToHost, s));
         } else {
-            memset(hjo.p, 0, (n + 1) * 8);
+            memset(hs.h_json_off.p, 0, (n + 1) * 8);
         }
         e = cudaStreamSynchronize(s);
         if (e != cudaSuccess)
             return fail(ctx, REGK_ERR_CUDA, "skip-mode result copy failed: %s", cudaGetErrorString(e));
-        res->flags = 0;
-        res->path_bytes = (uint8_t *)hpb.p;
-        res->json_bytes = (uint8_t *)hjb.p;
-        if (off32) {
-            res->path_off32 = (uint32_t *)hpo.p;
-            res->json_off32 = (uint32_t *)hjo.p;
-        } else {
-            res->path_off = (uint64_t *)hpo.p;
-            res->json_off = (uint64_t *)hjo.p;
-        }
+        host_results(res, hs, off32);
     }
-    ctx->skip_last.valid = true;
-    ctx->skip_last.n = n;
-    ctx->skip_last.n_skipped = nskip;
-    ctx->skip_last.bad_bits = fs.bad_bits;
+    ctx->skip.last.valid = true;
+    ctx->skip.last.n = n;
+    ctx->skip.last.n_skipped = nskip;
+    ctx->skip.last.bad_bits = fs.bad_bits;
     return REGK_OK;
 }
 
@@ -2126,10 +2084,10 @@ int regk_skipped_records(regk_ctx *ctx, uint32_t flags, regk_skipped *out)
 {
     if (!ctx || !out)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_skipped_records: NULL argument");
-    if (!ctx->skip_last.valid)
+    if (!ctx->skip.last.valid)
         return fail(ctx, REGK_ERR_STATE, "regk_skipped_records: the batch finished last was not a REGK_SKIP_BAD batch");
     memset(out, 0, sizeof *out);
-    const regk_ctx::SkipLast &sl = ctx->skip_last;
+    const regk_ctx::Skip::Last &sl = ctx->skip.last;
     out->n = sl.n;
     out->n_skipped = sl.n_skipped;
     out->bad_bits = sl.bad_bits;
@@ -2137,19 +2095,18 @@ int regk_skipped_records(regk_ctx *ctx, uint32_t flags, regk_skipped *out)
         return REGK_OK;
     if (flags & REGK_OUT_DEVICE) {
         out->flags = REGK_OUT_DEVICE;
-        out->index = (const uint64_t *)ctx->skip_index.p;
-        out->bits = (const uint8_t *)ctx->skip_bits.p;
+        out->index = (const uint64_t *)ctx->skip.index.p;
+        out->bits = (const uint8_t *)ctx->skip.bits.p;
         return REGK_OK;
     }
     CK(cudaSetDevice(ctx->device));
     int rc;
-    if ((rc = ensure_host(ctx, ctx->h_skip_index, sl.n_skipped * 8)) || (rc = ensure_host(ctx, ctx->h_skip_bits, sl.n_skipped)))
+    if ((rc = to_host(ctx, ctx->skip.h_index, ctx->skip.index.p, sl.n_skipped * 8, ctx->stream)) ||
+        (rc = to_host(ctx, ctx->skip.h_bits, ctx->skip.bits.p, sl.n_skipped, ctx->stream)))
         return rc;
-    CK(cudaMemcpyAsync(ctx->h_skip_index.p, ctx->skip_index.p, sl.n_skipped * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_skip_bits.p, ctx->skip_bits.p, sl.n_skipped, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    out->index = (const uint64_t *)ctx->h_skip_index.p;
-    out->bits = (const uint8_t *)ctx->h_skip_bits.p;
+    out->index = (const uint64_t *)ctx->skip.h_index.p;
+    out->bits = (const uint8_t *)ctx->skip.h_bits.p;
     return REGK_OK;
 }
 
@@ -2169,8 +2126,9 @@ int regk_finish(regk_ctx *ctx, regk_result *res)
         return fail(ctx, REGK_ERR_CUDA, "kernel execution failed: %s", cudaGetErrorString(e));
     uint32_t extra_launches = 0;
     if (slot->job) {
-        if (ctx->h_gather_flag && *ctx->h_gather_flag == 2u) {
-            *ctx->h_gather_flag = 0;
+        uint32_t *flag = (uint32_t *)ctx->h_gather_flag.p;
+        if (flag && *flag == 2u) {
+            *flag = 0;
             return fail(ctx, REGK_ERR_CUDA, "job step: a peer did not reach the exchange in time (mailbox wait timed out)");
         }
         if (slot->h_status->needs_exact && !slot->h_status->bad_bits)
@@ -2181,7 +2139,7 @@ int regk_finish(regk_ctx *ctx, regk_result *res)
     if (!slot->job && slot->h_status->needs_exact && !slot->h_status->bad_bits && slot->did_path) {
         /* Some domain has empty labels (path.join drops them): the closed-form offsets do not hold.
            Re-run the path half with exact lengths: length kernel + last-CTA scan, then compose. */
-        if (ctx->pending && slot->hset < 0)         /* device outputs are single-buffered; host sets are not */
+        if (ctx->pending && !ctx->is_async(slot->set))      /* device outputs are single-buffered; host sets are not */
             return fail(ctx, REGK_ERR_STATE,
                 "batch needs the exact-offset redo but later batches are in flight; finish them in order");
         PathParams p = slot->path_params;
@@ -2205,9 +2163,9 @@ int regk_finish(regk_ctx *ctx, regk_result *res)
             regk_path_kernel<false, true><<<ntiles_r, TILE, slot->path_smem, s>>>(p, JsonParams{});
         CK(cudaGetLastError());
         if (slot->off32) {
-            int rc2 = narrow_offsets(ctx, p.out_off, slot->hset >= 0 ? ctx->hset[slot->hset].off32_p : ctx->off32_p, p.n, s);
-            if (rc2)
-                return rc2;
+            const int rc = narrow_offsets(ctx, p.out_off, slot->set->off32_p, p.n, s);
+            if (rc)
+                return rc;
         }
         CK(cudaMemcpyAsync(slot->h_status, slot->d_status, sizeof(DevStatus), cudaMemcpyDeviceToHost, s));
         e = cudaStreamSynchronize(s);
@@ -2220,25 +2178,18 @@ int regk_finish(regk_ctx *ctx, regk_result *res)
     const DevStatus st = *slot->h_status;
     const uint64_t n = slot->n;
     const bool out_dev = slot->flags & REGK_OUT_DEVICE;
-    ctx->skip_last = regk_ctx::SkipLast{};
+    ctx->skip.last = regk_ctx::Skip::Last{};
     if (slot->flags & REGK_SKIP_BAD) {
         if (st.bad_bits && !(st.bad_bits & REGK_BAD_TOO_LARGE) && !st.overflow)
             return finish_skip(ctx, slot, st, res);
         if (!st.bad_bits) {
-            ctx->skip_last.valid = true;
-            ctx->skip_last.n = n;
+            ctx->skip.last.valid = true;
+            ctx->skip.last.n = n;
         }
     }
-    ctx->last_gen++;
-    ctx->last_path_bytes = st.bad_bits ? nullptr : slot->dev_path_bytes;
-    ctx->last_path_off = st.bad_bits ? nullptr : slot->dev_path_off;
-    ctx->last_n = (st.bad_bits || !slot->dev_path_off) ? 0 : n;
-    ctx->last_json_bytes = st.bad_bits ? nullptr : slot->dev_json_bytes;
-    ctx->last_json_off = st.bad_bits ? nullptr : slot->dev_json_off;
-    ctx->last_json_n = (st.bad_bits || !slot->dev_json_off) ? 0 : n;
-    ctx->last_host_off = slot->dev_host_off;
-    ctx->last_host_stride = slot->host_stride;
-    ctx->last_alias = slot->alias;
+    const bool ok = !st.bad_bits;
+    set_last(ctx, ok ? slot->dev_path_bytes : nullptr, ok ? slot->dev_path_off : nullptr, ok ? slot->dev_json_bytes : nullptr,
+        ok ? slot->dev_json_off : nullptr, n, slot->dev_host_off, slot->host_stride, slot->alias);
     float ms_p = 0, ms_jl = 0, ms_j = 0;
     if (slot->timed) {
         cudaEventElapsedTime(&ms_p, slot->ev[0], slot->ev[1]);
@@ -2272,7 +2223,7 @@ int regk_finish(regk_ctx *ctx, regk_result *res)
             (unsigned long long)res->first_bad, st.bad_bits);
     }
     if (slot->job) {
-        const unsigned long long *hb = ctx->h_job_bases + 8 * ((size_t)(slot - ctx->slots));
+        const unsigned long long *hb = (const unsigned long long *)ctx->h_job_bases.p + 8 * ((size_t)(slot - ctx->slots));
         res->flags = REGK_OUT_DEVICE;
         res->path_bytes = (uint8_t *)ctx->job.path_bytes[ctx->job.rank];
         res->path_off = ctx->job.path_off[ctx->job.rank];
@@ -2284,63 +2235,28 @@ int regk_finish(regk_ctx *ctx, regk_result *res)
         res->job_json_total = hb[5];
         return REGK_OK;
     }
+    regk_ctx::HostSet &hs = *slot->set;
     if (out_dev) {
         res->flags = REGK_OUT_DEVICE;
-        res->path_bytes = (uint8_t *)ctx->path_bytes.p;
-        res->path_off = (uint64_t *)ctx->path_off.p;
-        res->json_bytes = (uint8_t *)ctx->json_bytes.p;
-        res->json_off = (uint64_t *)ctx->json_off.p;
+        res->path_bytes = (uint8_t *)hs.path_bytes.p;
+        res->path_off = (uint64_t *)hs.path_off.p;
+        res->json_bytes = (uint8_t *)hs.json_bytes.p;
+        res->json_off = (uint64_t *)hs.json_off.p;
         return REGK_OK;
     }
     int rc;
-    if (slot->hset >= 0) {
-        regk_ctx::HostSet &hs = ctx->hset[slot->hset];
+    if (ctx->is_async(&hs)) {
         if (!slot->d2h_issued && (rc = issue_d2h(ctx, *slot)))
             return rc;
         e = cudaEventSynchronize(hs.e_out);
         if (e != cudaSuccess)
             return fail(ctx, REGK_ERR_CUDA, "device-to-host copy failed: %s", cudaGetErrorString(e));
-        res->flags = 0;
-        res->path_bytes = (uint8_t *)hs.h_path_bytes.p;
-        res->json_bytes = (uint8_t *)hs.h_json_bytes.p;
-        if (slot->off32) {
-            res->path_off32 = (uint32_t *)hs.h_path_off.p;
-            res->json_off32 = (uint32_t *)hs.h_json_off.p;
-        } else {
-            res->path_off = (uint64_t *)hs.h_path_off.p;
-            res->json_off = (uint64_t *)hs.h_json_off.p;
-        }
-        return REGK_OK;
-    }
-    const bool do_path = !(slot->flags & REGK_NO_PATH), do_json = !(slot->flags & REGK_NO_JSON);
-    if ((rc = ensure_host(ctx, ctx->h_path_bytes, st.path_total + 16)) || (rc = ensure_host(ctx, ctx->h_path_off, (n + 1) * 8)) ||
-        (rc = ensure_host(ctx, ctx->h_json_bytes, st.json_total + 16)) || (rc = ensure_host(ctx, ctx->h_json_off, (n + 1) * 8)))
-        return rc;
-    slot->off32 = slot->off32 && st.path_total < (1ull << 32) && st.json_total < (1ull << 32);
-    const size_t ow = slot->off32 ? 4 : 8;
-    if (n && do_path) {
-        CK(cudaMemcpyAsync(ctx->h_path_bytes.p, ctx->path_bytes.p, st.path_total, cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(ctx->h_path_off.p, slot->off32 ? ctx->off32_p.p : ctx->path_off.p, (n + 1) * ow, cudaMemcpyDeviceToHost, s));
     } else {
-        memset(ctx->h_path_off.p, 0, (n + 1) * 8);
+        if ((rc = enqueue_d2h(ctx, *slot, s)))
+            return rc;
+        CK(cudaStreamSynchronize(s));
     }
-    if (n && do_json) {
-        CK(cudaMemcpyAsync(ctx->h_json_bytes.p, ctx->json_bytes.p, st.json_total, cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(ctx->h_json_off.p, slot->off32 ? ctx->off32_j.p : ctx->json_off.p, (n + 1) * ow, cudaMemcpyDeviceToHost, s));
-    } else {
-        memset(ctx->h_json_off.p, 0, (n + 1) * 8);
-    }
-    CK(cudaStreamSynchronize(s));
-    res->flags = 0;
-    res->path_bytes = (uint8_t *)ctx->h_path_bytes.p;
-    res->json_bytes = (uint8_t *)ctx->h_json_bytes.p;
-    if (slot->off32) {
-        res->path_off32 = (uint32_t *)ctx->h_path_off.p;
-        res->json_off32 = (uint32_t *)ctx->h_json_off.p;
-    } else {
-        res->path_off = (uint64_t *)ctx->h_path_off.p;
-        res->json_off = (uint64_t *)ctx->h_json_off.p;
-    }
+    host_results(res, hs, slot->off32);
     return REGK_OK;
 }
 
@@ -2380,11 +2296,9 @@ int regk_service_records(regk_ctx *ctx, const regk_service_batch *b, regk_result
                 return fail(ctx, REGK_ERR_INVALID_ARG, "regk_service_records: device array %d is not 16-byte aligned", i);
             dev[i] = src[i];
         } else {
-            if ((rc = ensure_dev(ctx, ctx->svc_in[i], sz[i] + 16)))
+            if ((rc = stage_in(ctx, ctx->svc.in[i], src[i], sz[i], s)))
                 return rc;
-            if (sz[i])
-                CK(cudaMemcpyAsync(ctx->svc_in[i].p, src[i], sz[i], cudaMemcpyHostToDevice, s));
-            dev[i] = ctx->svc_in[i].p;
+            dev[i] = ctx->svc.in[i].p;
         }
     }
     /* 58 fixed + 3 commas + '}}}' + "srvce":"" + "proto":"" + "port": + 10 digits + "ttl": + '-' and 10 digits */
@@ -2392,13 +2306,14 @@ int regk_service_records(regk_ctx *ctx, const regk_service_batch *b, regk_result
     const uint64_t ntiles = (n + TILE - 1) / TILE;
     const size_t totals_off = 128, super_off = (totals_off + ntiles * 4 + 15) & ~(size_t)15;
     const size_t work_bytes = super_off + (ntiles / SUPER + 1) * 8 + 64;
-    if ((rc = ensure_dev(ctx, ctx->json_bytes, cap)) || (rc = ensure_dev(ctx, ctx->json_off, (n + 1) * 8)) ||
-        (rc = ensure_dev(ctx, ctx->svc_work, work_bytes)))
+    regk_ctx::HostSet &os = ctx->sync_set;      /* the payloads go where a batch's payloads go */
+    if ((rc = ensure_dev(ctx, os.json_bytes, cap)) || (rc = ensure_dev(ctx, os.json_off, (n + 1) * 8)) ||
+        (rc = ensure_dev(ctx, ctx->svc.work, work_bytes)))
         return rc;
-    uint8_t *wk = (uint8_t *)ctx->svc_work.p;
+    uint8_t *wk = (uint8_t *)ctx->svc.work.p;
     CK(cudaMemsetAsync(wk, 0, work_bytes, s));
     if (n == 0)
-        CK(cudaMemsetAsync(ctx->json_off.p, 0, 8, s));
+        CK(cudaMemsetAsync(os.json_off.p, 0, 8, s));
     regk_ctx::Slot &slot = ctx->slots[0];
     uint32_t launches = 0;
     if (n) {
@@ -2411,8 +2326,8 @@ int regk_service_records(regk_ctx *ctx, const regk_service_batch *b, regk_result
         p.port = (const uint32_t *)dev[4];
         p.ttl = (const int32_t *)dev[5];
         p.key_order = (const uint8_t *)dev[6];
-        p.out_bytes = (uint8_t *)ctx->json_bytes.p;
-        p.out_off = (unsigned long long *)ctx->json_off.p;
+        p.out_bytes = (uint8_t *)os.json_bytes.p;
+        p.out_off = (unsigned long long *)os.json_off.p;
         p.out_capacity = cap;
         p.tile_total = (uint32_t *)(wk + totals_off);
         p.super_total = (unsigned long long *)(wk + super_off);
@@ -2422,8 +2337,8 @@ int regk_service_records(regk_ctx *ctx, const regk_service_batch *b, regk_result
         const uint64_t mean = 58 + 3 + 3 + 20 + 13 + 17 + (srvce_len + proto_len) / n + 2;
         p.out_cap = (uint32_t)align16(std::min<uint64_t>(mean * TILE * 9 / 8 + 512, 98304));
         const size_t smem = (size_t)p.out_cap + 32;
-        if (smem_attr_needs_raise(ctx->device, 3, smem))
-            CK(cudaFuncSetAttribute(regk_service_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if ((rc = set_smem_limit(ctx, (const void *)regk_service_kernel, smem)))
+            return rc;
         CK(cudaEventRecord(slot.ev[0], s));
         regk_service_len_kernel<<<(unsigned)std::min<uint64_t>(ntiles, (uint64_t)ctx->sm_count * 8), TILE, 0, s>>>(p, (uint32_t)ntiles);
         CK(cudaGetLastError());
@@ -2433,9 +2348,8 @@ int regk_service_records(regk_ctx *ctx, const regk_service_batch *b, regk_result
         launches = 2;
     }
     CK(cudaMemcpyAsync(slot.h_status, wk, sizeof(DevStatus), cudaMemcpyDeviceToHost, s));
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_service_records: kernel execution failed: %s", cudaGetErrorString(e));
+    if ((rc = sync_or_fail(ctx, s, "regk_service_records")))
+        return rc;
     const DevStatus st = *slot.h_status;
     res->n = n;
     res->launches = launches;
@@ -2453,23 +2367,19 @@ int regk_service_records(regk_ctx *ctx, const regk_service_batch *b, regk_result
             "service record %llu is outside the supported input domain (REGK_BAD bits 0x%x); no output produced",
             (unsigned long long)res->first_bad, st.bad_bits);
     res->json_total = st.json_total;
-    ctx->last_gen++;
-    ctx->last_path_off = nullptr;                   /* the payload buffers were reused */
-    ctx->last_json_off = nullptr;
+    set_last(ctx, nullptr, nullptr, nullptr, nullptr, 0, nullptr, 0, false);      /* the payload buffers were reused */
     if (out_dev) {
         res->flags = REGK_OUT_DEVICE;
-        res->json_bytes = (uint8_t *)ctx->json_bytes.p;
-        res->json_off = (uint64_t *)ctx->json_off.p;
+        res->json_bytes = (uint8_t *)os.json_bytes.p;
+        res->json_off = (uint64_t *)os.json_off.p;
         return REGK_OK;
     }
-    if ((rc = ensure_host(ctx, ctx->h_json_bytes, st.json_total + 16)) || (rc = ensure_host(ctx, ctx->h_json_off, (n + 1) * 8)))
+    if ((rc = to_host(ctx, os.h_json_bytes, os.json_bytes.p, st.json_total, s)) ||
+        (rc = to_host(ctx, os.h_json_off, os.json_off.p, (n + 1) * 8, s)))
         return rc;
-    if (st.json_total)
-        CK(cudaMemcpyAsync(ctx->h_json_bytes.p, ctx->json_bytes.p, st.json_total, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(ctx->h_json_off.p, ctx->json_off.p, (n + 1) * 8, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    res->json_bytes = (uint8_t *)ctx->h_json_bytes.p;
-    res->json_off = (uint64_t *)ctx->h_json_off.p;
+    res->json_bytes = (uint8_t *)os.h_json_bytes.p;
+    res->json_off = (uint64_t *)os.h_json_off.p;
     return REGK_OK;
 }
 
@@ -2500,17 +2410,17 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
     const bool has_data = o->op != REGK_ZK_DELETE && !getdata;
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "regk_jute_requests: batches are still in flight; finish them first");
-    if (!ctx->last_path_off || (has_data && (!ctx->last_json_off || ctx->last_n != ctx->last_json_n)))
+    if (!ctx->last.path_off || (has_data && (!ctx->last.json_off || ctx->last.n != ctx->last.json_n)))
         return fail(ctx, REGK_ERR_STATE, "regk_jute_requests: no finished batch with %s on this context",
             has_data ? "both a path and a payload stream" : "a path stream");
-    const FrameSrc src{ctx->last_n, ctx->last_path_bytes, ctx->last_path_off, has_data ? ctx->last_json_bytes : nullptr,
-                       has_data ? ctx->last_json_off : nullptr};
-    const int rc = frame_requests(ctx, src, o, ctx->jute_bytes, ctx->jute_off, ctx->h_jute_bytes, ctx->h_jute_off, out);
+    const FrameSrc src{ctx->last.n, ctx->last.path_bytes, ctx->last.path_off, has_data ? ctx->last.json_bytes : nullptr,
+                       has_data ? ctx->last.json_off : nullptr};
+    const int rc = frame_requests(ctx, src, o, ctx->frames, out);
     if (rc == REGK_OK && getdata) {
         ctx->gd_valid = true;
-        ctx->gd_gen = ctx->last_gen;
+        ctx->gd_gen = ctx->last.gen;
         ctx->gd_xid = o->xid_base;
-        ctx->gd_n = ctx->last_n;
+        ctx->gd_n = ctx->last.n;
     }
     return rc;
 }
@@ -2532,13 +2442,13 @@ int regk_decode(regk_ctx *ctx, const regk_decode_in *in, regk_decode_out *out)
     const uint64_t *po = in->path_off, *jo = in->json_off;
     int rc;
     if (last) {
-        if (!ctx->last_path_off && !ctx->last_json_off)
+        if (!ctx->last.path_off && !ctx->last.json_off)
             return fail(ctx, REGK_ERR_STATE, "regk_decode: no finished batch on this context");
-        n = ctx->last_path_off ? ctx->last_n : ctx->last_json_n;
-        pb = ctx->last_path_off ? ctx->last_path_bytes : nullptr;
-        po = (const uint64_t *)ctx->last_path_off;
-        jb = ctx->last_json_off ? ctx->last_json_bytes : nullptr;
-        jo = (const uint64_t *)ctx->last_json_off;
+        n = ctx->last.path_off ? ctx->last.n : ctx->last.json_n;
+        pb = ctx->last.path_off ? ctx->last.path_bytes : nullptr;
+        po = (const uint64_t *)ctx->last.path_off;
+        jb = ctx->last.json_off ? ctx->last.json_bytes : nullptr;
+        jo = (const uint64_t *)ctx->last.json_off;
         unsigned long long tot[2] = {0, 0};
         if (po)
             CK(cudaMemcpyAsync(&tot[0], po + n, 8, cudaMemcpyDeviceToHost, s));
@@ -2567,11 +2477,9 @@ int regk_decode(regk_ctx *ctx, const regk_decode_in *in, regk_decode_out *out)
             for (int i = 0; i < 4; i++) {
                 if (!src[i] || !n || ((i == 0 || i == 2) && !src[i + 1]))
                     continue;
-                if ((rc = ensure_dev(ctx, ctx->dec_in[i], sz[i] + 16)))
+                if ((rc = stage_in(ctx, ctx->dec.in[i], src[i], sz[i], s)))
                     return rc;
-                if (sz[i])
-                    CK(cudaMemcpyAsync(ctx->dec_in[i].p, src[i], sz[i], cudaMemcpyHostToDevice, s));
-                dev[i] = ctx->dec_in[i].p;
+                dev[i] = ctx->dec.in[i].p;
             }
             pb = (const uint8_t *)dev[0];
             po = (const uint64_t *)dev[1];
@@ -2584,8 +2492,8 @@ int regk_decode(regk_ctx *ctx, const regk_decode_in *in, regk_decode_out *out)
     if (!jo)
         jb = nullptr;
     const uint64_t ports_len = json_total / 2 + 1;
-    if ((rc = ensure_dev(ctx, ctx->dec_rec, (n + 1) * sizeof(Decoded))) || (rc = ensure_dev(ctx, ctx->dec_dom, path_total + 16)) ||
-        (rc = ensure_dev(ctx, ctx->dec_ports, ports_len * 4 + 16)))
+    if ((rc = ensure_dev(ctx, ctx->dec.rec, (n + 1) * sizeof(Decoded))) || (rc = ensure_dev(ctx, ctx->dec.dom, path_total + 16)) ||
+        (rc = ensure_dev(ctx, ctx->dec.ports, ports_len * 4 + 16)))
         return rc;
     out->n = n;
     out->flags = dev_out ? REGK_OUT_DEVICE : 0;
@@ -2595,14 +2503,14 @@ int regk_decode(regk_ctx *ctx, const regk_decode_in *in, regk_decode_out *out)
     if (n) {
         DecodeParams p{};
         p.n = n;
-        p.path_bytes = po ? (pb ? pb : (const uint8_t *)ctx->dec_dom.p) : nullptr;     /* an empty stream still has offsets */
+        p.path_bytes = po ? (pb ? pb : (const uint8_t *)ctx->dec.dom.p) : nullptr;     /* an empty stream still has offsets */
         p.path_off = (const unsigned long long *)po;
-        p.json_bytes = jo ? (jb ? jb : (const uint8_t *)ctx->dec_dom.p) : nullptr;
+        p.json_bytes = jo ? (jb ? jb : (const uint8_t *)ctx->dec.dom.p) : nullptr;
         p.json_off = (const unsigned long long *)jo;
         p.host_nodes = in->host_nodes;
-        p.out = (Decoded *)ctx->dec_rec.p;
-        p.dom_bytes = (uint8_t *)ctx->dec_dom.p;
-        p.ports = (uint32_t *)ctx->dec_ports.p;
+        p.out = (Decoded *)ctx->dec.rec.p;
+        p.dom_bytes = (uint8_t *)ctx->dec.dom.p;
+        p.ports = (uint32_t *)ctx->dec.ports.p;
         /* staging budgets: 9/8 of a tile's mean share of each stream plus slack; streams handed in by the caller
            carry no slack behind their last byte, the library's own buffers have >= 16 bytes */
         p.path_cap = (uint32_t)align16(std::min<uint64_t>(path_total * DEC_TILE / n * 9 / 8 + 1024, 49152));
@@ -2613,46 +2521,38 @@ int regk_decode(regk_ctx *ctx, const regk_decode_in *in, regk_decode_out *out)
         /* [path slice, later the result records][slash bitmap][payload slice, later the domain image] (regk_decode.cuh) */
         const size_t dsmem = std::max<size_t>((size_t)p.path_cap + 32, DEC_TILE * sizeof(Decoded)) + ((p.path_cap / 8 + 47) & ~15u) +
             std::max<size_t>(p.json_cap, p.path_cap) + 32 + 16;
-        {
-            static std::mutex mu;
-            static size_t high[64];
-            std::lock_guard<std::mutex> lock(mu);
-            if (dsmem > high[ctx->device & 63]) {
-                CK(cudaFuncSetAttribute(regk_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dsmem));
-                high[ctx->device & 63] = dsmem;
-            }
-        }
+        if ((rc = set_smem_limit(ctx, (const void *)regk_decode_kernel, dsmem)))
+            return rc;
         CK(cudaEventRecord(e0, s));
         regk_decode_kernel<<<(unsigned)((n + DEC_TILE - 1) / DEC_TILE), DEC_TILE, dsmem, s>>>(p);
         CK(cudaGetLastError());
         CK(cudaEventRecord(e1, s));
         out->launches = 1;
     }
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_decode: kernel execution failed: %s", cudaGetErrorString(e));
+    if ((rc = sync_or_fail(ctx, s, "regk_decode")))
+        return rc;
     if (n)
         cudaEventElapsedTime(&out->kernel_ms, e0, e1);
     if (dev_out) {
-        out->rec = (const regk_decoded *)ctx->dec_rec.p;
-        out->dom_bytes = (const uint8_t *)ctx->dec_dom.p;
-        out->ports = (const uint32_t *)ctx->dec_ports.p;
+        out->rec = (const regk_decoded *)ctx->dec.rec.p;
+        out->dom_bytes = (const uint8_t *)ctx->dec.dom.p;
+        out->ports = (const uint32_t *)ctx->dec.ports.p;
         return REGK_OK;
     }
-    if ((rc = ensure_host(ctx, ctx->h_dec_rec, (n + 1) * sizeof(Decoded))) || (rc = ensure_host(ctx, ctx->h_dec_dom, path_total + 16)) ||
-        (rc = ensure_host(ctx, ctx->h_dec_ports, ports_len * 4 + 16)))
+    if ((rc = ensure_host(ctx, ctx->dec.h_rec, (n + 1) * sizeof(Decoded))) || (rc = ensure_host(ctx, ctx->dec.h_dom, path_total + 16)) ||
+        (rc = ensure_host(ctx, ctx->dec.h_ports, ports_len * 4 + 16)))
         return rc;
     if (n) {
-        CK(cudaMemcpyAsync(ctx->h_dec_rec.p, ctx->dec_rec.p, n * sizeof(Decoded), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(ctx->dec.h_rec.p, ctx->dec.rec.p, n * sizeof(Decoded), cudaMemcpyDeviceToHost, s));
         if (po && path_total)
-            CK(cudaMemcpyAsync(ctx->h_dec_dom.p, ctx->dec_dom.p, path_total, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(ctx->dec.h_dom.p, ctx->dec.dom.p, path_total, cudaMemcpyDeviceToHost, s));
         if (jo)
-            CK(cudaMemcpyAsync(ctx->h_dec_ports.p, ctx->dec_ports.p, ports_len * 4, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(ctx->dec.h_ports.p, ctx->dec.ports.p, ports_len * 4, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
     }
-    out->rec = (const regk_decoded *)ctx->h_dec_rec.p;
-    out->dom_bytes = (const uint8_t *)ctx->h_dec_dom.p;
-    out->ports = (const uint32_t *)ctx->h_dec_ports.p;
+    out->rec = (const regk_decoded *)ctx->dec.h_rec.p;
+    out->dom_bytes = (const uint8_t *)ctx->dec.h_dom.p;
+    out->ports = (const uint32_t *)ctx->dec.h_ports.p;
     return REGK_OK;
 }
 
@@ -2663,9 +2563,9 @@ int regk_parent_dirs(regk_ctx *ctx, uint32_t flags, regk_parents *out)
     memset(out, 0, sizeof *out);
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "regk_parent_dirs: batches are still in flight; finish them first");
-    if (!ctx->last_path_off || !ctx->last_path_bytes)
+    if (!ctx->last.path_off || !ctx->last.path_bytes)
         return fail(ctx, REGK_ERR_STATE, "regk_parent_dirs: no finished batch with a path stream on this context");
-    const uint64_t n = ctx->last_n;
+    const uint64_t n = ctx->last.n;
     if (n >= 0xFFFFFFFEull)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_parent_dirs: batch too large");
     CK(cudaSetDevice(ctx->device));
@@ -2676,25 +2576,19 @@ int regk_parent_dirs(regk_ctx *ctx, uint32_t flags, regk_parents *out)
     if (n == 0)
         return REGK_OK;
     int rc;
-    if ((rc = ensure_host(ctx, ctx->h_par_count, 8)))
+    if ((rc = ensure_host(ctx, ctx->par.h_count, 8)) || (rc = ensure_event(ctx, ctx->par.ev[0])) || (rc = ensure_event(ctx, ctx->par.ev[1])))
         return rc;
-    if (!ctx->par_ev[0]) {
-        CK(cudaEventCreate(&ctx->par_ev[0]));
-        CK(cudaEventCreate(&ctx->par_ev[1]));
-    }
-    cudaEvent_t e0 = ctx->par_ev[0], e1 = ctx->par_ev[1];
+    cudaEvent_t e0 = ctx->par.ev[0], e1 = ctx->par.ev[1];
     ParentParams p{};
-    if ((rc = enqueue_parent_pass(ctx, ctx->par_len, ctx->par_slot, ctx->par_table, ctx->par_totals, ctx->par_unique, n, e0, &p)))
+    if ((rc = enqueue_parent_pass(ctx, ctx->par.pass, n, e0, &p)))
         return rc;
     CK(cudaEventRecord(e1, s));
-    CK(cudaMemcpyAsync(ctx->h_par_count.p, p.n_unique, 8, cudaMemcpyDeviceToHost, s));
-    cudaError_t e = cudaStreamSynchronize(s);
+    CK(cudaMemcpyAsync(ctx->par.h_count.p, p.n_unique, 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, "regk_parent_dirs")))
+        return rc;
     float ms = 0;
-    if (e == cudaSuccess)
-        cudaEventElapsedTime(&ms, e0, e1);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_parent_dirs: kernel execution failed: %s", cudaGetErrorString(e));
-    const uint64_t nu = *(const unsigned long long *)ctx->h_par_count.p;
+    cudaEventElapsedTime(&ms, e0, e1);
+    const uint64_t nu = *(const unsigned long long *)ctx->par.h_count.p;
     out->n_unique = nu;
     out->launches = 3;
     out->kernel_ms = ms;
@@ -2703,13 +2597,11 @@ int regk_parent_dirs(regk_ctx *ctx, uint32_t flags, regk_parents *out)
         out->unique_first = (const uint64_t *)p.unique_first;
         return REGK_OK;
     }
-    if ((rc = ensure_host(ctx, ctx->h_par_len, n * 4)) || (rc = ensure_host(ctx, ctx->h_par_unique, nu * 8 + 8)))
+    if ((rc = to_host(ctx, ctx->par.h_len, p.parent_len, n * 4, s)) || (rc = to_host(ctx, ctx->par.h_unique, p.unique_first, nu * 8, s)))
         return rc;
-    CK(cudaMemcpyAsync(ctx->h_par_len.p, p.parent_len, n * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(ctx->h_par_unique.p, p.unique_first, nu * 8, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    out->parent_len = (const uint32_t *)ctx->h_par_len.p;
-    out->unique_first = (const uint64_t *)ctx->h_par_unique.p;
+    out->parent_len = (const uint32_t *)ctx->par.h_len.p;
+    out->unique_first = (const uint64_t *)ctx->par.h_unique.p;
     return REGK_OK;
 }
 
@@ -2720,30 +2612,27 @@ int regk_mkdirp_dirs(regk_ctx *ctx, uint32_t flags, regk_dirs *out)
     memset(out, 0, sizeof *out);
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "regk_mkdirp_dirs: batches are still in flight; finish them first");
-    if (!ctx->last_path_off || !ctx->last_path_bytes)
+    if (!ctx->last.path_off || !ctx->last.path_bytes)
         return fail(ctx, REGK_ERR_STATE, "regk_mkdirp_dirs: no finished batch with a path stream on this context");
-    const uint64_t n = ctx->last_n;
+    const uint64_t n = ctx->last.n;
     if (n >= 0xFFFFFFFEull)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_mkdirp_dirs: batch too large");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     const bool dev_out = flags & REGK_OUT_DEVICE;
-    ctx->mk_valid = false;
-    DevBuf *mk = ctx->mk;
+    ctx->mk.valid = false;
+    regk_ctx::Mkdirp &mk = ctx->mk;
     int rc;
-    if ((rc = ensure_host(ctx, ctx->h_mk_count, 64)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_COUNT], 64)))
+    if ((rc = ensure_host(ctx, mk.h_count, 64)) || (rc = ensure_dev(ctx, mk.count, 64)))
         return rc;
-    for (auto &ev : ctx->mk_ev)
-        if (!ev)
-            CK(cudaEventCreate(&ev));
-    unsigned long long *hc = (unsigned long long *)ctx->h_mk_count.p;
-    unsigned long long *dc = (unsigned long long *)mk[regk_ctx::MK_COUNT].p;
+    for (Event &ev : mk.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
+    unsigned long long *hc = (unsigned long long *)mk.h_count.p;
+    unsigned long long *dc = (unsigned long long *)mk.count.p;
     auto read_counters = [&](const void *src, size_t bytes) -> int {
         CK(cudaMemcpyAsync(hc, src, bytes, cudaMemcpyDeviceToHost, s));
-        const cudaError_t e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess)
-            return fail(ctx, REGK_ERR_CUDA, "regk_mkdirp_dirs: kernel execution failed: %s", cudaGetErrorString(e));
-        return REGK_OK;
+        return sync_or_fail(ctx, s, "regk_mkdirp_dirs");
     };
     std::vector<uint64_t> depth_off(1, 0);
     uint64_t n_invalid = 0, n_dirs = 0, bytes = 0;
@@ -2752,36 +2641,35 @@ int regk_mkdirp_dirs(regk_ctx *ctx, uint32_t flags, regk_dirs *out)
     if (n) {
         /* 1. the distinct immediate directories, on buffers of its own (regk_parent_dirs' results stay as they are) */
         ParentParams pp{};
-        if ((rc = enqueue_parent_pass(ctx, mk[regk_ctx::MK_PLEN], mk[regk_ctx::MK_PSLOT], mk[regk_ctx::MK_PTABLE],
-                 mk[regk_ctx::MK_PTOTALS], mk[regk_ctx::MK_PUNIQUE], n, ctx->mk_ev[0], &pp)))
+        if ((rc = enqueue_parent_pass(ctx, mk.pass, n, mk.ev[0], &pp)))
             return rc;
         launches += 3;
-        CK(cudaEventRecord(ctx->mk_ev[1], s));
+        CK(cudaEventRecord(mk.ev[1], s));
         if ((rc = read_counters(pp.n_unique, 8)))
             return rc;
         const uint64_t nu = hc[0];
         /* workspace for up to nu items per pass: flags, two work lists, two-level totals of two counts */
         const uint64_t ntiles = (nu + MK_TILE - 1) / MK_TILE, tt = align16(ntiles * 4), st = (ntiles / SUPER + 1) * 8;
         const size_t totals_bytes = 2 * tt + 2 * st + 16;
-        if ((rc = ensure_dev(ctx, mk[regk_ctx::MK_FLAGS], nu + 16)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_LIST0], nu * 16 + 16)) ||
-            (rc = ensure_dev(ctx, mk[regk_ctx::MK_LIST1], nu * 16 + 16)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_TOTALS], totals_bytes)) ||
-            (rc = ensure_dev(ctx, mk[regk_ctx::MK_INVALID], nu * 8 + 8)))
+        if ((rc = ensure_dev(ctx, mk.flags, nu + 16)) || (rc = ensure_dev(ctx, mk.list[0], nu * 16 + 16)) ||
+            (rc = ensure_dev(ctx, mk.list[1], nu * 16 + 16)) || (rc = ensure_dev(ctx, mk.totals, totals_bytes)) ||
+            (rc = ensure_dev(ctx, mk.invalid, nu * 8 + 8)))
             return rc;
-        uint8_t *tb = (uint8_t *)mk[regk_ctx::MK_TOTALS].p;
+        uint8_t *tb = (uint8_t *)mk.totals.p;
         MkdirpParams p{};
-        p.path_bytes = ctx->last_path_bytes;
-        p.path_off = ctx->last_path_off;
+        p.path_bytes = ctx->last.path_bytes;
+        p.path_off = ctx->last.path_off;
         p.parent_len = pp.parent_len;
         p.unique_first = pp.unique_first;
         p.n_unique = nu;
-        p.flags = (uint8_t *)mk[regk_ctx::MK_FLAGS].p;
+        p.flags = (uint8_t *)mk.flags.p;
         p.tile_a = (uint32_t *)tb;
         p.tile_b = (uint32_t *)(tb + tt);
         p.super_a = (unsigned long long *)(tb + 2 * tt);
         p.super_b = (unsigned long long *)(tb + 2 * tt + st);
         p.counters = dc;
-        p.invalid = (unsigned long long *)mk[regk_ctx::MK_INVALID].p;
-        uint4 *list[2] = {(uint4 *)mk[regk_ctx::MK_LIST0].p, (uint4 *)mk[regk_ctx::MK_LIST1].p};
+        p.invalid = (unsigned long long *)mk.invalid.p;
+        uint4 *list[2] = {(uint4 *)mk.list[0].p, (uint4 *)mk.list[1].p};
         CK(cudaMemsetAsync(dc, 0, 64, s));
         /* 2. root / invalid / depth of each; the invalid list and the depth-1 work list */
         p.m = nu;
@@ -2810,13 +2698,13 @@ int regk_mkdirp_dirs(regk_ctx *ctx, uint32_t flags, regk_dirs *out)
         if (slots > (1ull << 32))
             return fail(ctx, REGK_ERR_INVALID_ARG, "regk_mkdirp_dirs: %llu directory entries are too many for one table",
                 (unsigned long long)entries);
-        if ((rc = ensure_dev(ctx, mk[regk_ctx::MK_TABLE], slots * 8)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DREC], entries * 8 + 8)) ||
-            (rc = ensure_dev(ctx, mk[regk_ctx::MK_DLEN], entries * 4 + 8)))
+        if ((rc = ensure_dev(ctx, mk.table, slots * 8)) || (rc = ensure_dev(ctx, mk.drec, entries * 8 + 8)) ||
+            (rc = ensure_dev(ctx, mk.dlen, entries * 4 + 8)))
             return rc;
-        p.table = (unsigned long long *)mk[regk_ctx::MK_TABLE].p;
+        p.table = (unsigned long long *)mk.table.p;
         p.mask = (uint32_t)(slots - 1);
-        p.dir_rec = (unsigned long long *)mk[regk_ctx::MK_DREC].p;
-        p.dir_len = (uint32_t *)mk[regk_ctx::MK_DLEN].p;
+        p.dir_rec = (unsigned long long *)mk.drec.p;
+        p.dir_len = (uint32_t *)mk.dlen.p;
         CK(cudaMemsetAsync(p.table, 0, slots * 8, s));
         /* 4. one depth at a time: extend + insert, mark, split; the host reads how many directories and entries remain */
         for (int cur = 0; m; cur ^= 1) {
@@ -2838,54 +2726,53 @@ int regk_mkdirp_dirs(regk_ctx *ctx, uint32_t flags, regk_dirs *out)
             m = hc[1];
             bytes = hc[2];
         }
-        CK(cudaEventRecord(ctx->mk_ev[2], s));
+        CK(cudaEventRecord(mk.ev[2], s));
         /* 5. dir_off and the packed bytes */
         const uint64_t dt = (n_dirs + MK_TILE - 1) / MK_TILE, dtt = dt * 8, dst = (dt / SUPER + 1) * 8;
-        if ((rc = ensure_dev(ctx, mk[regk_ctx::MK_DBYTES], bytes + 16)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DOFF], (n_dirs + 1) * 8)) ||
-            (rc = ensure_dev(ctx, mk[regk_ctx::MK_TOTALS], dtt + dst + 16)))
+        if ((rc = ensure_dev(ctx, mk.dbytes, bytes + 16)) || (rc = ensure_dev(ctx, mk.doff, (n_dirs + 1) * 8)) ||
+            (rc = ensure_dev(ctx, mk.totals, dtt + dst + 16)))
             return rc;
         if (n_dirs) {
             MkGatherParams g{};
             g.n_dirs = n_dirs;
-            g.path_bytes = ctx->last_path_bytes;
-            g.path_off = ctx->last_path_off;
+            g.path_bytes = ctx->last.path_bytes;
+            g.path_off = ctx->last.path_off;
             g.dir_rec = p.dir_rec;
             g.dir_len = p.dir_len;
-            g.tile_total = (unsigned long long *)mk[regk_ctx::MK_TOTALS].p;
-            g.super_total = (unsigned long long *)((uint8_t *)mk[regk_ctx::MK_TOTALS].p + dtt);
-            g.dir_bytes = (uint8_t *)mk[regk_ctx::MK_DBYTES].p;
-            g.dir_off = (unsigned long long *)mk[regk_ctx::MK_DOFF].p;
+            g.tile_total = (unsigned long long *)mk.totals.p;
+            g.super_total = (unsigned long long *)((uint8_t *)mk.totals.p + dtt);
+            g.dir_bytes = (uint8_t *)mk.dbytes.p;
+            g.dir_off = (unsigned long long *)mk.doff.p;
             CK(cudaMemsetAsync(g.super_total, 0, dst, s));
             regk_mkdirp_len_kernel<<<(unsigned)dt, MK_TILE, 0, s>>>(g);
             regk_mkdirp_gather_kernel<<<(unsigned)dt, MK_TILE, 0, s>>>(g);
             CK(cudaGetLastError());
             launches += 2;
         } else {
-            CK(cudaMemsetAsync(mk[regk_ctx::MK_DOFF].p, 0, 8, s));
+            CK(cudaMemsetAsync(mk.doff.p, 0, 8, s));
         }
-        CK(cudaEventRecord(ctx->mk_ev[3], s));
-        const cudaError_t e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess)
-            return fail(ctx, REGK_ERR_CUDA, "regk_mkdirp_dirs: kernel execution failed: %s", cudaGetErrorString(e));
-        for (int k = 0; k < 3; k++)
-            cudaEventElapsedTime(&ms[k], ctx->mk_ev[k], ctx->mk_ev[k + 1]);
-    } else {
-        if ((rc = ensure_dev(ctx, mk[regk_ctx::MK_DOFF], 8)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DBYTES], 16)) ||
-            (rc = ensure_dev(ctx, mk[regk_ctx::MK_DREC], 8)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DLEN], 8)) ||
-            (rc = ensure_dev(ctx, mk[regk_ctx::MK_INVALID], 8)))
+        CK(cudaEventRecord(mk.ev[3], s));
+        if ((rc = sync_or_fail(ctx, s, "regk_mkdirp_dirs")))
             return rc;
-        CK(cudaMemsetAsync(mk[regk_ctx::MK_DOFF].p, 0, 8, s));
+        for (int k = 0; k < 3; k++)
+            cudaEventElapsedTime(&ms[k], mk.ev[k], mk.ev[k + 1]);
+    } else {
+        if ((rc = ensure_dev(ctx, mk.doff, 8)) || (rc = ensure_dev(ctx, mk.dbytes, 16)) ||
+            (rc = ensure_dev(ctx, mk.drec, 8)) || (rc = ensure_dev(ctx, mk.dlen, 8)) ||
+            (rc = ensure_dev(ctx, mk.invalid, 8)))
+            return rc;
+        CK(cudaMemsetAsync(mk.doff.p, 0, 8, s));
     }
     /* depth_off was counted on the host; the device result gets a copy */
     const size_t nd1 = depth_off.size();
-    if ((rc = ensure_host(ctx, ctx->h_mk_depth, nd1 * 8)) || (rc = ensure_dev(ctx, mk[regk_ctx::MK_DEPTH], nd1 * 8)))
+    if ((rc = ensure_host(ctx, mk.h_depth, nd1 * 8)) || (rc = ensure_dev(ctx, mk.depth, nd1 * 8)))
         return rc;
-    memcpy(ctx->h_mk_depth.p, depth_off.data(), nd1 * 8);
-    CK(cudaMemcpyAsync(mk[regk_ctx::MK_DEPTH].p, ctx->h_mk_depth.p, nd1 * 8, cudaMemcpyHostToDevice, s));
+    memcpy(mk.h_depth.p, depth_off.data(), nd1 * 8);
+    CK(cudaMemcpyAsync(mk.depth.p, mk.h_depth.p, nd1 * 8, cudaMemcpyHostToDevice, s));
     CK(cudaStreamSynchronize(s));
-    ctx->mk_valid = true;
-    ctx->mk_n_dirs = n_dirs;
-    ctx->mk_bytes = bytes;
+    mk.valid = true;
+    mk.n_dirs = n_dirs;
+    mk.bytes = bytes;
     out->n = n;
     out->n_dirs = n_dirs;
     out->n_invalid = n_invalid;
@@ -2897,21 +2784,15 @@ int regk_mkdirp_dirs(regk_ctx *ctx, uint32_t flags, regk_dirs *out)
     out->closure_ms = ms[1];
     out->gather_ms = ms[2];
     out->kernel_ms = ms[0] + ms[1] + ms[2];
-    const void *dsrc[6] = {mk[regk_ctx::MK_DREC].p, mk[regk_ctx::MK_DLEN].p, mk[regk_ctx::MK_DEPTH].p, mk[regk_ctx::MK_DBYTES].p,
-                           mk[regk_ctx::MK_DOFF].p, mk[regk_ctx::MK_INVALID].p};
+    const void *dsrc[6] = {mk.drec.p, mk.dlen.p, mk.depth.p, mk.dbytes.p, mk.doff.p, mk.invalid.p};
     if (!dev_out) {
-        HostBuf *hb[6] = {&ctx->h_mk_drec, &ctx->h_mk_dlen, &ctx->h_mk_depth, &ctx->h_mk_dbytes, &ctx->h_mk_doff, &ctx->h_mk_invalid};
+        HostBuf *hb[6] = {&mk.h_drec, &mk.h_dlen, &mk.h_depth, &mk.h_dbytes, &mk.h_doff, &mk.h_invalid};
         const size_t sz[6] = {n_dirs * 8, n_dirs * 4, 0, bytes, (n_dirs + 1) * 8, n_invalid * 8};
         for (int k = 0; k < 6; k++) {
-            if (k == 2)
-                continue;                               /* already on the host */
-            if ((rc = ensure_host(ctx, *hb[k], sz[k] + 16)))
+            if (k != 2 && (rc = to_host(ctx, *hb[k], dsrc[k], sz[k], s)))       /* depth_off is on the host already */
                 return rc;
-            if (sz[k])
-                CK(cudaMemcpyAsync(hb[k]->p, dsrc[k], sz[k], cudaMemcpyDeviceToHost, s));
             dsrc[k] = hb[k]->p;
         }
-        dsrc[2] = ctx->h_mk_depth.p;
         CK(cudaStreamSynchronize(s));
     }
     out->dir_rec = (const uint64_t *)dsrc[0];
@@ -2930,24 +2811,24 @@ int regk_mkdirp_requests(regk_ctx *ctx, int32_t xid_base, uint32_t zk_flags, uin
     memset(out, 0, sizeof *out);
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "regk_mkdirp_requests: batches are still in flight; finish them first");
-    if (!ctx->mk_valid)
+    if (!ctx->mk.valid)
         return fail(ctx, REGK_ERR_STATE, "regk_mkdirp_requests: no directory set on this context; call regk_mkdirp_dirs first");
     CK(cudaSetDevice(ctx->device));
-    const uint64_t nd = ctx->mk_n_dirs;
+    const uint64_t nd = ctx->mk.n_dirs;
     int rc;
     /* CreateRequest with an empty data buffer: the payload offsets are all zero */
-    if ((rc = ensure_dev(ctx, ctx->mk[regk_ctx::MK_ZERO], (nd + 1) * 8)))
+    if ((rc = ensure_dev(ctx, ctx->mk.zero, (nd + 1) * 8)))
         return rc;
-    CK(cudaMemsetAsync(ctx->mk[regk_ctx::MK_ZERO].p, 0, (nd + 1) * 8, ctx->stream));
+    CK(cudaMemsetAsync(ctx->mk.zero.p, 0, (nd + 1) * 8, ctx->stream));
     regk_jute_opts o{};
     o.op = REGK_ZK_CREATE;
     o.flags = flags;
     o.xid_base = xid_base;
     o.zk_flags = zk_flags;
-    FrameSrc src{nd, (const uint8_t *)ctx->mk[regk_ctx::MK_DBYTES].p, (const unsigned long long *)ctx->mk[regk_ctx::MK_DOFF].p,
-                 (const uint8_t *)ctx->mk[regk_ctx::MK_DBYTES].p, (const unsigned long long *)ctx->mk[regk_ctx::MK_ZERO].p};
+    FrameSrc src{nd, (const uint8_t *)ctx->mk.dbytes.p, (const unsigned long long *)ctx->mk.doff.p,
+                 (const uint8_t *)ctx->mk.dbytes.p, (const unsigned long long *)ctx->mk.zero.p};
     src.who = "regk_mkdirp_requests";
-    return frame_requests(ctx, src, &o, ctx->mk[regk_ctx::MK_FBYTES], ctx->mk[regk_ctx::MK_FOFF], ctx->h_mk_fbytes, ctx->h_mk_foff, out);
+    return frame_requests(ctx, src, &o, ctx->mk.frames, out);
 }
 
 /* regk_reconcile (st == NULL) and regk_reconcile_owned: one implementation, the same four passes; `rep` / `n_rep` receive
@@ -2955,15 +2836,15 @@ int regk_mkdirp_requests(regk_ctx *ctx, int32_t xid_base, uint32_t zk_flags, uin
 static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_node_stat *st, uint32_t flags, regk_delta *out,
     const uint64_t **rep, uint64_t *n_rep, const char *who)
 {
-    ctx->rc_valid = false;
+    ctx->rc.valid = false;
     if (in->flags & REGK_DECODE_LAST)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams", who);
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "%s: batches are still in flight; finish them first", who);
-    if (!ctx->last_path_off || !ctx->last_json_off || ctx->last_n != ctx->last_json_n)
+    if (!ctx->last.path_off || !ctx->last.json_off || ctx->last.n != ctx->last.json_n)
         return fail(ctx, REGK_ERR_STATE, "%s: no finished batch with both a path and a payload stream on this context "
                                          "(an empty batch or a REGK_JOB_STEP result leaves none)", who);
-    const uint64_t n = ctx->last_n, m = in->n;
+    const uint64_t n = ctx->last.n, m = in->n;
     if (n >= 0xFFFFFFFFull || m >= 0xFFFFFFFFull)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: %llu records and %llu nodes: both must be below 2^32 - 1", who,
             (unsigned long long)n, (unsigned long long)m);
@@ -2982,7 +2863,7 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device stats (version needs 4-byte, ephemeral_owner 8-byte alignment)", who);
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
-    DevBuf *rb = ctx->rc;
+    regk_ctx::Reconcile &rb = ctx->rc;
     int rc;
     if (m && !in_dev) {
         path_total = po[m];
@@ -2996,19 +2877,16 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
             return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets without bytes", who);
         const void *src[6] = {pb, po, jb, jo, sver, sown};
         const size_t sz[6] = {(size_t)path_total, (size_t)(m + 1) * 8, (size_t)json_total, (size_t)(m + 1) * 8, (size_t)m * 4, (size_t)m * 8};
-        for (int k = 0; k < (st ? 6 : 4); k++) {
-            if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_IN_PB + k], sz[k] + 16)))
+        for (int k = 0; k < (st ? 6 : 4); k++)
+            if ((rc = stage_in(ctx, rb.in[k], src[k], sz[k], s)))
                 return rc;
-            if (sz[k])
-                CK(cudaMemcpyAsync(rb[regk_ctx::RC_IN_PB + k].p, src[k], sz[k], cudaMemcpyHostToDevice, s));
-        }
-        pb = (const uint8_t *)rb[regk_ctx::RC_IN_PB].p;
-        po = (const uint64_t *)rb[regk_ctx::RC_IN_PO].p;
-        jb = (const uint8_t *)rb[regk_ctx::RC_IN_JB].p;
-        jo = (const uint64_t *)rb[regk_ctx::RC_IN_JO].p;
+        pb = (const uint8_t *)rb.in[0].p;
+        po = (const uint64_t *)rb.in[1].p;
+        jb = (const uint8_t *)rb.in[2].p;
+        jo = (const uint64_t *)rb.in[3].p;
         if (st) {
-            sver = (const int32_t *)rb[regk_ctx::RC_IN_VER].p;
-            sown = (const int64_t *)rb[regk_ctx::RC_IN_OWN].p;
+            sver = (const int32_t *)rb.in[4].p;
+            sown = (const int64_t *)rb.in[5].p;
         }
     } else if (m) {
         if ((path_total && !pb) || (json_total && !jb))
@@ -3017,16 +2895,16 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
             return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device snapshot (bytes need 4-byte, offsets 8-byte alignment)", who);
     }
     /* an empty stream is never read; its kernels still get a valid pointer */
-    if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_IN_PB], 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_IN_JB], 16)))
+    if ((rc = ensure_dev(ctx, rb.in[0], 16)) || (rc = ensure_dev(ctx, rb.in[2], 16)))
         return rc;
     if (!pb)
-        pb = (const uint8_t *)rb[regk_ctx::RC_IN_PB].p;
+        pb = (const uint8_t *)rb.in[0].p;
     if (!jb)
-        jb = (const uint8_t *)rb[regk_ctx::RC_IN_JB].p;
+        jb = (const uint8_t *)rb.in[2].p;
     /* the batch's totals */
     unsigned long long tot[2] = {0, 0};
-    CK(cudaMemcpyAsync(&tot[0], ctx->last_path_off + n, 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(&tot[1], ctx->last_json_off + n, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&tot[0], ctx->last.path_off + n, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&tot[1], ctx->last.json_off + n, 8, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     /* tables: at most half full; "reconcile_tight_table" = 1: the smallest power of two above the entries */
     const bool tight = opt_get(ctx, "reconcile_tight_table", 0) != 0;
@@ -3041,32 +2919,32 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
     const size_t ttr = align16(tiles_r * 4), str = (tiles_r / SUPER + 1) * 8, tto = align16(tiles_o * 4), sto = (tiles_o / SUPER + 1) * 8;
     const size_t totals_bytes = RC_NREC_LISTS * (ttr + str) + tto + sto;
     const size_t counters_bytes = RC_NCOUNTERS * 8;
-    if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_TOBS], so * 4)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_TDES], sd * 4)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RC_SLOTO], m * 4 + 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_HASHO], m * 4 + 16)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RC_SLOTD], n * 4)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_CLS], n + 16)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RC_MATCH], n * 8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_OBSCLS], m + 16)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RC_TOTALS], totals_bytes)) || (rc = ensure_dev(ctx, rb[regk_ctx::RC_COUNT], counters_bytes)) ||
-        (rc = ensure_host(ctx, ctx->h_rc_count, counters_bytes)))
+    if ((rc = ensure_dev(ctx, rb.t_obs, so * 4)) || (rc = ensure_dev(ctx, rb.t_des, sd * 4)) ||
+        (rc = ensure_dev(ctx, rb.slot_obs, m * 4 + 16)) || (rc = ensure_dev(ctx, rb.hash_obs, m * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb.slot_des, n * 4)) || (rc = ensure_dev(ctx, rb.cls, n + 16)) ||
+        (rc = ensure_dev(ctx, rb.match, n * 8)) || (rc = ensure_dev(ctx, rb.obs_cls, m + 16)) ||
+        (rc = ensure_dev(ctx, rb.totals, totals_bytes)) || (rc = ensure_dev(ctx, rb.count, counters_bytes)) ||
+        (rc = ensure_host(ctx, rb.h_count, counters_bytes)))
         return rc;
     for (int l = 0; l < RC_NLISTS; l++)
-        if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_LIST0 + l], (l == RC_LDELETE ? m : n) * 8 + 8)))
+        if ((rc = ensure_dev(ctx, rb.list[l], (l == RC_LDELETE ? m : n) * 8 + 8)))
             return rc;
     for (int k = 0; k < RC_NGATHERS; k++)
-        if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_LEN0 + k], (k == RC_GDELETE ? m : n) * 4 + 8)))
+        if ((rc = ensure_dev(ctx, rb.len[k], (k == RC_GDELETE ? m : n) * 4 + 8)))
             return rc;
     for (int k = 0; st && k < RC_NVER; k++)
-        if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_VER0 + k], (k == RC_VDELETE ? m : n) * 4 + 8)))
+        if ((rc = ensure_dev(ctx, rb.ver[k], (k == RC_VDELETE ? m : n) * 4 + 8)))
             return rc;
-    for (auto &ev : ctx->rc_ev)
-        if (!ev)
-            CK(cudaEventCreate(&ev));
+    for (Event &ev : rb.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
     ReconcileParams p{};
     p.n = n;
     p.m = m;
-    p.d_path = ctx->last_path_bytes;
-    p.d_path_off = ctx->last_path_off;
-    p.d_json = ctx->last_json_bytes;
-    p.d_json_off = ctx->last_json_off;
+    p.d_path = ctx->last.path_bytes;
+    p.d_path_off = ctx->last.path_off;
+    p.d_json = ctx->last.json_bytes;
+    p.d_json_off = ctx->last.json_off;
     p.d_path_limit = tot[0] + 16;                   /* every stream buffer of this library has >= 16 bytes of slack */
     p.d_json_limit = tot[1] + 16;
     p.o_path = pb;
@@ -3081,35 +2959,35 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
         p.o_owner = (const long long *)sown;
         p.want = st->zk_flags == 1u ? (long long)st->session : 0ll;
         for (int k = 0; k < RC_NVER; k++)
-            p.ver[k] = (int32_t *)rb[regk_ctx::RC_VER0 + k].p;
+            p.ver[k] = (int32_t *)rb.ver[k].p;
     }
     p.mask_o = (uint32_t)(so - 1);
     p.mask_d = (uint32_t)(sd - 1);
-    p.t_obs = (uint32_t *)rb[regk_ctx::RC_TOBS].p;
-    p.t_des = (uint32_t *)rb[regk_ctx::RC_TDES].p;
-    p.slot_obs = (uint32_t *)rb[regk_ctx::RC_SLOTO].p;
-    p.hash_obs = (uint32_t *)rb[regk_ctx::RC_HASHO].p;
-    p.slot_des = (uint32_t *)rb[regk_ctx::RC_SLOTD].p;
-    p.cls = (uint8_t *)rb[regk_ctx::RC_CLS].p;
-    p.match = (unsigned long long *)rb[regk_ctx::RC_MATCH].p;
-    p.obs_cls = (uint8_t *)rb[regk_ctx::RC_OBSCLS].p;
-    uint8_t *tb = (uint8_t *)rb[regk_ctx::RC_TOTALS].p;
+    p.t_obs = (uint32_t *)rb.t_obs.p;
+    p.t_des = (uint32_t *)rb.t_des.p;
+    p.slot_obs = (uint32_t *)rb.slot_obs.p;
+    p.hash_obs = (uint32_t *)rb.hash_obs.p;
+    p.slot_des = (uint32_t *)rb.slot_des.p;
+    p.cls = (uint8_t *)rb.cls.p;
+    p.match = (unsigned long long *)rb.match.p;
+    p.obs_cls = (uint8_t *)rb.obs_cls.p;
+    uint8_t *tb = (uint8_t *)rb.totals.p;
     for (int l = 0; l < RC_NLISTS; l++) {
         const bool del = l == RC_LDELETE;
         p.tile_total[l] = (uint32_t *)(tb + (size_t)l * (ttr + str));
         p.super_total[l] = (unsigned long long *)(tb + (size_t)l * (ttr + str) + (del ? tto : ttr));
-        p.list[l] = (unsigned long long *)rb[regk_ctx::RC_LIST0 + l].p;
+        p.list[l] = (unsigned long long *)rb.list[l].p;
     }
     for (int k = 0; k < RC_NGATHERS; k++)
-        p.len[k] = (uint32_t *)rb[regk_ctx::RC_LEN0 + k].p;
-    p.counters = (unsigned long long *)rb[regk_ctx::RC_COUNT].p;
+        p.len[k] = (uint32_t *)rb.len[k].p;
+    p.counters = (unsigned long long *)rb.count.p;
     p.tiles_r = (uint32_t)tiles_r;
     CK(cudaMemsetAsync(p.t_obs, 0, so * 4, s));
     CK(cudaMemsetAsync(p.t_des, 0, sd * 4, s));
     CK(cudaMemsetAsync(tb, 0, totals_bytes, s));
     CK(cudaMemsetAsync(p.counters, 0, counters_bytes, s));
     CK(cudaMemsetAsync(p.counters, 0xFF, 16, s));   /* no bad node, no duplicate node */
-    CK(cudaEventRecord(ctx->rc_ev[0], s));
+    CK(cudaEventRecord(rb.ev[0], s));
     uint32_t launches = 0;
     if (m) {
         regk_reconcile_insert_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(p);
@@ -3120,11 +2998,10 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
     regk_reconcile_compact_kernel<<<(unsigned)(tiles_r + tiles_o), RC_TILE, 0, s>>>(p);
     CK(cudaGetLastError());
     launches += 3;
-    unsigned long long *hc = (unsigned long long *)ctx->h_rc_count.p;
+    unsigned long long *hc = (unsigned long long *)rb.h_count.p;
     CK(cudaMemcpyAsync(hc, p.counters, counters_bytes, cudaMemcpyDeviceToHost, s));
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "%s: kernel execution failed: %s", who, cudaGetErrorString(e));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
     if (hc[RC_C_BAD] != ~0ull)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets are not monotone or reach past the totals at node %llu", who,
             hc[RC_C_BAD]);
@@ -3148,11 +3025,11 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
     for (int g = 0; g < RC_NGATHERS; g++)
         gmax = std::max<uint64_t>(gmax, cnt[g_list[g]]);
     const uint64_t gt = (gmax + MK_TILE - 1) / MK_TILE;
-    if ((rc = ensure_dev(ctx, rb[regk_ctx::RC_GTOTALS], gt * 8 + (gt / SUPER + 1) * 8 + 16)))
+    if ((rc = ensure_dev(ctx, rb.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)))
         return rc;
     for (int g = 0; g < RC_NGATHERS; g++) {
         const uint64_t c = cnt[g_list[g]], bytes = hc[RC_C_BYTES + g];
-        DevBuf &gb = rb[regk_ctx::RC_G0B + 2 * g], &go = rb[regk_ctx::RC_G0B + 2 * g + 1];
+        DevBuf &gb = rb.gather[g].bytes, &go = rb.gather[g].off;
         if ((rc = ensure_dev(ctx, gb, bytes + 16)) || (rc = ensure_dev(ctx, go, (c + 1) * 8)))
             return rc;
         if (!c) {
@@ -3166,7 +3043,7 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
         gp.path_off = g_off[g];
         gp.dir_rec = p.list[g_list[g]];
         gp.dir_len = p.len[g];
-        gp.tile_total = (unsigned long long *)rb[regk_ctx::RC_GTOTALS].p;
+        gp.tile_total = (unsigned long long *)rb.gtotals.p;
         gp.super_total = gp.tile_total + dt;
         gp.dir_bytes = (uint8_t *)gb.p;
         gp.dir_off = (unsigned long long *)go.p;
@@ -3176,37 +3053,34 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
         CK(cudaGetLastError());
         launches += 2;
     }
-    CK(cudaEventRecord(ctx->rc_ev[1], s));
-    e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "%s: kernel execution failed: %s", who, cudaGetErrorString(e));
+    CK(cudaEventRecord(rb.ev[1], s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
     float ms = 0;
-    cudaEventElapsedTime(&ms, ctx->rc_ev[0], ctx->rc_ev[1]);
+    cudaEventElapsedTime(&ms, rb.ev[0], rb.ev[1]);
     const int NOUT = 3 + RC_NLISTS;                 /* cls, match, obs_cls, then the lists */
     const void *dsrc[NOUT] = {p.cls, p.match, p.obs_cls};
     for (int l = 0; l < RC_NLISTS; l++)
         dsrc[3 + l] = p.list[l];
     if (!dev_out) {
-        HostBuf *hb[NOUT] = {&ctx->h_rc_cls, &ctx->h_rc_match, &ctx->h_rc_obscls};
+        HostBuf *hb[NOUT] = {&rb.h_cls, &rb.h_match, &rb.h_obs_cls};
         size_t sz[NOUT] = {n, n * 8, m};
         for (int l = 0; l < RC_NLISTS; l++) {
-            hb[3 + l] = &ctx->h_rc_list[l];
+            hb[3 + l] = &rb.h_list[l];
             sz[3 + l] = cnt[l] * 8;
         }
         for (int k = 0; k < NOUT; k++) {
-            if ((rc = ensure_host(ctx, *hb[k], sz[k] + 16)))
+            if ((rc = to_host(ctx, *hb[k], dsrc[k], sz[k], s)))
                 return rc;
-            if (sz[k])
-                CK(cudaMemcpyAsync(hb[k]->p, dsrc[k], sz[k], cudaMemcpyDeviceToHost, s));
             dsrc[k] = hb[k]->p;
         }
         CK(cudaStreamSynchronize(s));
     }
-    ctx->rc_valid = true;
-    ctx->rc_owned = st != nullptr;
-    ctx->rc_zk_flags = st ? st->zk_flags : 0u;
+    rb.valid = true;
+    rb.owned = st != nullptr;
+    rb.zk_flags = st ? st->zk_flags : 0u;
     for (int l = 0; l < RC_NLISTS; l++)
-        ctx->rc_count[l] = cnt[l];
+        rb.n_list[l] = cnt[l];
     out->n = n;
     out->m = m;
     out->n_create = cnt[RC_LCREATE];
@@ -3244,7 +3118,7 @@ int regk_reconcile_owned(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
     if (!ctx || !in || !out)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_owned: NULL argument");
     memset(out, 0, sizeof *out);
-    ctx->rc_valid = false;
+    ctx->rc.valid = false;
     if (!st)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_owned: NULL stat; regk_reconcile compares bytes alone");
     if (st->zk_flags > 1u)
@@ -3274,32 +3148,31 @@ int regk_reconcile_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames 
                                                "multi transaction");
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "regk_reconcile_requests: batches are still in flight; finish them first");
-    if (!ctx->rc_valid)
+    if (!ctx->rc.valid)
         return fail(ctx, REGK_ERR_STATE, "regk_reconcile_requests: no reconcile result on this context; call regk_reconcile first");
-    if ((replace || observed) && !ctx->rc_owned)
+    if ((replace || observed) && !ctx->rc.owned)
         return fail(ctx, REGK_ERR_STATE, "regk_reconcile_requests: replace frames and observed versions need node stats; the last "
                                          "reconcile was regk_reconcile, call regk_reconcile_owned");
-    if (ctx->rc_owned && (replace || o->op == REGK_ZK_CREATE) && o->zk_flags != ctx->rc_zk_flags)
+    if (ctx->rc.owned && (replace || o->op == REGK_ZK_CREATE) && o->zk_flags != ctx->rc.zk_flags)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: zk_flags %u differs from the CreateMode %u regk_reconcile_owned "
                                                "classified with; nodes created so would be classed REPLACE again", o->zk_flags,
-                    ctx->rc_zk_flags);
+                    ctx->rc.zk_flags);
     CK(cudaSetDevice(ctx->device));
     /* gathered streams: create paths / payloads, update paths / payloads, delete paths, replace paths / payloads */
     const int g = o->op == REGK_ZK_CREATE ? RC_GCREATE : o->op == REGK_ZK_SETDATA ? RC_GUPDATE : replace ? RC_GREPLACE : RC_GDELETE;
     const int l = o->op == REGK_ZK_CREATE ? RC_LCREATE : o->op == REGK_ZK_SETDATA ? RC_LUPDATE : replace ? RC_LREPLACE : RC_LDELETE;
-    const uint64_t c = ctx->rc_count[l];
-    DevBuf *rb = ctx->rc;
+    const uint64_t c = ctx->rc.n_list[l];
+    regk_ctx::Reconcile &rb = ctx->rc;
     const bool data = g != RC_GDELETE;
-    FrameSrc src{c, (const uint8_t *)rb[regk_ctx::RC_G0B + 2 * g].p, (const unsigned long long *)rb[regk_ctx::RC_G0B + 2 * g + 1].p,
-                 data ? (const uint8_t *)rb[regk_ctx::RC_G0B + 2 * g + 2].p : nullptr,
-                 data ? (const unsigned long long *)rb[regk_ctx::RC_G0B + 2 * g + 3].p : nullptr};
+    FrameSrc src{c, (const uint8_t *)rb.gather[g].bytes.p, (const unsigned long long *)rb.gather[g].off.p,
+                 data ? (const uint8_t *)rb.gather[g + 1].bytes.p : nullptr,
+                 data ? (const unsigned long long *)rb.gather[g + 1].off.p : nullptr};
     src.who = "regk_reconcile_requests";
     if (!replace && !observed)
-        return frame_requests(ctx, src, o, rb[regk_ctx::RC_FBYTES], rb[regk_ctx::RC_FOFF], ctx->h_rc_fbytes, ctx->h_rc_foff, out);
+        return frame_requests(ctx, src, o, rb.frames, out);
     const int v = l == RC_LUPDATE ? RC_VUPDATE : l == RC_LREPLACE ? RC_VREPLACE : RC_VDELETE;
-    const int32_t *ver = observed ? (const int32_t *)rb[regk_ctx::RC_VER0 + v].p : nullptr;
-    return frame_entry_requests(ctx, src, o, ver, replace, rb[regk_ctx::RC_FBYTES], rb[regk_ctx::RC_FOFF], ctx->h_rc_fbytes,
-                                ctx->h_rc_foff, out);
+    const int32_t *ver = observed ? (const int32_t *)rb.ver[v].p : nullptr;
+    return frame_entry_requests(ctx, src, o, ver, replace, rb.frames, out);
 }
 
 static const char *reply_reason(uint32_t code)
@@ -3328,7 +3201,7 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
     if (!ctx->gd_valid)
         return fail(ctx, REGK_ERR_STATE, "regk_read_replies: no getData framing (regk_jute_requests with REGK_ZK_GETDATA) of the "
                                          "batch finished last");
-    if (ctx->gd_gen != ctx->last_gen || !ctx->last_path_off)
+    if (ctx->gd_gen != ctx->last.gen || !ctx->last.path_off)
         return fail(ctx, REGK_ERR_STATE, "regk_read_replies: a batch finished after the getData framing; frame its getData "
                                          "requests first");
     if (!bytes && len)
@@ -3347,18 +3220,16 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_replies: %llu records: must be below 2^32 - 1", (unsigned long long)n);
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
-    DevBuf *rb = ctx->rq;
+    regk_ctx::Replies &rb = ctx->rq;
     int rc;
-    for (auto &ev : ctx->rq_ev)
-        if (!ev)
-            CK(cudaEventCreate(&ev));
+    for (Event &ev : rb.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
     const uint8_t *ds = bytes;
     if (!in_dev) {
-        if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_STREAM], len + 16)))
+        if ((rc = stage_in(ctx, rb.stream, bytes, len, s)))
             return rc;
-        if (len)
-            CK(cudaMemcpyAsync(rb[regk_ctx::RQ_STREAM].p, bytes, len, cudaMemcpyHostToDevice, s));
-        ds = (const uint8_t *)rb[regk_ctx::RQ_STREAM].p;
+        ds = (const uint8_t *)rb.stream.p;
     }
     const uint64_t nblk = (len + 15) / 16, tiles_s = (nblk + RP_TILE - 1) / RP_TILE, tiles_r = (n + RP_TILE - 1) / RP_TILE;
     uint64_t slots = 1024;
@@ -3367,38 +3238,38 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
     /* two-level totals of the candidate pass (the chain and node passes get theirs once the candidates are counted) */
     const size_t totals_bytes = align16(tiles_s * 4) + (tiles_s / SUPER + 1) * 8;
     const size_t n8 = n * 8 + 16, n4 = n * 4 + 16;
-    if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_WORD], nblk * 4 + 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_TOTALS], totals_bytes)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_TBASE], tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_ERRA], n4)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_DPOS], n8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_DLEN], n4)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_VER], n4)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_OWN], n8)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_SLOT], n4)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_TABLE], slots * 4)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_COUNT], RQ_NCOUNTERS * 8)) || (rc = ensure_host(ctx, ctx->h_rq_count, RQ_NCOUNTERS * 8)))
+    if ((rc = ensure_dev(ctx, rb.word, nblk * 4 + 16)) || (rc = ensure_dev(ctx, rb.totals, totals_bytes)) ||
+        (rc = ensure_dev(ctx, rb.tile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, rb.err, n4)) ||
+        (rc = ensure_dev(ctx, rb.data_pos, n8)) || (rc = ensure_dev(ctx, rb.dlen, n4)) ||
+        (rc = ensure_dev(ctx, rb.ver, n4)) || (rc = ensure_dev(ctx, rb.own, n8)) ||
+        (rc = ensure_dev(ctx, rb.slot, n4)) || (rc = ensure_dev(ctx, rb.table, slots * 4)) ||
+        (rc = ensure_dev(ctx, rb.count, RQ_NCOUNTERS * 8)) || (rc = ensure_host(ctx, rb.h_count, RQ_NCOUNTERS * 8)))
         return rc;
     RepParams p{};
     p.s = ds;
     p.len = len;
     p.xid_base = xb;
     p.n = n;
-    p.word = (uint32_t *)rb[regk_ctx::RQ_WORD].p;
-    p.tile_total = (uint32_t *)rb[regk_ctx::RQ_TOTALS].p;
-    p.super_total = (unsigned long long *)((uint8_t *)rb[regk_ctx::RQ_TOTALS].p + align16(tiles_s * 4));
-    p.tile_base = (unsigned long long *)rb[regk_ctx::RQ_TBASE].p;
-    p.err = (int32_t *)rb[regk_ctx::RQ_ERRA].p;
-    p.data_pos = (unsigned long long *)rb[regk_ctx::RQ_DPOS].p;
-    p.dlen = (uint32_t *)rb[regk_ctx::RQ_DLEN].p;
-    p.ver = (int32_t *)rb[regk_ctx::RQ_VER].p;
-    p.own = (long long *)rb[regk_ctx::RQ_OWN].p;
-    p.slot = (uint32_t *)rb[regk_ctx::RQ_SLOT].p;
-    p.d_path = ctx->last_path_bytes;
-    p.d_path_off = ctx->last_path_off;
-    p.table = (uint32_t *)rb[regk_ctx::RQ_TABLE].p;
+    p.word = (uint32_t *)rb.word.p;
+    p.tile_total = (uint32_t *)rb.totals.p;
+    p.super_total = (unsigned long long *)((uint8_t *)rb.totals.p + align16(tiles_s * 4));
+    p.tile_base = (unsigned long long *)rb.tile_base.p;
+    p.err = (int32_t *)rb.err.p;
+    p.data_pos = (unsigned long long *)rb.data_pos.p;
+    p.dlen = (uint32_t *)rb.dlen.p;
+    p.ver = (int32_t *)rb.ver.p;
+    p.own = (long long *)rb.own.p;
+    p.slot = (uint32_t *)rb.slot.p;
+    p.d_path = ctx->last.path_bytes;
+    p.d_path_off = ctx->last.path_off;
+    p.table = (uint32_t *)rb.table.p;
     p.mask_t = (uint32_t)(slots - 1);
-    p.counters = (unsigned long long *)rb[regk_ctx::RQ_COUNT].p;
-    unsigned long long *hc = (unsigned long long *)ctx->h_rq_count.p;
+    p.counters = (unsigned long long *)rb.count.p;
+    unsigned long long *hc = (unsigned long long *)rb.h_count.p;
     CK(cudaMemsetAsync(p.counters, 0, RQ_NCOUNTERS * 8, s));
     CK(cudaMemsetAsync(p.counters + RQ_ERR, 0xFF, 8, s));
     CK(cudaMemsetAsync(p.tile_total, 0, totals_bytes, s));
-    CK(cudaEventRecord(ctx->rq_ev[0], s));
+    CK(cudaEventRecord(rb.ev[0], s));
     uint32_t launches = 0;
     /* 1. candidates: the plausible positions; their count from the CTA totals' upper level */
     const uint64_t nsup = tiles_s / SUPER + 1;
@@ -3409,9 +3280,8 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
         launches++;
         CK(cudaMemcpyAsync(sup.data(), p.super_total, nsup * 8, cudaMemcpyDeviceToHost, s));
     }
-    cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_read_replies: kernel execution failed: %s", cudaGetErrorString(e));
+    if ((rc = sync_or_fail(ctx, s, "regk_read_replies")))
+        return rc;
     uint64_t C = 0;
     for (unsigned long long v : sup)
         C += v;
@@ -3424,17 +3294,17 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
         K++;
     const size_t tiles_c = (C + RP_TILE - 1) / RP_TILE, tiles2 = std::max<uint64_t>(tiles_c, tiles_r);
     const size_t totals2_bytes = align16(tiles2 * 4) + (tiles2 / SUPER + 1) * 8;
-    if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_CAND], C * 8 + 16)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_MARK], C + 16)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_JUMP], (size_t)(K + 1) * C * 4 + 16)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_TOTALS2], totals2_bytes)))
+    if ((rc = ensure_dev(ctx, rb.cand, C * 8 + 16)) || (rc = ensure_dev(ctx, rb.mark, C + 16)) ||
+        (rc = ensure_dev(ctx, rb.jump, (size_t)(K + 1) * C * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb.totals2, totals2_bytes)))
         return rc;
-    p.cand = (unsigned long long *)rb[regk_ctx::RQ_CAND].p;
-    p.marked = (uint8_t *)rb[regk_ctx::RQ_MARK].p;
+    p.cand = (unsigned long long *)rb.cand.p;
+    p.marked = (uint8_t *)rb.mark.p;
     p.C = C;
-    uint32_t *J = (uint32_t *)rb[regk_ctx::RQ_JUMP].p;
+    uint32_t *J = (uint32_t *)rb.jump.p;
     RepParams p2 = p;                                   /* the chain and node passes' totals */
-    p2.tile_total = (uint32_t *)rb[regk_ctx::RQ_TOTALS2].p;
-    p2.super_total = (unsigned long long *)((uint8_t *)rb[regk_ctx::RQ_TOTALS2].p + align16(tiles2 * 4));
+    p2.tile_total = (uint32_t *)rb.totals2.p;
+    p2.super_total = (unsigned long long *)((uint8_t *)rb.totals2.p + align16(tiles2 * 4));
     const unsigned g256 = (unsigned)((C + 255) / 256);
     if (C) {
         regk_replies_compact_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(p);
@@ -3452,9 +3322,8 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
         launches += 2 * K + 6;
     }
     CK(cudaMemcpyAsync(hc, p.counters, RQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
-    e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_read_replies: kernel execution failed: %s", cudaGetErrorString(e));
+    if ((rc = sync_or_fail(ctx, s, "regk_read_replies")))
+        return rc;
     if (hc[RQ_ERR] != ~0ull) {
         /* the smallest record whose frame fails the full check; the frame starts 24 bytes before its data */
         const uint64_t k = hc[RQ_ERR] >> 8;
@@ -3495,15 +3364,15 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
                     h.len, h.xid, (unsigned long long)done, want);
     }
     /* 4. the nodes: found records, one per distinct path, in record order */
-    if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_NREC], n8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_NVER], n4)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_NOWN], n8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_NPLEN], n4)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_NDLEN], n4)))
+    if ((rc = ensure_dev(ctx, rb.node_rec, n8)) || (rc = ensure_dev(ctx, rb.node_ver, n4)) ||
+        (rc = ensure_dev(ctx, rb.node_own, n8)) || (rc = ensure_dev(ctx, rb.node_plen, n4)) ||
+        (rc = ensure_dev(ctx, rb.node_dlen, n4)))
         return rc;
-    p.node_rec = (unsigned long long *)rb[regk_ctx::RQ_NREC].p;
-    p.node_ver = (int32_t *)rb[regk_ctx::RQ_NVER].p;
-    p.node_own = (long long *)rb[regk_ctx::RQ_NOWN].p;
-    p.node_plen = (uint32_t *)rb[regk_ctx::RQ_NPLEN].p;
-    p.node_dlen = (uint32_t *)rb[regk_ctx::RQ_NDLEN].p;
+    p.node_rec = (unsigned long long *)rb.node_rec.p;
+    p.node_ver = (int32_t *)rb.node_ver.p;
+    p.node_own = (long long *)rb.node_own.p;
+    p.node_plen = (uint32_t *)rb.node_plen.p;
+    p.node_dlen = (uint32_t *)rb.node_dlen.p;
     p.tile_total = p2.tile_total;
     p.super_total = p2.super_total;
     CK(cudaMemsetAsync(p.table, 0, slots * 4, s));
@@ -3514,25 +3383,24 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
     CK(cudaGetLastError());
     launches += 3;
     CK(cudaMemcpyAsync(hc, p.counters, RQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
-    e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_read_replies: kernel execution failed: %s", cudaGetErrorString(e));
+    if ((rc = sync_or_fail(ctx, s, "regk_read_replies")))
+        return rc;
     const uint64_t m = hc[RQ_M];
     /* 5. the snapshot's streams: node paths from the batch, node data from the reply stream */
     const uint64_t gt = (m + MK_TILE - 1) / MK_TILE;
-    if ((rc = ensure_dev(ctx, rb[regk_ctx::RQ_GTOT], gt * 8 + (gt / SUPER + 1) * 8 + 16)) ||
-        (rc = ensure_dev(ctx, rb[regk_ctx::RQ_PO], (m + 1) * 8)) || (rc = ensure_dev(ctx, rb[regk_ctx::RQ_JO], (m + 1) * 8)))
+    if ((rc = ensure_dev(ctx, rb.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)) ||
+        (rc = ensure_dev(ctx, rb.snap_off[0], (m + 1) * 8)) || (rc = ensure_dev(ctx, rb.snap_off[1], (m + 1) * 8)))
         return rc;
     uint64_t totals[2] = {0, 0};
     for (int g = 0; g < 2; g++) {
-        DevBuf &gb = rb[g ? regk_ctx::RQ_JB : regk_ctx::RQ_PB], &go = rb[g ? regk_ctx::RQ_JO : regk_ctx::RQ_PO];
+        DevBuf &gb = rb.snap_bytes[g], &go = rb.snap_off[g];
         MkGatherParams gp{};
         gp.n_dirs = m;
-        gp.path_bytes = g ? ds : ctx->last_path_bytes;
-        gp.path_off = g ? p.data_pos : ctx->last_path_off;
+        gp.path_bytes = g ? ds : ctx->last.path_bytes;
+        gp.path_off = g ? p.data_pos : ctx->last.path_off;
         gp.dir_rec = p.node_rec;
         gp.dir_len = g ? p.node_dlen : p.node_plen;
-        gp.tile_total = (unsigned long long *)rb[regk_ctx::RQ_GTOT].p;
+        gp.tile_total = (unsigned long long *)rb.gtotals.p;
         gp.super_total = gp.tile_total + gt;
         gp.dir_off = (unsigned long long *)go.p;
         if (!m) {
@@ -3556,24 +3424,19 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
         CK(cudaGetLastError());
         launches += 2;
     }
-    CK(cudaEventRecord(ctx->rq_ev[1], s));
-    e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess)
-        return fail(ctx, REGK_ERR_CUDA, "regk_read_replies: kernel execution failed: %s", cudaGetErrorString(e));
+    CK(cudaEventRecord(rb.ev[1], s));
+    if ((rc = sync_or_fail(ctx, s, "regk_read_replies")))
+        return rc;
     float ms = 0;
-    cudaEventElapsedTime(&ms, ctx->rq_ev[0], ctx->rq_ev[1]);
+    cudaEventElapsedTime(&ms, rb.ev[0], rb.ev[1]);
     const int32_t *err_out = p.err;
     const uint64_t *rec_out = (const uint64_t *)p.node_rec;
     if (!dev_out) {
-        if ((rc = ensure_host(ctx, ctx->h_rq_err, n * 4 + 16)) || (rc = ensure_host(ctx, ctx->h_rq_node, m * 8 + 16)))
+        if ((rc = to_host(ctx, rb.h_err, p.err, n * 4, s)) || (rc = to_host(ctx, rb.h_node, p.node_rec, m * 8, s)))
             return rc;
-        if (n)
-            CK(cudaMemcpyAsync(ctx->h_rq_err.p, p.err, n * 4, cudaMemcpyDeviceToHost, s));
-        if (m)
-            CK(cudaMemcpyAsync(ctx->h_rq_node.p, p.node_rec, m * 8, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
-        err_out = (const int32_t *)ctx->h_rq_err.p;
-        rec_out = (const uint64_t *)ctx->h_rq_node.p;
+        err_out = (const int32_t *)rb.h_err.p;
+        rec_out = (const uint64_t *)rb.h_node.p;
     }
     out->n = n;
     out->m = m;
@@ -3590,10 +3453,10 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
     out->snapshot.flags = REGK_IN_DEVICE;
     out->snapshot.path_total = totals[0];
     out->snapshot.json_total = totals[1];
-    out->snapshot.path_bytes = (const uint8_t *)rb[regk_ctx::RQ_PB].p;
-    out->snapshot.path_off = (const uint64_t *)rb[regk_ctx::RQ_PO].p;
-    out->snapshot.json_bytes = (const uint8_t *)rb[regk_ctx::RQ_JB].p;
-    out->snapshot.json_off = (const uint64_t *)rb[regk_ctx::RQ_JO].p;
+    out->snapshot.path_bytes = (const uint8_t *)rb.snap_bytes[0].p;
+    out->snapshot.path_off = (const uint64_t *)rb.snap_off[0].p;
+    out->snapshot.json_bytes = (const uint8_t *)rb.snap_bytes[1].p;
+    out->snapshot.json_off = (const uint64_t *)rb.snap_off[1].p;
     out->version = p.node_ver;
     out->ephemeral_owner = (const int64_t *)p.node_own;
     out->kernel_ms = ms;
