@@ -675,6 +675,91 @@ typedef struct regk_replies {
 
 int         regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t flags, regk_replies *out);
 
+/*
+ * ---- list the batch's service directories and find the instances it no longer produces (the reference removes a node
+ * only through its own unregister, lib/register.js:254-295, or through session expiry, which keeps a dead instance in
+ * DNS for minutes, README.md:70-76, :764-779) ------------------------------------------------------------------------
+ * regk_children_requests, opts->op:
+ *   REGK_ZK_GETCHILDREN  one GetChildrenRequest{dir, watch = false} per directory of the batch finished last: frame k =
+ *                        len | xid_base + k (wrapping) | 8 | P | dir | 0, 17 + P bytes (the getData layout).  The
+ *                        directories are the distinct parent directories of its paths, in order of first record (the
+ *                        unique_first order of regk_parent_dirs); directory k = path_{dir_rec[k]}[0, dir_len[k]).  "/"
+ *                        is not listed (its children are /zookeeper and every other tree), nor is a directory
+ *                        ZooKeeper rejects (regk_mkdirp_dirs' INVALID rule): their first records come back in
+ *                        regk_read_children's unlisted[].  A skip-mode batch contributes its kept records.  group != 0
+ *                        is REGK_ERR_INVALID_ARG.  REGK_ERR_STATE: a batch of alias nodes (REGK_NODE_ALIAS: an alias
+ *                        node's parent is a domain's parent directory, which holds other services - only a host-node
+ *                        batch's directories are service directories whose children are that service's instances), no
+ *                        finished batch with a path stream (a REGK_NO_PATH batch, an empty batch, a REGK_JOB_STEP
+ *                        result), a pending batch.  A successful call records the batch, xid_base, the number of
+ *                        directories d and the directory set for regk_read_children; it leaves the REGK_ZK_GETDATA
+ *                        record of regk_jute_requests and the results of regk_parent_dirs / regk_mkdirp_dirs as they are.
+ *   REGK_ZK_DELETE       DeleteRequest{path, version} for every stale child of the last regk_read_children call
+ *                        (REGK_ERR_STATE without one), in stale order; version and group mean what they mean for
+ *                        regk_reconcile_requests.  A getChildren reply carries no Stat of a child, so version is
+ *                        opts->version (-1 = any).  Built from the library's own copy of the stale paths: neither the
+ *                        reply stream nor the batch is needed.
+ * Any other op is REGK_ERR_INVALID_ARG.  flags: REGK_OUT_DEVICE returns device pointers, else pinned host arrays; each
+ * op's frames are valid until the next call with that op.
+ *
+ * regk_read_children: bytes[start, len) = what the caller read off the session after sending the getChildren frames,
+ * from the first reply's length word on; host memory, or device memory with REGK_IN_DEVICE (bytes 16-byte aligned;
+ * start need not be, so the getData replies and these can be one stream: start = regk_replies.consumed).  Every
+ * position reported, consumed included, counts from bytes.  Frame = int len | ReplyHeader{int xid; long zxid; int err}
+ * | body; body = GetChildrenResponse{int count | count x (int L | L bytes)} iff err == 0 (len == 20 + sum(4 + L_i));
+ * count == -1 (a null vector) reads as no children.  Replies come in order: the k-th frame that is not a watch
+ * notification (xid -1) or a ping (xid -2) carries xid_base + k and answers directory k; notifications and pings met
+ * before the d-th reply are skipped and counted, and the stream may go on past it.
+ * Child q of directory k is listing entry child_off[k] + q, in the reply's order.  Listing path e = directory + '/' +
+ * name (listing: ALWAYS device, REGK_IN_DEVICE, host_nodes = 1, every entry with empty data - regk_decode reads the
+ * instance names back out of it).  cls[e] = REGK_DELTA_KEEP when path e is a path of the batch or a proper ancestor
+ * directory of one (a prefix of a listed directory that ends at a component boundary), else REGK_CHILD_STALE; stale[]
+ * lists the stale entries ascending.  Names are compared byte for byte (a hash only picks a table slot).  Two equal
+ * names in one reply are not looked for, since a server cannot hold them: both get the same class.
+ * OWNERSHIP: every child of a listed directory that the batch does not produce is stale, so list only directories
+ * whose instances the batch is authoritative for.  A directory whose reply carries an error contributes no children:
+ * NONODE (-101) only means it does not exist yet, and the deletes for the other directories stay correct.  Listing is
+ * not recursive: a stale child that has children of its own fails its delete with NOTEMPTY.
+ * n_found + n_missing + n_error == n_dirs.  dir_rec, dir_len, err, child_off, cls, stale and unlisted are pinned host
+ * arrays, or device arrays with REGK_OUT_DEVICE; all results stay valid until the next regk_read_children call (a later
+ * batch or framing does not touch them).
+ * REGK_ERR_STATE: no REGK_ZK_GETCHILDREN framing, a batch finished since it, a pending batch.  REGK_ERR_INVALID_ARG (the
+ * message names the byte position - the frame's, and the entry's for an entry fault - and the expected xid; it is the
+ * first fault a front-to-back reader meets): the stream ends before the d-th reply is complete, len < 16, a negative
+ * xid other than -1 / -2, an xid outside the framed range, a reply out of order, an error reply with a body, a count
+ * below -1, a success frame too short for its count, an entry that runs past its frame, L < 1, a name holding '/' or
+ * NUL or equal to "." or "..", entries that end before their frame does; an xid range that covers -1 or -2; d or the
+ * number of children not below 2^32 - 1; start > len; NULL pointers; a misaligned device stream.
+ * PARITY UNPINNED: the layouts are restated from zookeeper.jute and tested against an independent restatement.
+ */
+#define REGK_ZK_GETCHILDREN 8u
+#define REGK_CHILD_STALE    1u      /* regk_children.cls[]; REGK_DELTA_KEEP (0) otherwise */
+
+int         regk_children_requests(regk_ctx *ctx, const regk_jute_opts *opts, regk_frames *out);
+
+typedef struct regk_children {
+    uint64_t n_dirs;                /* d: directories listed */
+    uint64_t n_children;            /* listing entries */
+    uint64_t n_stale;
+    uint64_t n_found, n_missing, n_error;   /* replies with err 0 / NONODE (-101) / any other err */
+    uint64_t n_skipped;             /* watch notifications and pings met before the d-th reply */
+    uint64_t consumed;              /* stream position of the end of the d-th reply (start when d == 0) */
+    uint64_t n_unlisted;
+    uint32_t flags, launches;       /* REGK_OUT_DEVICE */
+    const uint64_t *dir_rec;        /* [n_dirs] first record of directory k */
+    const uint32_t *dir_len;        /* [n_dirs] */
+    const int32_t  *err;            /* [n_dirs] ReplyHeader.err of directory k's reply */
+    const uint64_t *child_off;      /* [n_dirs + 1] */
+    const uint8_t  *cls;            /* [n_children] REGK_DELTA_KEEP / REGK_CHILD_STALE */
+    const uint64_t *stale;          /* [n_stale] listing indices, ascending */
+    const uint64_t *unlisted;       /* [n_unlisted] first records of "/" and of directories ZooKeeper rejects */
+    regk_decode_in  listing;        /* ALWAYS device: path e = directory + '/' + name, empty data */
+    float kernel_ms;
+} regk_children;
+
+int         regk_read_children(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, uint32_t flags,
+                               regk_children *out);
+
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);
 int64_t     regk_get_option(const regk_ctx *ctx, const char *name);

@@ -96,6 +96,7 @@ class CJuteOpts(C.Structure):        # regk_jute_opts
 
 ZK_CREATE, ZK_DELETE, ZK_SETDATA = 1, 2, 5
 ZK_GETDATA = 4                      # jute_requests: GetDataRequest{path, watch = false}; its replies go to read_replies()
+ZK_GETCHILDREN = 8                  # children_requests: GetChildrenRequest{dir, watch = false}; replies go to read_children()
 ZK_REPLACE = 256                    # reconcile_requests after reconcile_owned: delete + create in one multi transaction
 FLAG_ZK_VERSION_OBSERVED = 1 << 9   # regk_jute_opts.flags: each frame carries its node's Stat.version
 
@@ -257,6 +258,59 @@ class Replies:
                         d2h(self._out.version, m, np.int32), d2h(self._out.ephemeral_owner, m, np.int64))
 
 
+class CChildren(C.Structure):       # regk_children
+    _fields_ = [("n_dirs", C.c_uint64), ("n_children", C.c_uint64), ("n_stale", C.c_uint64), ("n_found", C.c_uint64),
+                ("n_missing", C.c_uint64), ("n_error", C.c_uint64), ("n_skipped", C.c_uint64), ("consumed", C.c_uint64),
+                ("n_unlisted", C.c_uint64), ("flags", C.c_uint32), ("launches", C.c_uint32),
+                ("dir_rec", C.c_void_p), ("dir_len", C.c_void_p), ("err", C.c_void_p), ("child_off", C.c_void_p),
+                ("cls", C.c_void_p), ("stale", C.c_void_p), ("unlisted", C.c_void_p), ("listing", CDecodeIn),
+                ("kernel_ms", C.c_float)]
+
+
+CHILD_KEEP, CHILD_STALE = 0, 1      # Children.cls
+
+
+class Children:
+    """What read_children() made of the replies to the last getChildren framing: directory k is
+    path(dir_rec[k])[:dir_len[k]] and err[k] its reply's ReplyHeader.err; its children are listing entries
+    child_off[k]:child_off[k+1] in the reply's order, cls[e] is CHILD_KEEP (a path of the batch, or a directory on the way
+    to one) or CHILD_STALE, stale lists the stale entries ascending and unlisted the first records of the directories not
+    listed ("/" and directories ZooKeeper rejects).  Counts: n_dirs, n_children, n_stale, n_found / n_missing / n_error,
+    n_skipped, n_unlisted, and `consumed` (stream position of the end of the last reply).  The listing paths stay on the
+    device: listing() and stale_paths() copy them out.  Valid until the next read_children() call on the context."""
+
+    def __init__(self, ctx, out):
+        self._ctx, self._out = ctx, out
+        d, m = int(out.n_dirs), int(out.n_children)
+        self.n_dirs, self.n_children, self.n_stale = d, m, int(out.n_stale)
+        self.n_found, self.n_missing, self.n_error = int(out.n_found), int(out.n_missing), int(out.n_error)
+        self.n_skipped, self.consumed, self.n_unlisted = int(out.n_skipped), int(out.consumed), int(out.n_unlisted)
+        self.launches, self.kernel_ms = int(out.launches), float(out.kernel_ms)
+        self.dir_rec = _as_np(out.dir_rec, d, np.uint64).copy()
+        self.dir_len = _as_np(out.dir_len, d, np.uint32).copy()
+        self.err = _as_np(out.err, d, np.int32).copy()
+        self.child_off = _as_np(out.child_off, d + 1, np.uint64).copy()
+        self.cls = _as_np(out.cls, m, np.uint8).copy()
+        self.stale = _as_np(out.stale, self.n_stale, np.uint64).copy()
+        self.unlisted = _as_np(out.unlisted, self.n_unlisted, np.uint64).copy()
+
+    def cdecode_in(self):
+        """the device regk_decode_in of the listing.  Returns (struct, keepalive)."""
+        return self._out.listing, None
+
+    def listing(self):
+        """host copy of the listing paths, as a list of bytes"""
+        s, m = self._out.listing, self.n_children
+        b = self._ctx._d2h(s.path_bytes, int(s.path_total), np.uint8).tobytes()
+        off = self._ctx._d2h(s.path_off, m + 1, np.uint64)
+        return [b[int(off[e]):int(off[e + 1])] for e in range(m)]
+
+    def stale_paths(self):
+        """host copy of the stale paths, in stale order"""
+        lst = self.listing()
+        return [lst[int(e)] for e in self.stale]
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -269,7 +323,7 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_gather_push", "regk_parent_dirs", "regk_job_bind", "regk_service_records",
            "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records", "regk_mkdirp_dirs",
            "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned",
-           "regk_read_replies"]
+           "regk_read_replies", "regk_children_requests", "regk_read_children"]
 
 _lib = None
 
@@ -327,6 +381,8 @@ def load_library():
     lib.regk_reconcile_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     lib.regk_reconcile_owned.argtypes = [vp, C.POINTER(CDecodeIn), C.POINTER(CNodeStat), u32, C.POINTER(CDeltaOwned)]
     lib.regk_read_replies.argtypes = [vp, vp, u64, u32, C.POINTER(CReplies)]
+    lib.regk_children_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
+    lib.regk_read_children.argtypes = [vp, vp, u64, u64, u32, C.POINTER(CChildren)]
     _lib = lib
     return lib
 
@@ -725,6 +781,48 @@ class Context:
         del keep
         self._check(rc)
         return out if device else Replies(self, out)
+
+    # -- the batch's service directories listed, and the children it does not produce --
+    def children_requests(self, op: int = ZK_GETCHILDREN, xid_base: int = 1, version: int = -1, group: int = 0,
+                          device: bool = False):
+        """regk_children_requests: ZK_GETCHILDREN frames one GetChildrenRequest per service directory of the batch
+        finished last (its distinct parent directories but "/" and rejected ones, in order of first record); ZK_DELETE
+        frames a DeleteRequest at `version` for every stale child of the last read_children(), singly or as multi
+        transactions of `group`.  Returns (frame_bytes, frame_off uint64[frames+1], kernel_ms), or the raw CFrames with
+        device=True."""
+        xid = (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31
+        o = CJuteOpts(int(op), FLAG_OUT_DEVICE if device else 0, xid, 0, int(version), int(group))
+        out = CFrames()
+        self._check(self._lib.regk_children_requests(self._h, C.byref(o), C.byref(out)))
+        if device:
+            return out
+        n = int(out.n)
+        return (_as_np(out.frame_bytes, int(out.total), np.uint8).copy(), _as_np(out.frame_off, n + 1, np.uint64).copy(),
+                float(out.kernel_ms))
+
+    def read_children(self, stream, start: int = 0, device: bool = False):
+        """regk_read_children: `stream` (a NumPy uint8 array, or a contiguous CUDA uint8 tensor) holds, from byte `start`
+        on, the bytes read off the session after sending the frames of the last children_requests(ZK_GETCHILDREN) call
+        (start = the getData replies' `consumed` when both come in one stream).  Returns a Children, or the raw CChildren
+        (its small arrays on the device) with device=True.  Every child of a listed directory that the batch does not
+        produce is stale: list only directories whose instances the batch is authoritative for."""
+        flags = FLAG_OUT_DEVICE if device else 0
+        if hasattr(stream, "data_ptr"):
+            import torch
+            if not stream.is_cuda or stream.dtype != torch.uint8 or not stream.is_contiguous():
+                raise ValueError("a device stream is a contiguous CUDA uint8 tensor")
+            keep, ptr, n = stream, stream.data_ptr() or None, stream.numel()
+            flags |= FLAG_IN_DEVICE
+        else:
+            keep = np.ascontiguousarray(stream)
+            if keep.dtype != np.uint8 or keep.ndim != 1:
+                raise ValueError("a host stream is a one-dimensional uint8 array")
+            ptr, n = _np_ptr(keep), keep.size
+        out = CChildren()
+        rc = self._lib.regk_read_children(self._h, ptr, n, int(start), flags, C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else Children(self, out)
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

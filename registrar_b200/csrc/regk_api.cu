@@ -33,6 +33,7 @@
 #include "regk_mkdirp.cuh"
 #include "regk_reconcile.cuh"
 #include "regk_replies.cuh"
+#include "regk_children.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -218,6 +219,28 @@ struct regk_ctx {
         HostBuf h_count, h_err, h_node;
         Event ev[2];
     } rq;
+    /* regk_children_requests / regk_read_children (regk_children.cuh).  The last REGK_ZK_GETCHILDREN framing: its own
+       parent pass, the directory set (listed and unlisted) and its packed bytes, the batch it framed, xid_base, d.
+       The last read: frame and entry chains, per-directory arrays, the listing, the keep table, the stale list and
+       its packed paths (the REGK_ZK_DELETE framing reads those), and copies of the set it read against. */
+    struct Children {
+        ParentPass pass;
+        DevBuf totals, count, unlisted, drec, dlen, dbytes, doff;
+        HostBuf h_count;
+        FrameBufs frames[2];                    /* getChildren, delete */
+        bool framed = false;
+        uint64_t gen = 0, n = 0, d = 0, n_unlisted = 0, prefixes = 0;
+        int32_t xid = 0;
+        DevBuf stream, word, ftotals, tile_base, cand, mark, jump, totals2, fpos, fend, err, cnt, seed_g, last_g1, name_bad,
+            end_pos, fault_pos, child_off;
+        DevBuf eword, etotals, etile_base, ecand, emark, ejump, etotals2, ent_pos, ent_nlen, ent_k, ent_plen;
+        DevBuf gtotals, lst_bytes, lst_off, lst_zero, table, cls, stotals, stale, stale_len, sbytes, soff;
+        DevBuf r_drec, r_dlen, r_unlisted;
+        HostBuf h_drec, h_dlen, h_err, h_child_off, h_cls, h_stale, h_unlisted;
+        Event ev[2];
+        bool read = false;                      /* the stale list of the last regk_read_children is in stale .. soff */
+        uint64_t n_stale = 0;
+    } ch;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     struct Skip {
@@ -889,7 +912,7 @@ static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_op
     p.multi = multi ? 1u : 0u;
     /* what follows the data: create - acl vector [OPEN_ACL_UNSAFE] + flags; delete / setData - the expected version */
     uint8_t tail[48] = {0};
-    if (o->op == REGK_ZK_GETDATA) {
+    if (o->op == REGK_ZK_GETDATA || o->op == REGK_ZK_GETCHILDREN) {
         p.tail_len = 1;                                 /* watch = false */
     } else if (o->op == REGK_ZK_CREATE) {
         static const uint8_t acl[27] = {0, 0, 0, 1, 0, 0, 0, 31, 0, 0, 0, 5, 'w', 'o', 'r', 'l', 'd', 0, 0, 0, 6, 'a', 'n', 'y', 'o', 'n', 'e'};
@@ -3459,6 +3482,608 @@ int regk_read_replies(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_
     out->snapshot.json_off = (const uint64_t *)rb.snap_off[1].p;
     out->version = p.node_ver;
     out->ephemeral_owner = (const int64_t *)p.node_own;
+    out->kernel_ms = ms;
+    return REGK_OK;
+}
+
+/* The strings (path_bytes at path_off[rec[k]], len[k] bytes), k < m, packed into `bytes` / `off` by the mkdirp gather pair
+   (regk_mkdirp.cuh); *total = their byte count.  Synchronises once to size `bytes`. */
+static int pack_strings(regk_ctx *ctx, uint64_t m, const uint8_t *path_bytes, const unsigned long long *path_off,
+    const unsigned long long *rec, const uint32_t *len, DevBuf &totals, DevBuf &bytes, DevBuf &off, uint64_t *total,
+    uint32_t *launches)
+{
+    cudaStream_t s = ctx->stream;
+    const uint64_t gt = (m + MK_TILE - 1) / MK_TILE;
+    int rc;
+    *total = 0;
+    if ((rc = ensure_dev(ctx, totals, gt * 8 + (gt / SUPER + 1) * 8 + 16)) || (rc = ensure_dev(ctx, off, (m + 1) * 8)))
+        return rc;
+    if (!m) {
+        if ((rc = ensure_dev(ctx, bytes, 16)))
+            return rc;
+        CK(cudaMemsetAsync(off.p, 0, 8, s));
+        return REGK_OK;
+    }
+    MkGatherParams gp{};
+    gp.n_dirs = m;
+    gp.path_bytes = path_bytes;
+    gp.path_off = path_off;
+    gp.dir_rec = rec;
+    gp.dir_len = len;
+    gp.tile_total = (unsigned long long *)totals.p;
+    gp.super_total = gp.tile_total + gt;
+    gp.dir_off = (unsigned long long *)off.p;
+    CK(cudaMemsetAsync(gp.super_total, 0, (gt / SUPER + 1) * 8, s));
+    regk_mkdirp_len_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(gp);
+    std::vector<unsigned long long> gs(gt / SUPER + 1);
+    CK(cudaMemcpyAsync(gs.data(), gp.super_total, gs.size() * 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (unsigned long long v : gs)
+        *total += v;
+    if ((rc = ensure_dev(ctx, bytes, *total + 16)))
+        return rc;
+    gp.dir_bytes = (uint8_t *)bytes.p;
+    regk_mkdirp_gather_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(gp);
+    CK(cudaGetLastError());
+    *launches += 2;
+    return REGK_OK;
+}
+
+/* The directory set of the batch finished last (n >= 1 records) into ctx->ch: its distinct parents in parent order,
+   listed (valid, not "/") to drec / dlen and packed to dbytes / doff, the others' first records to unlisted. */
+static int children_dirs(regk_ctx *ctx)
+{
+    regk_ctx::Children &ch = ctx->ch;
+    cudaStream_t s = ctx->stream;
+    const uint64_t n = ctx->last.n;
+    int rc;
+    if ((rc = ensure_host(ctx, ch.h_count, CQ_NCOUNTERS * 8)) || (rc = ensure_dev(ctx, ch.count, CQ_NCOUNTERS * 8)))
+        return rc;
+    unsigned long long *hc = (unsigned long long *)ch.h_count.p;
+    ParentParams pp{};
+    if ((rc = enqueue_parent_pass(ctx, ch.pass, n, nullptr, &pp)))
+        return rc;
+    CK(cudaMemcpyAsync(hc, pp.n_unique, 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, "regk_children_requests")))
+        return rc;
+    const uint64_t nu = hc[0];
+    const uint64_t ntiles = (nu + MK_TILE - 1) / MK_TILE, tt = align16(ntiles * 4), st = (ntiles / SUPER + 1) * 8;
+    const size_t totals_bytes = 2 * tt + 2 * st + 16;
+    if ((rc = ensure_dev(ctx, ch.totals, totals_bytes)) || (rc = ensure_dev(ctx, ch.unlisted, nu * 8 + 8)) ||
+        (rc = ensure_dev(ctx, ch.drec, nu * 8 + 8)) || (rc = ensure_dev(ctx, ch.dlen, nu * 4 + 8)))
+        return rc;
+    uint8_t *tb = (uint8_t *)ch.totals.p;
+    ChDirParams dp{};
+    dp.path_bytes = ctx->last.path_bytes;
+    dp.path_off = ctx->last.path_off;
+    dp.parent_len = pp.parent_len;
+    dp.unique_first = pp.unique_first;
+    dp.nu = nu;
+    dp.tile_a = (uint32_t *)tb;
+    dp.tile_b = (uint32_t *)(tb + tt);
+    dp.super_a = (unsigned long long *)(tb + 2 * tt);
+    dp.super_b = (unsigned long long *)(tb + 2 * tt + st);
+    dp.counters = (unsigned long long *)ch.count.p;
+    dp.unlisted = (unsigned long long *)ch.unlisted.p;
+    dp.dir_rec = (unsigned long long *)ch.drec.p;
+    dp.dir_len = (uint32_t *)ch.dlen.p;
+    CK(cudaMemsetAsync(tb, 0, totals_bytes, s));
+    CK(cudaMemsetAsync(ch.count.p, 0, CQ_NCOUNTERS * 8, s));
+    regk_children_dirs_count_kernel<<<(unsigned)ntiles, MK_TILE, 0, s>>>(dp);
+    regk_children_dirs_kernel<<<(unsigned)ntiles, MK_TILE, 0, s>>>(dp);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(hc, ch.count.p, CQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, "regk_children_requests")))
+        return rc;
+    ch.d = hc[CQ_LISTED];
+    ch.n_unlisted = hc[CQ_UNLISTED];
+    ch.prefixes = hc[CQ_PREFIXES];
+    uint64_t bytes = 0;
+    uint32_t launches = 0;
+    return pack_strings(ctx, ch.d, ctx->last.path_bytes, ctx->last.path_off, (const unsigned long long *)ch.drec.p,
+        (const uint32_t *)ch.dlen.p, ch.totals, ch.dbytes, ch.doff, &bytes, &launches);
+}
+
+int regk_children_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
+{
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_children_requests: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Children &ch = ctx->ch;
+    if (o->op == REGK_ZK_DELETE) {
+        if (o->group > 65536)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_children_requests: at most 65536 operations per multi transaction");
+        if (ctx->pending)
+            return fail(ctx, REGK_ERR_STATE, "regk_children_requests: batches are still in flight; finish them first");
+        if (!ch.read)
+            return fail(ctx, REGK_ERR_STATE, "regk_children_requests: no stale list on this context; call regk_read_children first");
+        CK(cudaSetDevice(ctx->device));
+        FrameSrc src{ch.n_stale, (const uint8_t *)ch.sbytes.p, (const unsigned long long *)ch.soff.p, nullptr, nullptr};
+        src.who = "regk_children_requests";
+        return frame_requests(ctx, src, o, ch.frames[1], out);
+    }
+    if (o->op != REGK_ZK_GETCHILDREN)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_children_requests: op %u is not getChildren (8) or delete (2)", o->op);
+    if (o->group != 0)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_children_requests: getChildren requests cannot go in a multi transaction "
+                                               "(group %u)", o->group);
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_children_requests: batches are still in flight; finish them first");
+    if (!ctx->last.path_off || !ctx->last.path_bytes || ctx->last.n == 0)
+        return fail(ctx, REGK_ERR_STATE, "regk_children_requests: no finished batch with a path stream on this context (an "
+                                         "empty batch, a REGK_NO_PATH batch or a REGK_JOB_STEP result leaves none)");
+    if (ctx->last.alias)
+        return fail(ctx, REGK_ERR_STATE, "regk_children_requests: the batch finished last holds alias nodes; their parents are "
+                                         "domain directories that hold other services, not service directories");
+    if (ctx->last.n >= 0xFFFFFFFEull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_children_requests: batch too large");
+    CK(cudaSetDevice(ctx->device));
+    ch.framed = false;
+    int rc;
+    if ((rc = children_dirs(ctx)))
+        return rc;
+    FrameSrc src{ch.d, (const uint8_t *)ch.dbytes.p, (const unsigned long long *)ch.doff.p, nullptr, nullptr};
+    src.who = "regk_children_requests";
+    if ((rc = frame_requests(ctx, src, o, ch.frames[0], out)))
+        return rc;
+    ch.framed = true;
+    ch.gen = ctx->last.gen;
+    ch.n = ctx->last.n;
+    ch.xid = o->xid_base;
+    return REGK_OK;
+}
+
+static const char *children_reason(uint32_t code)
+{
+    switch (code) {
+    case CH_TRUNC: return "the stream ends inside the frame";
+    case CH_BAD_LEN: return "a frame length below 16 (no room for a ReplyHeader)";
+    case CH_NEG_XID: return "a negative xid other than -1 (notification) or -2 (ping)";
+    case CH_XID_RANGE: return "an xid outside the framed requests";
+    case CH_ERR_BODY: return "an error reply with a body";
+    case CH_SUCC_LEN: return "a success frame too short for its count";
+    case CH_NEG_COUNT: return "a child count below -1";
+    case CH_ORDER: return "a reply out of order, or for a directory that already has one";
+    case CH_ENT_TRUNC: return "an entry runs past the end of its frame";
+    case CH_ENT_EMPTY: return "an entry with an empty name";
+    case CH_NAME_SLASH: return "a name holding '/'";
+    case CH_NAME_NUL: return "a name holding a NUL byte";
+    case CH_NAME_DOT: return "a name that is '.' or '..'";
+    case CH_ENT_END: return "the entries end before the frame does";
+    default: return "internal error";
+    }
+}
+
+/* The chain machinery of regk_replies.cuh over the candidates p->word .. p->tile_base already count: compact, J_0 .. J_K
+   (2^(K+1) > reach), and the marking from the seeds `seed` enqueues.  Sets p->cand, p->marked, p->C; *j0 = J_0. */
+static int chain_pass(regk_ctx *ctx, RepParams *p, uint64_t tiles_s, uint64_t reach, DevBuf &cand, DevBuf &mark,
+    DevBuf &jump, const std::function<void(const RepParams &)> &seed, uint32_t **j0, uint32_t *launches, const char *who)
+{
+    cudaStream_t s = ctx->stream;
+    const uint64_t nsup = tiles_s / SUPER + 1;
+    std::vector<unsigned long long> sup(nsup, 0);
+    CK(cudaMemcpyAsync(sup.data(), p->super_total, nsup * 8, cudaMemcpyDeviceToHost, s));
+    int rc;
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    uint64_t C = 0;
+    for (unsigned long long v : sup)
+        C += v;
+    if (C >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: %llu plausible positions in the stream: must be below 2^32 - 1", who,
+            (unsigned long long)C);
+    uint32_t K = 0;
+    while ((1ull << (K + 1)) <= std::min<uint64_t>(reach, C))
+        K++;
+    if ((rc = ensure_dev(ctx, cand, C * 8 + 16)) || (rc = ensure_dev(ctx, mark, C + 16)) ||
+        (rc = ensure_dev(ctx, jump, (size_t)(K + 1) * C * 4 + 16)))
+        return rc;
+    p->cand = (unsigned long long *)cand.p;
+    p->marked = (uint8_t *)mark.p;
+    p->C = C;
+    uint32_t *J = (uint32_t *)jump.p;
+    *j0 = J;
+    if (!C)
+        return REGK_OK;
+    const unsigned g256 = (unsigned)((C + 255) / 256);
+    regk_replies_compact_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(*p);
+    regk_replies_succ_kernel<<<g256, 256, 0, s>>>(*p, J);
+    for (uint32_t l = 0; l < K; l++)
+        regk_replies_jump_kernel<<<g256, 256, 0, s>>>(J + (size_t)l * C, J + (size_t)(l + 1) * C, C);
+    CK(cudaMemsetAsync(p->marked, 0, C, s));
+    seed(*p);
+    for (uint32_t l = K + 1; l-- > 0;)
+        regk_replies_mark_kernel<<<g256, 256, 0, s>>>(*p, J + (size_t)l * C, 0u);
+    CK(cudaGetLastError());
+    *launches += 2 * K + 4;
+    return REGK_OK;
+}
+
+int regk_read_children(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, uint32_t flags, regk_children *out)
+{
+    const char *who = "regk_read_children";
+    if (!ctx || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Children &ch = ctx->ch;
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_children: batches are still in flight; finish them first");
+    if (!ch.framed)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_children: no getChildren framing (regk_children_requests with "
+                                         "REGK_ZK_GETCHILDREN) of the batch finished last");
+    if (ch.gen != ctx->last.gen || !ctx->last.path_off)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_children: a batch finished after the getChildren framing; frame its "
+                                         "getChildren requests first");
+    if (!bytes && len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: NULL stream of %llu bytes", (unsigned long long)len);
+    if (start > len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: start %llu is past the stream's %llu bytes",
+            (unsigned long long)start, (unsigned long long)len);
+    const bool in_dev = flags & REGK_IN_DEVICE, dev_out = flags & REGK_OUT_DEVICE;
+    if (in_dev && ((uintptr_t)bytes & 15u))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: misaligned device stream (16-byte alignment needed)");
+    const uint64_t d = ch.d;
+    const int32_t xb = ch.xid;
+    for (int32_t reserved : {-1, -2})
+        if ((uint64_t)((uint32_t)reserved - (uint32_t)xb) < d)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: the framed xids [%d, %d + %llu) cover %d, which ZooKeeper "
+                                                   "uses for %s", xb, xb, (unsigned long long)d, reserved,
+                        reserved == -1 ? "watch notifications" : "pings");
+    if (d >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: %llu directories: must be below 2^32 - 1", (unsigned long long)d);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    ch.read = false;
+    int rc;
+    for (Event &ev : ch.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
+    const uint8_t *ds = bytes;
+    if (!in_dev && len) {
+        if ((rc = stage_in(ctx, ch.stream, bytes, len, s)))
+            return rc;
+        ds = (const uint8_t *)ch.stream.p;
+    }
+    const uint64_t nblk = (len + 15) / 16, tiles_s = (nblk + RP_TILE - 1) / RP_TILE;
+    const size_t totals_bytes = align16(tiles_s * 4) + (tiles_s / SUPER + 1) * 8;
+    const size_t d8 = d * 8 + 16, d4 = d * 4 + 16;
+    if ((rc = ensure_dev(ctx, ch.word, nblk * 4 + 16)) || (rc = ensure_dev(ctx, ch.ftotals, totals_bytes)) ||
+        (rc = ensure_dev(ctx, ch.tile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, ch.fpos, d8)) ||
+        (rc = ensure_dev(ctx, ch.fend, d8)) || (rc = ensure_dev(ctx, ch.err, d4)) || (rc = ensure_dev(ctx, ch.cnt, d4)) ||
+        (rc = ensure_dev(ctx, ch.seed_g, d4)) || (rc = ensure_dev(ctx, ch.last_g1, d4)) ||
+        (rc = ensure_dev(ctx, ch.name_bad, d4)) || (rc = ensure_dev(ctx, ch.end_pos, d8)) ||
+        (rc = ensure_dev(ctx, ch.fault_pos, d8)) || (rc = ensure_dev(ctx, ch.child_off, d8)) ||
+        (rc = ensure_host(ctx, ch.h_count, CQ_NCOUNTERS * 8)) || (rc = ensure_dev(ctx, ch.count, CQ_NCOUNTERS * 8)))
+        return rc;
+    ChParams cp{};
+    RepParams &p = cp.r;
+    p.s = ds;
+    p.len = len;
+    p.xid_base = xb;
+    p.n = d;
+    p.word = (uint32_t *)ch.word.p;
+    p.tile_total = (uint32_t *)ch.ftotals.p;
+    p.super_total = (unsigned long long *)((uint8_t *)ch.ftotals.p + align16(tiles_s * 4));
+    p.tile_base = (unsigned long long *)ch.tile_base.p;
+    p.counters = (unsigned long long *)ch.count.p;
+    cp.start = start;
+    cp.d = d;
+    cp.fpos = (unsigned long long *)ch.fpos.p;
+    cp.fend = (unsigned long long *)ch.fend.p;
+    cp.err = (int32_t *)ch.err.p;
+    cp.cnt = (uint32_t *)ch.cnt.p;
+    cp.seed_g = (uint32_t *)ch.seed_g.p;
+    cp.last_g1 = (uint32_t *)ch.last_g1.p;
+    cp.name_bad = (uint32_t *)ch.name_bad.p;
+    cp.end_pos = (unsigned long long *)ch.end_pos.p;
+    cp.fault_pos = (unsigned long long *)ch.fault_pos.p;
+    cp.child_off = (unsigned long long *)ch.child_off.p;
+    cp.dir_len = (const uint32_t *)ch.dlen.p;
+    unsigned long long *hc = (unsigned long long *)ch.h_count.p;
+    CK(cudaMemsetAsync(p.counters, 0, CQ_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(p.counters + RQ_ERR, 0xFF, 8, s));
+    CK(cudaMemsetAsync(p.counters + CQ_ENT_ERR, 0xFF, 8, s));
+    CK(cudaMemsetAsync(p.tile_total, 0, totals_bytes, s));
+    CK(cudaEventRecord(ch.ev[0], s));
+    uint32_t launches = 0;
+    /* 1. the frame chain from `start` and the replies of the d directories */
+    RepParams pf = p;
+    if (d && len) {
+        regk_children_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(cp);
+        CK(cudaGetLastError());
+        launches++;
+        uint32_t *J = nullptr;
+        if ((rc = chain_pass(ctx, &pf, tiles_s, ~0ull, ch.cand, ch.mark, ch.jump, [&](const RepParams &q) {
+                regk_children_seed_kernel<<<1, 256, 0, s>>>(q, nullptr, nullptr, 1, start);
+            }, &J, &launches, who)))
+            return rc;
+        if (pf.C) {
+            const uint64_t tiles_c = (pf.C + RP_TILE - 1) / RP_TILE;
+            const size_t t2 = align16(tiles_c * 4) + (tiles_c / SUPER + 1) * 8;
+            if ((rc = ensure_dev(ctx, ch.totals2, t2)))
+                return rc;
+            cp.r = pf;
+            cp.r.tile_total = (uint32_t *)ch.totals2.p;
+            cp.r.super_total = (unsigned long long *)((uint8_t *)ch.totals2.p + align16(tiles_c * 4));
+            CK(cudaMemsetAsync(ch.totals2.p, 0, t2, s));
+            regk_replies_chain_count_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(cp.r);
+            regk_children_chain_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(cp);
+            CK(cudaGetLastError());
+            launches += 3;
+        }
+    }
+    CK(cudaMemcpyAsync(hc, p.counters, CQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    const uint64_t frame_err_k = hc[RQ_ERR] != ~0ull ? hc[RQ_ERR] >> 8 : d;
+    const uint64_t d_eff = std::min<uint64_t>(std::min<uint64_t>(frame_err_k, hc[RQ_NREP]), d);
+    const uint64_t n_skipped = hc[RQ_SKIP], n_found = hc[RQ_FOUND], n_missing = hc[RQ_MISSING], n_error = hc[RQ_ERROR];
+    const uint64_t consumed = d ? hc[RQ_CONSUMED] : start;
+    /* 2. the entry chains inside the success frames of the first d_eff replies; every frame's entries against its count */
+    uint64_t ne = 0;
+    if (d_eff) {
+        cp.d_eff = d_eff;
+        if ((rc = ensure_dev(ctx, ch.eword, nblk * 4 + 16)) || (rc = ensure_dev(ctx, ch.etotals, totals_bytes)) ||
+            (rc = ensure_dev(ctx, ch.etile_base, tiles_s * 8 + 16)))
+            return rc;
+        RepParams pe = p;
+        pe.word = (uint32_t *)ch.eword.p;
+        pe.tile_total = (uint32_t *)ch.etotals.p;
+        pe.super_total = (unsigned long long *)((uint8_t *)ch.etotals.p + align16(tiles_s * 4));
+        pe.tile_base = (unsigned long long *)ch.etile_base.p;
+        CK(cudaMemsetAsync(pe.tile_total, 0, totals_bytes, s));
+        CK(cudaMemsetAsync(cp.seed_g, 0xFF, d_eff * 4, s));
+        CK(cudaMemsetAsync(cp.name_bad, 0xFF, d_eff * 4, s));
+        CK(cudaMemsetAsync(cp.last_g1, 0, d_eff * 4, s));
+        cp.r = pe;
+        regk_children_ent_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(cp);
+        CK(cudaGetLastError());
+        launches++;
+        uint32_t *J = nullptr;
+        const unsigned gd = (unsigned)((d_eff + 255) / 256);
+        if ((rc = chain_pass(ctx, &pe, tiles_s, hc[CQ_MAXC] + 1, ch.ecand, ch.emark, ch.ejump, [&](const RepParams &q) {
+                regk_children_seed_kernel<<<gd, 256, 0, s>>>(q, cp.fpos, cp.cnt, d_eff, 24ull);
+            }, &J, &launches, who)))
+            return rc;
+        const uint64_t Ce = pe.C;
+        if ((rc = ensure_dev(ctx, ch.ent_pos, Ce * 8 + 16)) || (rc = ensure_dev(ctx, ch.ent_nlen, Ce * 4 + 16)) ||
+            (rc = ensure_dev(ctx, ch.ent_k, Ce * 4 + 16)) || (rc = ensure_dev(ctx, ch.ent_plen, Ce * 4 + 16)))
+            return rc;
+        cp.j0 = J;
+        cp.ent_pos = (unsigned long long *)ch.ent_pos.p;
+        cp.ent_nlen = (uint32_t *)ch.ent_nlen.p;
+        cp.ent_k = (uint32_t *)ch.ent_k.p;
+        cp.ent_plen = (uint32_t *)ch.ent_plen.p;
+        cp.r = pe;
+        if (Ce) {
+            const uint64_t tiles_e = (Ce + RP_TILE - 1) / RP_TILE;
+            const size_t t2 = align16(tiles_e * 4) + (tiles_e / SUPER + 1) * 8;
+            if ((rc = ensure_dev(ctx, ch.etotals2, t2)))
+                return rc;
+            cp.r.tile_total = (uint32_t *)ch.etotals2.p;
+            cp.r.super_total = (unsigned long long *)((uint8_t *)ch.etotals2.p + align16(tiles_e * 4));
+            CK(cudaMemsetAsync(ch.etotals2.p, 0, t2, s));
+            regk_children_ent_count_kernel<<<(unsigned)tiles_e, RP_TILE, 0, s>>>(cp.r);
+            regk_children_ent_kernel<<<(unsigned)tiles_e, RP_TILE, 0, s>>>(cp);
+            launches += 2;
+        }
+        regk_children_ent_frame_kernel<<<gd, 256, 0, s>>>(cp);
+        CK(cudaGetLastError());
+        launches++;
+        CK(cudaMemcpyAsync(hc, p.counters, CQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        ne = hc[CQ_NENT];
+    }
+    /* refusals: the first fault a front-to-back reader meets - an entry fault of a frame before any frame fault */
+    if (hc[CQ_ENT_ERR] != ~0ull) {
+        const uint64_t k = hc[CQ_ENT_ERR] >> 8;
+        const uint32_t code = (uint32_t)(hc[CQ_ENT_ERR] & 0xFF);
+        unsigned long long at[2] = {0, 0};
+        CK(cudaMemcpyAsync(&at[0], cp.fault_pos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&at[1], cp.fpos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: byte %llu: %s (entry of the reply frame at byte %llu); "
+                                               "expected the reply to directory %llu (xid %d)", at[0], children_reason(code), at[1],
+                    (unsigned long long)k, (int32_t)((uint32_t)xb + (uint32_t)k));
+    }
+    if (hc[RQ_ERR] != ~0ull) {
+        const uint64_t k = hc[RQ_ERR] >> 8;
+        const uint32_t code = (uint32_t)(hc[RQ_ERR] & 0xFF);
+        unsigned long long pos = 0;
+        CK(cudaMemcpyAsync(&pos, cp.fpos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: byte %llu: %s; expected the reply to directory %llu (xid %d)",
+            pos, children_reason(code), (unsigned long long)k, (int32_t)((uint32_t)xb + (uint32_t)k));
+    }
+    if (hc[RQ_NREP] < d) {
+        /* the chain stops before the d-th reply: the frame check where it stops names the reason */
+        uint64_t stop = start;
+        if (pf.C) {
+            regk_replies_stop_kernel<<<(unsigned)((pf.C + 255) / 256), 256, 0, s>>>(pf);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(hc + RQ_STOP, p.counters + RQ_STOP, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            stop = std::max<uint64_t>(stop, hc[RQ_STOP]);
+        }
+        const uint64_t done = hc[RQ_NREP];
+        uint8_t head[24] = {0};
+        const uint64_t avail = len - stop, take = std::min<uint64_t>(avail, sizeof head);
+        if (take) {
+            CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+        }
+        ChildHead h;
+        const uint32_t code = children_head(head, avail, xb, d, &h);
+        const int32_t want = (int32_t)((uint32_t)xb + (uint32_t)done);
+        if (code == CH_TRUNC)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: byte %llu: the stream ends before the reply to directory "
+                                                   "%llu (xid %d) is complete; %llu of %llu replies complete",
+                        (unsigned long long)stop, (unsigned long long)done, want, (unsigned long long)done, (unsigned long long)d);
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: byte %llu: %s (len %d, xid %d); expected the reply to "
+                                               "directory %llu (xid %d)", (unsigned long long)stop,
+                    code ? children_reason(code) : "internal error", h.len, h.xid, (unsigned long long)done, want);
+    }
+    if (ne >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: %llu children: must be below 2^32 - 1", (unsigned long long)ne);
+    if ((rc = ensure_dev(ctx, ch.child_off, d * 8 + 16)))
+        return rc;
+    CK(cudaMemcpyAsync(cp.child_off + d, &ne, 8, cudaMemcpyHostToDevice, s));
+    /* 3. the listing paths */
+    uint64_t lst_total = 0;
+    {
+        const uint64_t gt = (ne + MK_TILE - 1) / MK_TILE;
+        if ((rc = ensure_dev(ctx, ch.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)) ||
+            (rc = ensure_dev(ctx, ch.lst_off, (ne + 1) * 8)) || (rc = ensure_dev(ctx, ch.lst_zero, (ne + 1) * 8)))
+            return rc;
+        CK(cudaMemsetAsync(ch.lst_zero.p, 0, (ne + 1) * 8, s));
+        if (ne) {
+            MkGatherParams gp{};
+            gp.n_dirs = ne;
+            gp.dir_len = cp.ent_plen;
+            gp.tile_total = (unsigned long long *)ch.gtotals.p;
+            gp.super_total = gp.tile_total + gt;
+            CK(cudaMemsetAsync(gp.super_total, 0, (gt / SUPER + 1) * 8, s));
+            regk_mkdirp_len_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(gp);
+            std::vector<unsigned long long> gs(gt / SUPER + 1);
+            CK(cudaMemcpyAsync(gs.data(), gp.super_total, gs.size() * 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            for (unsigned long long v : gs)
+                lst_total += v;
+            if ((rc = ensure_dev(ctx, ch.lst_bytes, lst_total + 16)))
+                return rc;
+            ChGatherParams g{};
+            g.n = ne;
+            g.tile_total = gp.tile_total;
+            g.super_total = gp.super_total;
+            g.ent_k = cp.ent_k;
+            g.ent_nlen = cp.ent_nlen;
+            g.ent_plen = cp.ent_plen;
+            g.ent_pos = cp.ent_pos;
+            g.dir_bytes = (const uint8_t *)ch.dbytes.p;
+            g.dir_off = (const unsigned long long *)ch.doff.p;
+            g.s = ds;
+            g.out_bytes = (uint8_t *)ch.lst_bytes.p;
+            g.out_off = (unsigned long long *)ch.lst_off.p;
+            regk_children_gather_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(g);
+            CK(cudaGetLastError());
+            launches += 2;
+        } else {
+            if ((rc = ensure_dev(ctx, ch.lst_bytes, 16)))
+                return rc;
+            CK(cudaMemsetAsync(ch.lst_off.p, 0, 8, s));
+        }
+    }
+    /* 4. the keep table, every listing path's class, the stale list and its packed paths */
+    uint64_t n_stale = 0;
+    const uint64_t tiles_l = (ne + MK_TILE - 1) / MK_TILE;
+    if ((rc = ensure_dev(ctx, ch.cls, ne + 16)) || (rc = ensure_dev(ctx, ch.stale, ne * 8 + 16)) ||
+        (rc = ensure_dev(ctx, ch.stale_len, ne * 4 + 16)))
+        return rc;
+    if (ne) {
+        const uint64_t entries = ch.n + ch.prefixes;
+        uint64_t slots = 1024;
+        while (slots < 2 * entries)
+            slots <<= 1;
+        if (slots > (1ull << 32))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_children: %llu paths and directories are too many for one table",
+                (unsigned long long)entries);
+        const size_t st_bytes = align16(tiles_l * 4) + (tiles_l / SUPER + 1) * 8;
+        if ((rc = ensure_dev(ctx, ch.table, slots * 8)) || (rc = ensure_dev(ctx, ch.stotals, st_bytes)))
+            return rc;
+        ChKeepParams kp{};
+        kp.path_bytes = ctx->last.path_bytes;
+        kp.path_off = ctx->last.path_off;
+        kp.n = ch.n;
+        kp.dir_rec = (const unsigned long long *)ch.drec.p;
+        kp.dir_len = (const uint32_t *)ch.dlen.p;
+        kp.d = d;
+        kp.table = (unsigned long long *)ch.table.p;
+        kp.mask = (uint32_t)(slots - 1);
+        kp.lst_bytes = (const uint8_t *)ch.lst_bytes.p;
+        kp.lst_off = (const unsigned long long *)ch.lst_off.p;
+        kp.n_children = ne;
+        kp.cls = (uint8_t *)ch.cls.p;
+        kp.tile_total = (uint32_t *)ch.stotals.p;
+        kp.super_total = (unsigned long long *)((uint8_t *)ch.stotals.p + align16(tiles_l * 4));
+        kp.stale = (unsigned long long *)ch.stale.p;
+        kp.stale_len = (uint32_t *)ch.stale_len.p;
+        kp.counters = p.counters;
+        CK(cudaMemsetAsync(kp.table, 0, slots * 8, s));
+        CK(cudaMemsetAsync(ch.stotals.p, 0, st_bytes, s));
+        regk_children_keep_paths_kernel<<<(unsigned)((ch.n + 255) / 256), 256, 0, s>>>(kp);
+        if (d)
+            regk_children_keep_dirs_kernel<<<(unsigned)((d + 255) / 256), 256, 0, s>>>(kp);
+        regk_children_probe_kernel<<<(unsigned)tiles_l, MK_TILE, 0, s>>>(kp);
+        regk_children_stale_kernel<<<(unsigned)tiles_l, MK_TILE, 0, s>>>(kp);
+        CK(cudaGetLastError());
+        launches += d ? 4 : 3;
+        CK(cudaMemcpyAsync(hc + CQ_STALE, p.counters + CQ_STALE, 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        n_stale = hc[CQ_STALE];
+    }
+    uint64_t stale_bytes = 0;
+    if ((rc = pack_strings(ctx, n_stale, (const uint8_t *)ch.lst_bytes.p, (const unsigned long long *)ch.lst_off.p,
+             (const unsigned long long *)ch.stale.p, (const uint32_t *)ch.stale_len.p, ch.gtotals, ch.sbytes, ch.soff,
+             &stale_bytes, &launches)))
+        return rc;
+    /* the directory set this read answers, kept with the read (a later framing rebuilds the framing's own) */
+    const uint64_t nun = ch.n_unlisted;
+    if ((rc = ensure_dev(ctx, ch.r_drec, d * 8 + 8)) || (rc = ensure_dev(ctx, ch.r_dlen, d * 4 + 8)) ||
+        (rc = ensure_dev(ctx, ch.r_unlisted, nun * 8 + 8)))
+        return rc;
+    if (d) {
+        CK(cudaMemcpyAsync(ch.r_drec.p, ch.drec.p, d * 8, cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpyAsync(ch.r_dlen.p, ch.dlen.p, d * 4, cudaMemcpyDeviceToDevice, s));
+    }
+    if (nun)
+        CK(cudaMemcpyAsync(ch.r_unlisted.p, ch.unlisted.p, nun * 8, cudaMemcpyDeviceToDevice, s));
+    CK(cudaEventRecord(ch.ev[1], s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, ch.ev[0], ch.ev[1]);
+    const void *src[7] = {ch.r_drec.p, ch.r_dlen.p, ch.err.p, ch.child_off.p, ch.cls.p, ch.stale.p, ch.r_unlisted.p};
+    if (!dev_out) {
+        HostBuf *hb[7] = {&ch.h_drec, &ch.h_dlen, &ch.h_err, &ch.h_child_off, &ch.h_cls, &ch.h_stale, &ch.h_unlisted};
+        const size_t sz[7] = {d * 8, d * 4, d * 4, (d + 1) * 8, ne, n_stale * 8, nun * 8};
+        for (int k = 0; k < 7; k++) {
+            if ((rc = to_host(ctx, *hb[k], src[k], sz[k], s)))
+                return rc;
+            src[k] = hb[k]->p;
+        }
+        CK(cudaStreamSynchronize(s));
+    }
+    ch.read = true;
+    ch.n_stale = n_stale;
+    out->n_dirs = d;
+    out->n_children = ne;
+    out->n_stale = n_stale;
+    out->n_found = n_found;
+    out->n_missing = n_missing;
+    out->n_error = n_error;
+    out->n_skipped = n_skipped;
+    out->consumed = consumed;
+    out->n_unlisted = nun;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->dir_rec = (const uint64_t *)src[0];
+    out->dir_len = (const uint32_t *)src[1];
+    out->err = (const int32_t *)src[2];
+    out->child_off = (const uint64_t *)src[3];
+    out->cls = (const uint8_t *)src[4];
+    out->stale = (const uint64_t *)src[5];
+    out->unlisted = (const uint64_t *)src[6];
+    out->listing.n = ne;
+    out->listing.flags = REGK_IN_DEVICE;
+    out->listing.host_nodes = 1;
+    out->listing.path_total = lst_total;
+    out->listing.json_total = 0;
+    out->listing.path_bytes = (const uint8_t *)ch.lst_bytes.p;
+    out->listing.path_off = (const uint64_t *)ch.lst_off.p;
+    out->listing.json_bytes = (const uint8_t *)ch.lst_bytes.p;
+    out->listing.json_off = (const uint64_t *)ch.lst_zero.p;
     out->kernel_ms = ms;
     return REGK_OK;
 }
