@@ -760,6 +760,97 @@ typedef struct regk_children {
 int         regk_read_children(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, uint32_t flags,
                                regk_children *out);
 
+/*
+ * ---- the replies to the write frames this library made: each create, delete, setData and replace's outcome, mapped
+ * back to what it was framed for (the reference learns each write's outcome from its callback: cleanupPreviousEntries
+ * ignores NO_NODE, lib/register.js:88; zkplus' mkdirp ignores NODE_EXISTS) ---------------------------------------------
+ * Every successful write framing records what it framed, one record per source (opts->source):
+ *   REGK_RES_BATCH      the last regk_jute_frames, or regk_jute_requests with REGK_ZK_CREATE / _DELETE / _SETDATA (a
+ *                       REGK_ZK_GETDATA framing does not replace it); entry e = record e of the batch finished last
+ *   REGK_RES_MKDIRP     the last regk_mkdirp_requests; entry k = directory k of the mkdirp set
+ *   REGK_RES_RECONCILE  the last regk_reconcile_requests with opts->op (REGK_ZK_CREATE, _DELETE, _SETDATA or
+ *                       REGK_ZK_REPLACE: one record each, so the whole repair can be framed before anything is sent);
+ *                       entry e = list entry e
+ *   REGK_RES_STALE      the last regk_children_requests(REGK_ZK_DELETE); entry e = stale entry e
+ * The record holds the xid base, the frame count, the group (a replace frame holds max(g, 1) entries of two operations)
+ * and the entry count; the paths stay where the library keeps them (the batch's path stream, the mkdirp set, the
+ * reconcile's gathered streams, the packed stale paths).  REGK_ERR_STATE: no such framing, or the state it framed has
+ * changed since - a batch finished (BATCH), regk_mkdirp_dirs ran (MKDIRP), a reconcile ran (RECONCILE),
+ * regk_read_children ran (STALE) - or a pending batch.
+ * bytes[start, len) = what the caller read off the session after sending those frames, from the first reply's length
+ * word on; host memory, or device memory with REGK_IN_DEVICE in opts->flags (16-byte aligned; start need not be, so one
+ * stream can hold the replies of several sections: start = the previous section's consumed).  Positions count from
+ * bytes.  The k-th frame that is not a watch notification (xid -1) or a ping (xid -2) must carry xid_base + k and answers
+ * frame k; notifications and pings before the last reply are skipped and counted.
+ * Reply layouts (zookeeper.jute; big endian; frame = int len | ReplyHeader{int xid; long zxid; int err} | body):
+ *   create   err == 0: CreateResponse{path}, len == 20 + P; the path must equal the framed path byte for byte
+ *   delete   len == 16
+ *   setData  err == 0: Stat, len == 84; Stat.dataLength must equal the framed data's length; version[e] = Stat.version
+ *   error    err != 0: len == 16, no body; in a multi frame every operation then fails with err
+ *   multi    err == 0: MultiResponse, one MultiHeader{type, done = 0, err} + result per operation, then
+ *            MultiHeader{-1, 1, -1}.  Applied: typed results (type = the framed op; create 4 + P bytes of path, delete
+ *            none, setData a 68-byte Stat).  Rolled back: only ErrorResults (MultiHeader{-1, 0, e} ErrorResponse{e}, 13
+ *            bytes each): 0 before the failing operation, its code, then -2 (RUNTIMEINCONSISTENCY).
+ * Since a multi reply is all typed results or all ErrorResults and every framed path length is known, each entry's result
+ * position is closed form: frame + 20 + a prefix of the frame's result sizes (applied), frame + 20 + 13 x the operation
+ * index (rolled back).  cls[e]:
+ *   REGK_RES_DONE     the write took effect; also a delete answered NONODE (-101) and a mkdirp create answered
+ *                     NODEEXISTS (-110), the reference's two tolerances, with that code kept in err[e]
+ *   REGK_RES_FAILED   the entry's own operation failed (an error reply, the failing operation of a rolled-back multi, or
+ *                     any operation of a multi answered with a header error); err[e] is its code
+ *   REGK_RES_ABORTED  another entry's failure rolled its multi transaction back; err[e] is its operations' first nonzero
+ *                     code (-2 after the failing one), else 0
+ * version[e] = the new Stat.version of a setData that took effect, 0 for a create or replace that took effect, else -1.
+ * subject[e] = the record (BATCH; RECONCILE create, setData, replace), the snapshot node (RECONCILE delete), the directory
+ * (MKDIRP) or the listing entry (STALE) the entry was framed for.  failed[] / aborted[] list the FAILED / ABORTED entries
+ * ascending.  n_done + n_failed + n_aborted == n_entries.  The arrays are pinned host arrays, or device arrays with
+ * REGK_OUT_DEVICE; all stay valid until the next regk_read_results call.
+ * REGK_ERR_INVALID_ARG (the message names the byte position, that of the frame and of the entry, and the expected xid; it
+ * is the first fault a front-to-back reader meets): the stream ends before the last reply is complete, len < 16, a
+ * negative xid other than -1 / -2, an xid outside the framed range, a reply out of order, an error reply with a body, a
+ * success length that fits neither outcome of its frame, a MultiHeader of the wrong type, done flag or err, a missing
+ * closing MultiHeader, a create path echo that differs from the framed path, a Stat.dataLength that differs from the
+ * framed data, an ErrorResult whose two codes differ or that breaks the 0 / code / -2 order, a rolled-back multi with no
+ * nonzero ErrorResult; an xid range that covers -1 or -2; a source or op not listed above; start > len; NULL pointers; a
+ * misaligned device stream.
+ * PARITY UNPINNED: the layouts are restated from zookeeper.jute and the server's multi handling, and tested against an
+ * independent restatement, not against a server.
+ */
+#define REGK_RES_BATCH      1u
+#define REGK_RES_MKDIRP     2u
+#define REGK_RES_RECONCILE  3u
+#define REGK_RES_STALE      4u
+
+#define REGK_RES_DONE    0u         /* regk_results.cls[] */
+#define REGK_RES_FAILED  1u
+#define REGK_RES_ABORTED 2u
+
+typedef struct regk_results_opts {
+    uint32_t source;                /* REGK_RES_* */
+    uint32_t op;                    /* REGK_RES_RECONCILE: REGK_ZK_CREATE / _DELETE / _SETDATA / REGK_ZK_REPLACE */
+    uint32_t flags;                 /* REGK_IN_DEVICE | REGK_OUT_DEVICE */
+    uint32_t reserved;
+} regk_results_opts;
+
+typedef struct regk_results {
+    uint64_t n_frames, n_entries;
+    uint64_t n_done, n_failed, n_aborted;
+    uint64_t n_skipped;             /* watch notifications and pings met before the last reply */
+    uint64_t consumed;              /* stream position of the end of the last reply (start when there are no frames) */
+    uint32_t flags, launches;       /* REGK_OUT_DEVICE */
+    const int32_t  *frame_err;      /* [n_frames] ReplyHeader.err of frame k's reply */
+    const int32_t  *err;            /* [n_entries] */
+    const uint8_t  *cls;            /* [n_entries] REGK_RES_DONE / _FAILED / _ABORTED */
+    const int32_t  *version;        /* [n_entries] */
+    const uint64_t *subject;        /* [n_entries] */
+    const uint64_t *failed;         /* [n_failed] entry indices, ascending */
+    const uint64_t *aborted;        /* [n_aborted] */
+    float kernel_ms;
+} regk_results;
+
+int         regk_read_results(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start,
+                              const regk_results_opts *opts, regk_results *out);
+
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);
 int64_t     regk_get_option(const regk_ctx *ctx, const char *name);

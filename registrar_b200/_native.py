@@ -311,6 +311,52 @@ class Children:
         return [lst[int(e)] for e in self.stale]
 
 
+RES_BATCH, RES_MKDIRP, RES_RECONCILE, RES_STALE = 1, 2, 3, 4       # read_results sources
+RES_DONE, RES_FAILED, RES_ABORTED = 0, 1, 2                          # Results.cls
+
+
+class CResultsOpts(C.Structure):     # regk_results_opts
+    _fields_ = [("source", C.c_uint32), ("op", C.c_uint32), ("flags", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class CResults(C.Structure):         # regk_results
+    _fields_ = [("n_frames", C.c_uint64), ("n_entries", C.c_uint64), ("n_done", C.c_uint64), ("n_failed", C.c_uint64),
+                ("n_aborted", C.c_uint64), ("n_skipped", C.c_uint64), ("consumed", C.c_uint64),
+                ("flags", C.c_uint32), ("launches", C.c_uint32), ("frame_err", C.c_void_p), ("err", C.c_void_p),
+                ("cls", C.c_void_p), ("version", C.c_void_p), ("subject", C.c_void_p), ("failed", C.c_void_p),
+                ("aborted", C.c_void_p), ("kernel_ms", C.c_float)]
+
+
+class Results:
+    """What read_results() made of the replies to one write framing: frame_err[k] is frame k's ReplyHeader.err; entry e
+    (list entry e of the framing) has err[e], cls[e] (RES_DONE, RES_FAILED: its own operation failed, RES_ABORTED: its
+    multi transaction was rolled back by another entry), version[e] (the new Stat.version of a setData that took effect,
+    0 for a create or replace that did, else -1) and subject[e] (the record, snapshot node, directory or listing entry it
+    was framed for).  failed / aborted list those entries ascending.  Counts: n_frames, n_entries, n_done, n_failed,
+    n_aborted, n_skipped, and `consumed` (stream position of the end of the last reply)."""
+
+    def __init__(self, out):
+        f, n = int(out.n_frames), int(out.n_entries)
+        self.n_frames, self.n_entries = f, n
+        self.n_done, self.n_failed, self.n_aborted = int(out.n_done), int(out.n_failed), int(out.n_aborted)
+        self.n_skipped, self.consumed = int(out.n_skipped), int(out.consumed)
+        self.launches, self.kernel_ms = int(out.launches), float(out.kernel_ms)
+        self.frame_err = _as_np(out.frame_err, f, np.int32).copy()
+        self.err = _as_np(out.err, n, np.int32).copy()
+        self.cls = _as_np(out.cls, n, np.uint8).copy()
+        self.version = _as_np(out.version, n, np.int32).copy()
+        self.subject = _as_np(out.subject, n, np.uint64).copy()
+        self.failed = _as_np(out.failed, self.n_failed, np.uint64).copy()
+        self.aborted = _as_np(out.aborted, self.n_aborted, np.uint64).copy()
+
+    def failed_subjects(self):
+        """the subjects of the FAILED entries, ascending by entry"""
+        return self.subject[self.failed.astype(np.int64)]
+
+    def aborted_subjects(self):
+        return self.subject[self.aborted.astype(np.int64)]
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -323,7 +369,7 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_gather_push", "regk_parent_dirs", "regk_job_bind", "regk_service_records",
            "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records", "regk_mkdirp_dirs",
            "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned",
-           "regk_read_replies", "regk_children_requests", "regk_read_children"]
+           "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results"]
 
 _lib = None
 
@@ -383,6 +429,7 @@ def load_library():
     lib.regk_read_replies.argtypes = [vp, vp, u64, u32, C.POINTER(CReplies)]
     lib.regk_children_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     lib.regk_read_children.argtypes = [vp, vp, u64, u64, u32, C.POINTER(CChildren)]
+    lib.regk_read_results.argtypes = [vp, vp, u64, u64, C.POINTER(CResultsOpts), C.POINTER(CResults)]
     _lib = lib
     return lib
 
@@ -823,6 +870,32 @@ class Context:
         del keep
         self._check(rc)
         return out if device else Children(self, out)
+
+    # -- the replies to the write frames: which create, delete, setData and replace took effect --
+    def read_results(self, stream, source: int, op: Optional[int] = None, start: int = 0, device: bool = False):
+        """regk_read_results: `stream` (a NumPy uint8 array, or a contiguous CUDA uint8 tensor) holds, from byte `start`
+        on, the replies to the last write framing of `source`: RES_BATCH (jute_requests create / delete / setData),
+        RES_MKDIRP (mkdirp_requests), RES_RECONCILE (reconcile_requests with `op`) or RES_STALE (children_requests
+        ZK_DELETE).  Returns a Results, or the raw CResults (its arrays on the device) with device=True.  A delete
+        answered NONODE and a mkdirp create answered NODEEXISTS count as done, with the code kept in err."""
+        flags = FLAG_OUT_DEVICE if device else 0
+        if hasattr(stream, "data_ptr"):
+            import torch
+            if not stream.is_cuda or stream.dtype != torch.uint8 or not stream.is_contiguous():
+                raise ValueError("a device stream is a contiguous CUDA uint8 tensor")
+            keep, ptr, n = stream, stream.data_ptr() or None, stream.numel()
+            flags |= FLAG_IN_DEVICE
+        else:
+            keep = np.ascontiguousarray(stream)
+            if keep.dtype != np.uint8 or keep.ndim != 1:
+                raise ValueError("a host stream is a one-dimensional uint8 array")
+            ptr, n = _np_ptr(keep), keep.size
+        o = CResultsOpts(int(source), int(op or 0), flags, 0)
+        out = CResults()
+        rc = self._lib.regk_read_results(self._h, ptr, n, int(start), C.byref(o), C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else Results(out)
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

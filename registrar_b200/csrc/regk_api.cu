@@ -34,6 +34,7 @@
 #include "regk_reconcile.cuh"
 #include "regk_replies.cuh"
 #include "regk_children.cuh"
+#include "regk_results.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -188,6 +189,7 @@ struct regk_ctx {
         FrameBufs frames;
         bool valid = false;                     /* the set of the last regk_mkdirp_dirs call is in drec .. invalid */
         uint64_t n_dirs = 0, bytes = 0;
+        uint64_t gen = 0;                       /* bumped by every regk_mkdirp_dirs */
     } mk;
     /* regk_reconcile / regk_reconcile_owned (regk_reconcile.cuh): staged snapshot and stats, tables, outputs, lists,
        versions, the gathered request streams; regk_reconcile_requests' frames */
@@ -205,6 +207,7 @@ struct regk_ctx {
         bool owned = false;                     /* ... and it was regk_reconcile_owned: versions in ver */
         uint32_t zk_flags = 0;                  /* the CreateMode regk_reconcile_owned classified with */
         uint64_t n_list[RC_NLISTS] = {};        /* entries of each list: create, update, dup, replace, delete */
+        uint64_t gen = 0;                       /* bumped by every reconcile call */
     } rc;
     /* the last REGK_ZK_GETDATA framing: the batch it framed, xid_base, n (regk_read_replies reads its replies) */
     bool gd_valid = false;
@@ -240,7 +243,24 @@ struct regk_ctx {
         Event ev[2];
         bool read = false;                      /* the stale list of the last regk_read_children is in stale .. soff */
         uint64_t n_stale = 0;
+        uint64_t read_gen = 0;                  /* bumped by every regk_read_children */
     } ch;
+    /* regk_read_results (regk_results.cuh): what each write framing framed (one record per source, four for the
+       reconcile ops), and the last read's chain, per-frame and per-entry arrays and lists */
+    struct ResDesc {
+        bool valid = false;
+        ResFraming f{};
+        const unsigned long long *subject = nullptr;    /* device: what entry e stands for; NULL = e */
+        int32_t tol = 0;                        /* the code that still counts as done */
+        uint64_t gen = 0;                       /* the generation of the state it framed */
+    };
+    struct Results {
+        ResDesc batch, mkdirp, stale, rec[4];   /* rec: create, delete, setData, replace */
+        DevBuf stream, word, totals, tile_base, cand, mark, jump, totals2, count, fpos, ferr, err, cls, ver, subject, fault_at,
+            ltotals, failed, aborted;
+        HostBuf h_count, h_ferr, h_err, h_cls, h_ver, h_subject, h_failed, h_aborted;
+        Event ev[2];
+    } rs;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     struct Skip {
@@ -997,6 +1017,28 @@ static int frame_entry_requests(regk_ctx *ctx, const FrameSrc &src, const regk_j
             : multi ? (has_data ? launch_jute_entry<true, true, false>(ctx, p, G.smem) : launch_jute_entry<true, false, false>(ctx, p, G.smem))
                     : (has_data ? launch_jute_entry<false, true, false>(ctx, p, G.smem) : launch_jute_entry<false, false, false>(ctx, p, G.smem));
     });
+}
+
+/* What a successful write framing framed, for regk_read_results: src's entries in `frames` frames of o->group (0 counts
+   as 1), its paths and data where src has them, what each entry stands for (`subject`, NULL = itself), and the
+   generation of the state src lives in. */
+static void record_framing(regk_ctx::ResDesc &d, const FrameSrc &src, const regk_jute_opts *o, uint32_t op, bool multi,
+    uint64_t frames, const unsigned long long *subject, uint64_t gen)
+{
+    d.valid = true;
+    d.f = ResFraming{};
+    d.f.xid_base = o->xid_base;
+    d.f.op = op;
+    d.f.group = o->group ? o->group : 1u;
+    d.f.multi = multi ? 1u : 0u;
+    d.f.frames = frames;
+    d.f.entries = src.n;
+    d.f.path_bytes = src.path_bytes;
+    d.f.path_off = src.path_off;
+    d.f.data_off = src.json_off;
+    d.subject = subject;
+    d.tol = op == REGK_ZK_DELETE ? -101 : 0;    /* NONODE: cleanupPreviousEntries ignores it (lib/register.js:88) */
+    d.gen = gen;
 }
 
 /* regk_parents.cuh on the path stream of the batch finished last (n >= 1 records), into the given buffers: enqueues
@@ -2444,6 +2486,8 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
         ctx->gd_gen = ctx->last.gen;
         ctx->gd_xid = o->xid_base;
         ctx->gd_n = ctx->last.n;
+    } else if (rc == REGK_OK) {
+        record_framing(ctx->rs.batch, src, o, o->op, o->group != 0, out->n, nullptr, ctx->last.gen);
     }
     return rc;
 }
@@ -2644,6 +2688,7 @@ int regk_mkdirp_dirs(regk_ctx *ctx, uint32_t flags, regk_dirs *out)
     cudaStream_t s = ctx->stream;
     const bool dev_out = flags & REGK_OUT_DEVICE;
     ctx->mk.valid = false;
+    ctx->mk.gen++;
     regk_ctx::Mkdirp &mk = ctx->mk;
     int rc;
     if ((rc = ensure_host(ctx, mk.h_count, 64)) || (rc = ensure_dev(ctx, mk.count, 64)))
@@ -2851,7 +2896,11 @@ int regk_mkdirp_requests(regk_ctx *ctx, int32_t xid_base, uint32_t zk_flags, uin
     FrameSrc src{nd, (const uint8_t *)ctx->mk.dbytes.p, (const unsigned long long *)ctx->mk.doff.p,
                  (const uint8_t *)ctx->mk.dbytes.p, (const unsigned long long *)ctx->mk.zero.p};
     src.who = "regk_mkdirp_requests";
-    return frame_requests(ctx, src, &o, ctx->mk.frames, out);
+    if ((rc = frame_requests(ctx, src, &o, ctx->mk.frames, out)))
+        return rc;
+    record_framing(ctx->rs.mkdirp, src, &o, REGK_ZK_CREATE, false, out->n, nullptr, ctx->mk.gen);
+    ctx->rs.mkdirp.tol = -110;                  /* NODEEXISTS: zkplus' mkdirp tolerates it */
+    return REGK_OK;
 }
 
 /* regk_reconcile (st == NULL) and regk_reconcile_owned: one implementation, the same four passes; `rep` / `n_rep` receive
@@ -2860,6 +2909,7 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
     const uint64_t **rep, uint64_t *n_rep, const char *who)
 {
     ctx->rc.valid = false;
+    ctx->rc.gen++;
     if (in->flags & REGK_DECODE_LAST)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams", who);
     if (ctx->pending)
@@ -3191,11 +3241,20 @@ int regk_reconcile_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames 
                  data ? (const uint8_t *)rb.gather[g + 1].bytes.p : nullptr,
                  data ? (const unsigned long long *)rb.gather[g + 1].off.p : nullptr};
     src.who = "regk_reconcile_requests";
-    if (!replace && !observed)
-        return frame_requests(ctx, src, o, rb.frames, out);
-    const int v = l == RC_LUPDATE ? RC_VUPDATE : l == RC_LREPLACE ? RC_VREPLACE : RC_VDELETE;
-    const int32_t *ver = observed ? (const int32_t *)rb.ver[v].p : nullptr;
-    return frame_entry_requests(ctx, src, o, ver, replace, rb.frames, out);
+    int rc;
+    if (!replace && !observed) {
+        rc = frame_requests(ctx, src, o, rb.frames, out);
+    } else {
+        const int v = l == RC_LUPDATE ? RC_VUPDATE : l == RC_LREPLACE ? RC_VREPLACE : RC_VDELETE;
+        const int32_t *ver = observed ? (const int32_t *)rb.ver[v].p : nullptr;
+        rc = frame_entry_requests(ctx, src, o, ver, replace, rb.frames, out);
+    }
+    if (rc == REGK_OK) {
+        const int q = o->op == REGK_ZK_CREATE ? 0 : o->op == REGK_ZK_DELETE ? 1 : o->op == REGK_ZK_SETDATA ? 2 : 3;
+        record_framing(ctx->rs.rec[q], src, o, replace ? RS_REPLACE : o->op, replace || o->group != 0, out->n,
+            (const unsigned long long *)rb.list[l].p, rb.gen);
+    }
+    return rc;
 }
 
 static const char *reply_reason(uint32_t code)
@@ -3600,7 +3659,11 @@ int regk_children_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *
         CK(cudaSetDevice(ctx->device));
         FrameSrc src{ch.n_stale, (const uint8_t *)ch.sbytes.p, (const unsigned long long *)ch.soff.p, nullptr, nullptr};
         src.who = "regk_children_requests";
-        return frame_requests(ctx, src, o, ch.frames[1], out);
+        const int rc = frame_requests(ctx, src, o, ch.frames[1], out);
+        if (rc == REGK_OK)
+            record_framing(ctx->rs.stale, src, o, REGK_ZK_DELETE, o->group != 0, out->n, (const unsigned long long *)ch.stale.p,
+                ch.read_gen);
+        return rc;
     }
     if (o->op != REGK_ZK_GETCHILDREN)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_children_requests: op %u is not getChildren (8) or delete (2)", o->op);
@@ -3734,6 +3797,7 @@ int regk_read_children(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     ch.read = false;
+    ch.read_gen++;
     int rc;
     for (Event &ev : ch.ev)
         if ((rc = ensure_event(ctx, ev)))
@@ -4084,6 +4148,279 @@ int regk_read_children(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64
     out->listing.path_off = (const uint64_t *)ch.lst_off.p;
     out->listing.json_bytes = (const uint8_t *)ch.lst_bytes.p;
     out->listing.json_off = (const uint64_t *)ch.lst_zero.p;
+    out->kernel_ms = ms;
+    return REGK_OK;
+}
+
+static const char *results_reason(uint32_t code)
+{
+    switch (code) {
+    case RS_TRUNC: return "the stream ends inside the frame";
+    case RS_BAD_LEN: return "a frame length below 16 (no room for a ReplyHeader)";
+    case RS_NEG_XID: return "a negative xid other than -1 (notification) or -2 (ping)";
+    case RS_XID_RANGE: return "an xid outside the framed requests";
+    case RS_ERR_BODY: return "an error reply with a body";
+    case RS_SUCC_LEN: return "a success length that fits neither outcome of the frame";
+    case RS_ORDER: return "a reply out of order, or for a frame that already has one";
+    case RS_OP_TYPE: return "a MultiHeader of the wrong type, done flag or err";
+    case RS_PATH_ECHO: return "a create path echo that differs from the framed path";
+    case RS_STAT_LEN: return "Stat.dataLength differs from the framed data's length";
+    case RS_ERR_RESULT: return "an ErrorResult whose two codes differ";
+    case RS_ERR_SEQ: return "ErrorResults out of the 0 / failing code / -2 order";
+    case RS_CLOSE: return "the multi's closing MultiHeader{-1, true, -1} is missing";
+    case RS_NO_FAILURE: return "a rolled-back multi with no nonzero ErrorResult";
+    default: return "internal error";
+    }
+}
+
+int regk_read_results(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, const regk_results_opts *o,
+    regk_results *out)
+{
+    const char *who = "regk_read_results";
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Results &rs = ctx->rs;
+    const regk_ctx::ResDesc *dsc = nullptr;
+    uint64_t gen = 0;
+    const char *changed = "";
+    switch (o->source) {
+    case REGK_RES_BATCH:
+        dsc = &rs.batch, gen = ctx->last.gen, changed = "a batch finished";
+        break;
+    case REGK_RES_MKDIRP:
+        dsc = &rs.mkdirp, gen = ctx->mk.gen, changed = "regk_mkdirp_dirs ran";
+        break;
+    case REGK_RES_RECONCILE: {
+        const int q = o->op == REGK_ZK_CREATE ? 0 : o->op == REGK_ZK_DELETE ? 1 : o->op == REGK_ZK_SETDATA ? 2
+                    : o->op == REGK_ZK_REPLACE ? 3 : -1;
+        if (q < 0)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: op %u is not create (1), delete (2), setData (5) or "
+                                                   "replace (256)", o->op);
+        dsc = &rs.rec[q], gen = ctx->rc.gen, changed = "a reconcile ran";
+        break;
+    }
+    case REGK_RES_STALE:
+        dsc = &rs.stale, gen = ctx->ch.read_gen, changed = "regk_read_children ran";
+        break;
+    default:
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: source %u is not REGK_RES_BATCH (1), _MKDIRP (2), "
+                                               "_RECONCILE (3) or _STALE (4)", o->source);
+    }
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_results: batches are still in flight; finish them first");
+    if (!dsc->valid)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_results: no write framing of source %u on this context", o->source);
+    if (dsc->gen != gen)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_results: %s after the framing; its paths are gone, frame the writes again",
+            changed);
+    if (!bytes && len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: NULL stream of %llu bytes", (unsigned long long)len);
+    if (start > len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: start %llu is past the stream's %llu bytes",
+            (unsigned long long)start, (unsigned long long)len);
+    const bool in_dev = o->flags & REGK_IN_DEVICE, dev_out = o->flags & REGK_OUT_DEVICE;
+    if (in_dev && ((uintptr_t)bytes & 15u))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: misaligned device stream (16-byte alignment needed)");
+    const ResFraming &f = dsc->f;
+    const uint64_t F = f.frames, n = f.entries;
+    const int32_t xb = f.xid_base;
+    for (int32_t reserved : {-1, -2})
+        if ((uint64_t)((uint32_t)reserved - (uint32_t)xb) < F)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: the framed xids [%d, %d + %llu) cover %d, which ZooKeeper "
+                                                   "uses for %s", xb, xb, (unsigned long long)F, reserved,
+                        reserved == -1 ? "watch notifications" : "pings");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    for (Event &ev : rs.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
+    const uint8_t *ds = bytes;
+    if (!in_dev && len) {
+        if ((rc = stage_in(ctx, rs.stream, bytes, len, s)))
+            return rc;
+        ds = (const uint8_t *)rs.stream.p;
+    }
+    const uint64_t nblk = (len + 15) / 16, tiles_s = (nblk + RP_TILE - 1) / RP_TILE;
+    const uint64_t tiles_e = (n + RP_TILE - 1) / RP_TILE;
+    const size_t totals_bytes = align16(tiles_s * 4) + (tiles_s / SUPER + 1) * 8;
+    const size_t tt = align16(tiles_e * 4), st = (tiles_e / SUPER + 1) * 8, ltotals_bytes = 2 * tt + 2 * st;
+    if ((rc = ensure_dev(ctx, rs.word, nblk * 4 + 16)) || (rc = ensure_dev(ctx, rs.totals, totals_bytes)) ||
+        (rc = ensure_dev(ctx, rs.tile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, rs.fpos, F * 8 + 16)) ||
+        (rc = ensure_dev(ctx, rs.ferr, F * 4 + 16)) || (rc = ensure_dev(ctx, rs.err, n * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rs.cls, n + 16)) || (rc = ensure_dev(ctx, rs.ver, n * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rs.subject, n * 8 + 16)) || (rc = ensure_dev(ctx, rs.fault_at, n * 8 + 16)) ||
+        (rc = ensure_dev(ctx, rs.failed, n * 8 + 16)) || (rc = ensure_dev(ctx, rs.aborted, n * 8 + 16)) ||
+        (rc = ensure_dev(ctx, rs.ltotals, ltotals_bytes + 16)) || (rc = ensure_host(ctx, rs.h_count, RS_NCOUNTERS * 8)) ||
+        (rc = ensure_dev(ctx, rs.count, RS_NCOUNTERS * 8)))
+        return rc;
+    ResParams rp{};
+    RepParams &p = rp.r;
+    p.s = ds;
+    p.len = len;
+    p.xid_base = xb;
+    p.n = F;
+    p.word = (uint32_t *)rs.word.p;
+    p.tile_total = (uint32_t *)rs.totals.p;
+    p.super_total = (unsigned long long *)((uint8_t *)rs.totals.p + align16(tiles_s * 4));
+    p.tile_base = (unsigned long long *)rs.tile_base.p;
+    p.counters = (unsigned long long *)rs.count.p;
+    rp.f = f;
+    rp.start = start;
+    rp.tol = dsc->tol;
+    rp.fpos = (unsigned long long *)rs.fpos.p;
+    rp.ferr = (int32_t *)rs.ferr.p;
+    rp.subject_in = dsc->subject;
+    rp.err = (int32_t *)rs.err.p;
+    rp.cls = (uint8_t *)rs.cls.p;
+    rp.ver = (int32_t *)rs.ver.p;
+    rp.subject = (unsigned long long *)rs.subject.p;
+    rp.fault_at = (unsigned long long *)rs.fault_at.p;
+    uint8_t *lt = (uint8_t *)rs.ltotals.p;
+    rp.tile_a = (uint32_t *)lt;
+    rp.tile_b = (uint32_t *)(lt + tt);
+    rp.super_a = (unsigned long long *)(lt + 2 * tt);
+    rp.super_b = (unsigned long long *)(lt + 2 * tt + st);
+    rp.failed = (unsigned long long *)rs.failed.p;
+    rp.aborted = (unsigned long long *)rs.aborted.p;
+    unsigned long long *hc = (unsigned long long *)rs.h_count.p;
+    CK(cudaMemsetAsync(p.counters, 0, RS_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(p.counters + RQ_ERR, 0xFF, 8, s));
+    CK(cudaMemsetAsync(p.counters + RS_ENT_ERR, 0xFF, 8, s));
+    CK(cudaMemsetAsync(p.tile_total, 0, totals_bytes, s));
+    CK(cudaEventRecord(rs.ev[0], s));
+    uint32_t launches = 0;
+    /* 1. the frame chain from `start` and the replies of the F frames */
+    RepParams pf = p;
+    if (F && len) {
+        regk_results_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(rp);
+        CK(cudaGetLastError());
+        launches++;
+        uint32_t *J = nullptr;
+        if ((rc = chain_pass(ctx, &pf, tiles_s, ~0ull, rs.cand, rs.mark, rs.jump, [&](const RepParams &q) {
+                regk_children_seed_kernel<<<1, 256, 0, s>>>(q, nullptr, nullptr, 1, start);
+            }, &J, &launches, who)))
+            return rc;
+        if (pf.C) {
+            const uint64_t tiles_c = (pf.C + RP_TILE - 1) / RP_TILE;
+            const size_t t2 = align16(tiles_c * 4) + (tiles_c / SUPER + 1) * 8;
+            if ((rc = ensure_dev(ctx, rs.totals2, t2)))
+                return rc;
+            rp.r = pf;
+            rp.r.tile_total = (uint32_t *)rs.totals2.p;
+            rp.r.super_total = (unsigned long long *)((uint8_t *)rs.totals2.p + align16(tiles_c * 4));
+            CK(cudaMemsetAsync(rs.totals2.p, 0, t2, s));
+            regk_replies_chain_count_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(rp.r);
+            regk_results_chain_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(rp);
+            CK(cudaGetLastError());
+            launches += 3;
+        }
+    }
+    CK(cudaMemcpyAsync(hc, p.counters, RS_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    const uint64_t frame_err_k = hc[RQ_ERR] != ~0ull ? hc[RQ_ERR] >> 8 : F;
+    const uint64_t f_eff = std::min<uint64_t>(std::min<uint64_t>(frame_err_k, hc[RQ_NREP]), F);
+    const uint64_t n_skipped = hc[RQ_SKIP], consumed = F ? hc[RQ_CONSUMED] : start;
+    /* 2. every entry of the frames before the first frame fault, and the FAILED / ABORTED lists */
+    rp.n_eff = std::min<uint64_t>(f_eff * f.group, n);
+    if (rp.n_eff) {
+        const unsigned te = (unsigned)((rp.n_eff + RP_TILE - 1) / RP_TILE);
+        CK(cudaMemsetAsync(lt, 0, ltotals_bytes, s));
+        regk_results_entry_kernel<<<te, RP_TILE, 0, s>>>(rp);
+        regk_results_list_kernel<<<te, RP_TILE, 0, s>>>(rp);
+        CK(cudaGetLastError());
+        launches += 2;
+        CK(cudaMemcpyAsync(hc, p.counters, RS_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+    }
+    /* refusals: the first fault a front-to-back reader meets - an entry fault of a frame before any frame fault */
+    if (hc[RS_ENT_ERR] != ~0ull) {
+        const uint64_t e = hc[RS_ENT_ERR] >> 8, k = e / f.group;
+        const uint32_t code = (uint32_t)(hc[RS_ENT_ERR] & 0xFF);
+        unsigned long long at[2] = {0, 0};
+        CK(cudaMemcpyAsync(&at[0], rp.fault_at + e, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&at[1], rp.fpos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: byte %llu: %s (entry %llu of the reply frame at byte %llu); "
+                                               "expected the reply to frame %llu (xid %d)", at[0], results_reason(code),
+                    (unsigned long long)e, at[1], (unsigned long long)k, (int32_t)((uint32_t)xb + (uint32_t)k));
+    }
+    if (hc[RQ_ERR] != ~0ull) {
+        const uint64_t k = hc[RQ_ERR] >> 8;
+        const uint32_t code = (uint32_t)(hc[RQ_ERR] & 0xFF);
+        unsigned long long pos = 0;
+        CK(cudaMemcpyAsync(&pos, rp.fpos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: byte %llu: %s; expected the reply to frame %llu (xid %d)",
+            pos, results_reason(code), (unsigned long long)k, (int32_t)((uint32_t)xb + (uint32_t)k));
+    }
+    if (hc[RQ_NREP] < F) {
+        /* the chain stops before the last reply: the plausibility test where it stops names the reason */
+        uint64_t stop = start;
+        if (pf.C) {
+            regk_replies_stop_kernel<<<(unsigned)((pf.C + 255) / 256), 256, 0, s>>>(pf);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(hc + RQ_STOP, p.counters + RQ_STOP, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            stop = std::max<uint64_t>(stop, hc[RQ_STOP]);
+        }
+        const uint64_t done = hc[RQ_NREP];
+        uint8_t head[20] = {0};
+        const uint64_t avail = len - stop, take = std::min<uint64_t>(avail, sizeof head);
+        if (take) {
+            CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
+            regk_results_head_kernel<<<1, 1, 0, s>>>(rp, stop);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(hc + RQ_M, p.counters + RQ_M, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+        }
+        const int32_t want = (int32_t)((uint32_t)xb + (uint32_t)done);
+        const bool trunc = avail < 4 || ((int32_t)be32_at(head) >= 16 && (uint64_t)(int32_t)be32_at(head) + 4u > avail);
+        if (trunc)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: byte %llu: the stream ends before the reply to frame %llu "
+                                                   "(xid %d) is complete; %llu of %llu replies complete",
+                        (unsigned long long)stop, (unsigned long long)done, want, (unsigned long long)done, (unsigned long long)F);
+        const uint32_t code = (uint32_t)hc[RQ_M];
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_results: byte %llu: %s (len %d, xid %d); expected the reply to frame "
+                                               "%llu (xid %d)", (unsigned long long)stop, code ? results_reason(code) : "internal error",
+                    (int32_t)be32_at(head), take >= 8 ? (int32_t)be32_at(head + 4) : 0, (unsigned long long)done, want);
+    }
+    CK(cudaEventRecord(rs.ev[1], s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, rs.ev[0], rs.ev[1]);
+    const uint64_t n_failed = hc[RS_NFAILED], n_aborted = hc[RS_NABORTED];
+    const void *src[7] = {rs.ferr.p, rs.err.p, rs.cls.p, rs.ver.p, rs.subject.p, rs.failed.p, rs.aborted.p};
+    if (!dev_out) {
+        HostBuf *hb[7] = {&rs.h_ferr, &rs.h_err, &rs.h_cls, &rs.h_ver, &rs.h_subject, &rs.h_failed, &rs.h_aborted};
+        const size_t sz[7] = {F * 4, n * 4, n, n * 4, n * 8, n_failed * 8, n_aborted * 8};
+        for (int k = 0; k < 7; k++) {
+            if ((rc = to_host(ctx, *hb[k], src[k], sz[k], s)))
+                return rc;
+            src[k] = hb[k]->p;
+        }
+        CK(cudaStreamSynchronize(s));
+    }
+    out->n_frames = F;
+    out->n_entries = n;
+    out->n_done = hc[RS_NDONE];
+    out->n_failed = n_failed;
+    out->n_aborted = n_aborted;
+    out->n_skipped = n_skipped;
+    out->consumed = consumed;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->frame_err = (const int32_t *)src[0];
+    out->err = (const int32_t *)src[1];
+    out->cls = (const uint8_t *)src[2];
+    out->version = (const int32_t *)src[3];
+    out->subject = (const uint64_t *)src[4];
+    out->failed = (const uint64_t *)src[5];
+    out->aborted = (const uint64_t *)src[6];
     out->kernel_ms = ms;
     return REGK_OK;
 }
