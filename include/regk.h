@@ -381,9 +381,19 @@ int         regk_jute_frames(regk_ctx *ctx, uint32_t flags, int32_t xid_base, ui
  *                    replies regk_read_replies turns into a snapshot.  Frame i = len | xid_base + i (wrapping) | 4 | path
  *                    length | path | 0, 17 + P_i bytes.  Paths only; group != 0 is REGK_ERR_INVALID_ARG (a multi holds
  *                    no reads).  A successful call records the batch, xid_base and n for regk_read_replies.
+ *   REGK_ZK_EXISTS   ExistsRequest{path, watch = false}: the reference's own heartbeat request, zk.stat per node
+ *                    (lib/zk.js:30-35), whose replies regk_read_stats reads.  The getData layout with op word 3: frame i =
+ *                    len | xid_base + i (wrapping) | 3 | path length | path | 0, 17 + P_i bytes; group != 0 is
+ *                    REGK_ERR_INVALID_ARG.  The frames carry paths only, but the batch must have its payload stream too
+ *                    (REGK_ERR_STATE otherwise): regk_reconcile_stats classes the replies against the payload lengths.
+ *                    A successful call records the batch, xid_base and n in fields of its own, so an exists framing
+ *                    and a getData framing of one batch can both be outstanding (the frames share one buffer: copy or
+ *                    send the first before framing the second).  Like getData it leaves regk_read_results' record of
+ *                    the last write framing in force.
  */
 #define REGK_ZK_CREATE  1u
 #define REGK_ZK_DELETE  2u
+#define REGK_ZK_EXISTS  3u
 #define REGK_ZK_GETDATA 4u
 #define REGK_ZK_SETDATA 5u
 
@@ -850,6 +860,82 @@ typedef struct regk_results {
 
 int         regk_read_results(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start,
                               const regk_results_opts *opts, regk_results *out);
+
+/*
+ * ---- the heartbeat by stat: an exists per node, the replies read and the batch classed without any node data (the
+ * reference's heartbeat is zk.stat on every node, lib/zk.js:21-44: one ExistsRequest out and a 68-byte Stat back) ------
+ * regk_read_stats: bytes[start, len) = what the caller read off the session after sending the frames of the last
+ * REGK_ZK_EXISTS regk_jute_requests call, from the first reply's length word on; host memory, or device memory with
+ * REGK_IN_DEVICE (bytes 16-byte aligned; start need not be, so the replies can follow other sections in one stream).
+ * Positions, consumed included, count from bytes.  Frame = int len | ReplyHeader{int xid; long zxid; int err} | body, big
+ * endian; body = ExistsResponse{Stat (68 bytes)} iff err == 0, so len == 84 for a success and 16 otherwise.  Stat =
+ * czxid mzxid ctime mtime (8 each) | version cversion aversion (4 each) | ephemeralOwner (8) | dataLength numChildren (4
+ * each) | pzxid (8).  The k-th frame that is not a watch notification (xid -1) or a ping (xid -2) must carry xid_base + k
+ * (wrapping) and answers record k; notifications and pings met before the n-th reply are skipped and counted, and the
+ * stream may go on past it.  n_found + n_missing + n_error == n; the registry is healthy iff n_missing + n_error == 0,
+ * which is all the reference's heartbeat asks.
+ * err[k] = ReplyHeader.err; version, ephemeral_owner, data_length and mzxid are record k's Stat fields, 0 where err[k] !=
+ * 0.  The five arrays are pinned host arrays, or device arrays with REGK_OUT_DEVICE; the library keeps its device copies
+ * for regk_reconcile_stats either way.  All stay valid until the next regk_read_stats call; a later batch does not free
+ * them, but regk_reconcile_stats then refuses them.
+ * REGK_ERR_STATE: no REGK_ZK_EXISTS framing since the batch finished last, a batch finished since that framing, or a
+ * pending batch.  REGK_ERR_INVALID_ARG (the message names the byte position and the expected xid; it is the first fault
+ * a front-to-back reader meets): the stream ends before the n-th reply is complete (and says how many were), len < 16, a
+ * negative xid other than -1 / -2, an xid outside the framed range, a reply out of order or for a record that already
+ * has one, an error reply with a body, a success length other than 84, Stat.dataLength < 0; an xid range that covers -1
+ * or -2; start > len; NULL pointers; a misaligned device stream.
+ * PARITY UNPINNED: the layout is restated from zookeeper.jute and tested against an independent restatement.
+ */
+typedef struct regk_stats {
+    uint64_t n;                     /* requests: records of the framed batch */
+    uint64_t n_found, n_missing, n_error;   /* replies with err 0 / NONODE (-101) / any other err */
+    uint64_t n_skipped;             /* watch notifications and pings met before the n-th reply */
+    uint64_t consumed;              /* stream position of the end of the n-th reply */
+    uint32_t flags, launches;       /* REGK_OUT_DEVICE */
+    const int32_t *err;             /* [n] ReplyHeader.err of record k's reply */
+    const int32_t *version;         /* [n] Stat.version */
+    const int64_t *ephemeral_owner; /* [n] Stat.ephemeralOwner; 0 = persistent */
+    const int32_t *data_length;     /* [n] Stat.dataLength */
+    const int64_t *mzxid;           /* [n] Stat.mzxid: the zxid of the node's last write */
+    float kernel_ms;
+} regk_stats;
+
+int         regk_read_stats(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, uint32_t flags,
+                            regk_stats *out);
+
+/*
+ * regk_reconcile_stats: class the batch finished last from the stats of the last regk_read_stats call, and leave the
+ * context as regk_reconcile_owned leaves it: the lists, each update / replace entry's observed version and the gathered
+ * request streams, so regk_reconcile_requests (create / setData / replace, REGK_ZK_VERSION_OBSERVED, groups) and
+ * regk_read_results(REGK_RES_RECONCILE) follow unchanged.  Reply k answers record k, so there is no snapshot and no
+ * observed side: m == 0, n_delete == 0, obs_cls == NULL, and REGK_ZK_DELETE frames nothing (nodes the batch does not
+ * produce are regk_read_children's business).  want = session when zk_flags == 1 (EPHEMERAL), else 0.  Record i:
+ *   REGK_DELTA_DUP      an earlier record has the same path (compared byte for byte; the first occurrence decides)
+ *   REGK_DELTA_CREATE   its reply is NONODE
+ *   REGK_DELTA_REPLACE  found, and ephemeral_owner[i] != want; nothing else is looked at
+ *   REGK_DELTA_UPDATE   found, the owner is right, and data_length[i] differs from payload i's length - or known_mzxid
+ *                       is given and mzxid[i] != known_mzxid[i]
+ *   REGK_DELTA_SAME     otherwise
+ * match[i] = the first record with path i, or UINT64_MAX when that record's node is missing.
+ * n_same + n_create + n_update + n_dup + n_replace == n.
+ * WHAT A STAT CANNOT SEE: a node whose bytes changed to a payload of the same length (an address rewritten from 10.0.0.1
+ * to 10.0.0.2) is SAME unless known_mzxid is given.  known_mzxid[i] = the mzxid record i's node had when its bytes were
+ * last verified (a getData round whose regk_reconcile_owned said SAME, with the regk_read_stats of the same round sent
+ * first; INTEGRATION.md §3): any write since then moves mzxid and makes the record UPDATE.  NULL, or int64[n]: a host
+ * array, or a device array (8-byte aligned) with REGK_IN_DEVICE in flags.  flags: REGK_OUT_DEVICE as regk_reconcile.
+ * REGK_ERR_STATE: no regk_read_stats result, a batch finished since it, a pending batch; or a reply with an error other
+ * than NONODE - the message names the smallest such record and its code: a repair built over an unknown node state is
+ * never right.  REGK_ERR_INVALID_ARG: zk_flags other than 0 or 1, zk_flags == 1 with session == 0, a misaligned device
+ * known_mzxid, NULL pointers.  The delta's arrays are valid until the next reconcile call of any kind.
+ */
+typedef struct regk_stat_opts {
+    int64_t  session;               /* session id the repair will be sent on */
+    uint32_t zk_flags;              /* CreateMode of the batch's nodes: 1 = EPHEMERAL, 0 = persistent; nothing else */
+    uint32_t reserved;
+    const int64_t *known_mzxid;     /* [n] or NULL */
+} regk_stat_opts;
+
+int         regk_reconcile_stats(regk_ctx *ctx, const regk_stat_opts *opts, uint32_t flags, regk_delta_owned *out);
 
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);

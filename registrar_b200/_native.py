@@ -95,6 +95,7 @@ class CJuteOpts(C.Structure):        # regk_jute_opts
 
 
 ZK_CREATE, ZK_DELETE, ZK_SETDATA = 1, 2, 5
+ZK_EXISTS = 3                       # jute_requests: ExistsRequest{path, watch = false}; its replies go to read_stats()
 ZK_GETDATA = 4                      # jute_requests: GetDataRequest{path, watch = false}; its replies go to read_replies()
 ZK_GETCHILDREN = 8                  # children_requests: GetChildrenRequest{dir, watch = false}; replies go to read_children()
 ZK_REPLACE = 256                    # reconcile_requests after reconcile_owned: delete + create in one multi transaction
@@ -357,6 +358,36 @@ class Results:
         return self.subject[self.aborted.astype(np.int64)]
 
 
+class CStats(C.Structure):          # regk_stats
+    _fields_ = [("n", C.c_uint64), ("n_found", C.c_uint64), ("n_missing", C.c_uint64), ("n_error", C.c_uint64),
+                ("n_skipped", C.c_uint64), ("consumed", C.c_uint64), ("flags", C.c_uint32), ("launches", C.c_uint32),
+                ("err", C.c_void_p), ("version", C.c_void_p), ("ephemeral_owner", C.c_void_p),
+                ("data_length", C.c_void_p), ("mzxid", C.c_void_p), ("kernel_ms", C.c_float)]
+
+
+class CStatOpts(C.Structure):       # regk_stat_opts
+    _fields_ = [("session", C.c_int64), ("zk_flags", C.c_uint32), ("reserved", C.c_uint32), ("known_mzxid", C.c_void_p)]
+
+
+class Stats:
+    """What read_stats() made of the replies to the last exists framing: err[k] is the ReplyHeader.err of record k's reply
+    (0 found, -101 NONODE, other codes) and version / ephemeral_owner / data_length / mzxid its Stat fields (0 where
+    err[k] != 0), plus n_found / n_missing / n_error / n_skipped and `consumed` (stream position of the end of the n-th
+    reply).  The registry is healthy iff n_missing + n_error == 0.  Pass the object to Context.reconcile_stats(); the
+    library's device copies stay valid until the next read_stats() call on the context."""
+
+    def __init__(self, out):
+        n = int(out.n)
+        self.n, self.launches, self.kernel_ms = n, int(out.launches), float(out.kernel_ms)
+        self.n_found, self.n_missing, self.n_error = int(out.n_found), int(out.n_missing), int(out.n_error)
+        self.n_skipped, self.consumed = int(out.n_skipped), int(out.consumed)
+        self.err = _as_np(out.err, n, np.int32).copy()
+        self.version = _as_np(out.version, n, np.int32).copy()
+        self.ephemeral_owner = _as_np(out.ephemeral_owner, n, np.int64).copy()
+        self.data_length = _as_np(out.data_length, n, np.int32).copy()
+        self.mzxid = _as_np(out.mzxid, n, np.int64).copy()
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -369,7 +400,8 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_gather_push", "regk_parent_dirs", "regk_job_bind", "regk_service_records",
            "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records", "regk_mkdirp_dirs",
            "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned",
-           "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results"]
+           "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results", "regk_read_stats",
+           "regk_reconcile_stats"]
 
 _lib = None
 
@@ -430,6 +462,8 @@ def load_library():
     lib.regk_children_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     lib.regk_read_children.argtypes = [vp, vp, u64, u64, u32, C.POINTER(CChildren)]
     lib.regk_read_results.argtypes = [vp, vp, u64, u64, C.POINTER(CResultsOpts), C.POINTER(CResults)]
+    lib.regk_read_stats.argtypes = [vp, vp, u64, u64, u32, C.POINTER(CStats)]
+    lib.regk_reconcile_stats.argtypes = [vp, C.POINTER(CStatOpts), u32, C.POINTER(CDeltaOwned)]
     _lib = lib
     return lib
 
@@ -896,6 +930,58 @@ class Context:
         del keep
         self._check(rc)
         return out if device else Results(out)
+
+    # -- the heartbeat by stat: the replies to the exists frames, and the batch classed from them --
+    def read_stats(self, stream, start: int = 0, device: bool = False):
+        """regk_read_stats: `stream` (a NumPy uint8 array, or a contiguous CUDA uint8 tensor) holds, from byte `start` on,
+        the bytes read off the session after sending the frames of the last jute_requests(op=ZK_EXISTS) call.  Returns a
+        Stats (input of reconcile_stats()), or the raw CStats (its arrays on the device) with device=True."""
+        flags = FLAG_OUT_DEVICE if device else 0
+        if hasattr(stream, "data_ptr"):
+            import torch
+            if not stream.is_cuda or stream.dtype != torch.uint8 or not stream.is_contiguous():
+                raise ValueError("a device stream is a contiguous CUDA uint8 tensor")
+            keep, ptr, n = stream, stream.data_ptr() or None, stream.numel()
+            flags |= FLAG_IN_DEVICE
+        else:
+            keep = np.ascontiguousarray(stream)
+            if keep.dtype != np.uint8 or keep.ndim != 1:
+                raise ValueError("a host stream is a one-dimensional uint8 array")
+            ptr, n = _np_ptr(keep), keep.size
+        out = CStats()
+        rc = self._lib.regk_read_stats(self._h, ptr, n, int(start), flags, C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else Stats(out)
+
+    def reconcile_stats(self, stats, session: int, zk_flags: int = 1, known_mzxid=None, device: bool = False):
+        """regk_reconcile_stats: class the batch finished last from `stats`, the result of the last read_stats() on this
+        context (the library classes from its own device copies of it), with no node data: CREATE for a missing node,
+        REPLACE for a wrong owner, UPDATE for another data length - or, with known_mzxid (int64[n], a NumPy array or a
+        CUDA tensor: each node's mzxid when its bytes were last verified), for any write since.  A same-length change of
+        the bytes is SAME without known_mzxid.  Returns the Delta reconcile_owned() returns (m == 0, no deletes), or the
+        raw CDeltaOwned with device=True; reconcile_requests() and read_results() follow as after reconcile_owned()."""
+        if stats is None:
+            raise ValueError("reconcile_stats classes the result of read_stats()")
+        flags = FLAG_OUT_DEVICE if device else 0
+        keep, ptr = None, None
+        if known_mzxid is not None and hasattr(known_mzxid, "data_ptr"):
+            import torch
+            if not known_mzxid.is_cuda or known_mzxid.dtype != torch.int64 or not known_mzxid.is_contiguous():
+                raise ValueError("a device known_mzxid is a contiguous CUDA int64 tensor")
+            keep, ptr = known_mzxid, known_mzxid.data_ptr() or None
+            flags |= FLAG_IN_DEVICE
+        elif known_mzxid is not None:
+            keep = np.ascontiguousarray(known_mzxid, dtype=np.int64)
+            ptr = _np_ptr(keep)
+        if keep is not None and (keep.numel() if hasattr(keep, "numel") else keep.size) != int(stats.n):
+            raise ValueError("known_mzxid holds one mzxid per record of the batch")
+        o = CStatOpts(int(session), int(zk_flags), 0, ptr)
+        out = CDeltaOwned()
+        rc = self._lib.regk_reconcile_stats(self._h, C.byref(o), flags, C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else Delta(out.d, out.replace, out.n_replace)
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

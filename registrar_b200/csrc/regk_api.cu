@@ -35,6 +35,7 @@
 #include "regk_replies.cuh"
 #include "regk_children.cuh"
 #include "regk_results.cuh"
+#include "regk_stats.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -261,6 +262,18 @@ struct regk_ctx {
         HostBuf h_count, h_ferr, h_err, h_cls, h_ver, h_subject, h_failed, h_aborted;
         Event ev[2];
     } rs;
+    /* the last REGK_ZK_EXISTS framing (as gd_* above), and regk_read_stats (regk_stats.cuh): staged stream, candidates,
+       jump tables, the per-record arrays regk_reconcile_stats classes from, and the batch they answer */
+    bool ex_valid = false;
+    uint64_t ex_gen = 0, ex_n = 0;
+    int32_t ex_xid = 0;
+    struct Stats {
+        DevBuf stream, word, totals, tile_base, cand, mark, jump, totals2, count, fpos, err, ver, own, dlen, mzxid, known;
+        HostBuf h_count, h_err, h_ver, h_own, h_dlen, h_mzxid;
+        Event ev[2];
+        bool read = false;                      /* the arrays of the last regk_read_stats are in err .. mzxid */
+        uint64_t gen = 0, n = 0;                /* the batch generation and the records they answer */
+    } sq;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     struct Skip {
@@ -932,7 +945,7 @@ static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_op
     p.multi = multi ? 1u : 0u;
     /* what follows the data: create - acl vector [OPEN_ACL_UNSAFE] + flags; delete / setData - the expected version */
     uint8_t tail[48] = {0};
-    if (o->op == REGK_ZK_GETDATA || o->op == REGK_ZK_GETCHILDREN) {
+    if (o->op == REGK_ZK_GETDATA || o->op == REGK_ZK_GETCHILDREN || o->op == REGK_ZK_EXISTS) {
         p.tail_len = 1;                                 /* watch = false */
     } else if (o->op == REGK_ZK_CREATE) {
         static const uint8_t acl[27] = {0, 0, 0, 1, 0, 0, 0, 31, 0, 0, 0, 5, 'w', 'o', 'r', 'l', 'd', 0, 0, 0, 6, 'a', 'n', 'y', 'o', 'n', 'e'};
@@ -1154,7 +1167,7 @@ int regk_set_option(regk_ctx *ctx, const char *name, int64_t value)
     if (!ctx || !name)
         return REGK_ERR_INVALID_ARG;
     static const char *known[] = {"async", "force_generic", "dom_cap", "json_out_cap", "chunk_records", "time_every", "offsets32",
-                                  "mkdirp_tight_table", "reconcile_tight_table", nullptr};
+                                  "mkdirp_tight_table", "reconcile_tight_table", "stats_cand_shared", nullptr};
     for (const char **k = known; *k; k++)
         if (!strcmp(*k, name)) {
             ctx->opt[name] = value;
@@ -2463,21 +2476,23 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
     if (!ctx || !o || !out)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: NULL argument");
     memset(out, 0, sizeof *out);
-    const bool getdata = o->op == REGK_ZK_GETDATA;
-    if (o->op != REGK_ZK_CREATE && o->op != REGK_ZK_DELETE && o->op != REGK_ZK_SETDATA && !getdata)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: op %u is not create (1), delete (2), getData (4) or setData (5)",
-            o->op);
+    const bool getdata = o->op == REGK_ZK_GETDATA, exists = o->op == REGK_ZK_EXISTS;
+    if (o->op != REGK_ZK_CREATE && o->op != REGK_ZK_DELETE && o->op != REGK_ZK_SETDATA && !getdata && !exists)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: op %u is not create (1), delete (2), exists (3), getData (4) "
+                                               "or setData (5)", o->op);
     if (o->group > 65536)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: at most 65536 operations per multi transaction");
-    if (getdata && o->group != 0)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: getData requests cannot go in a multi transaction (group %u)",
-            o->group);
-    const bool has_data = o->op != REGK_ZK_DELETE && !getdata;
+    if ((getdata || exists) && o->group != 0)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: %s requests cannot go in a multi transaction (group %u)",
+            getdata ? "getData" : "exists", o->group);
+    const bool has_data = o->op != REGK_ZK_DELETE && !getdata && !exists;
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "regk_jute_requests: batches are still in flight; finish them first");
-    if (!ctx->last.path_off || (has_data && (!ctx->last.json_off || ctx->last.n != ctx->last.json_n)))
+    /* an exists frame carries no data, but its replies are classed against the payload lengths (regk_reconcile_stats) */
+    const bool need_json = has_data || exists;
+    if (!ctx->last.path_off || (need_json && (!ctx->last.json_off || ctx->last.n != ctx->last.json_n)))
         return fail(ctx, REGK_ERR_STATE, "regk_jute_requests: no finished batch with %s on this context",
-            has_data ? "both a path and a payload stream" : "a path stream");
+            need_json ? "both a path and a payload stream" : "a path stream");
     const FrameSrc src{ctx->last.n, ctx->last.path_bytes, ctx->last.path_off, has_data ? ctx->last.json_bytes : nullptr,
                        has_data ? ctx->last.json_off : nullptr};
     const int rc = frame_requests(ctx, src, o, ctx->frames, out);
@@ -2486,6 +2501,11 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
         ctx->gd_gen = ctx->last.gen;
         ctx->gd_xid = o->xid_base;
         ctx->gd_n = ctx->last.n;
+    } else if (rc == REGK_OK && exists) {
+        ctx->ex_valid = true;
+        ctx->ex_gen = ctx->last.gen;
+        ctx->ex_xid = o->xid_base;
+        ctx->ex_n = ctx->last.n;
     } else if (rc == REGK_OK) {
         record_framing(ctx->rs.batch, src, o, o->op, o->group != 0, out->n, nullptr, ctx->last.gen);
     }
@@ -2903,77 +2923,15 @@ int regk_mkdirp_requests(regk_ctx *ctx, int32_t xid_base, uint32_t zk_flags, uin
     return REGK_OK;
 }
 
-/* regk_reconcile (st == NULL) and regk_reconcile_owned: one implementation, the same four passes; `rep` / `n_rep` receive
-   the replace list of the owned call */
-static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_node_stat *st, uint32_t flags, regk_delta *out,
-    const uint64_t **rep, uint64_t *n_rep, const char *who)
+/* What every reconcile's passes share, from the batch finished last (n records), the node count m and whether versions
+   are carried: sizes and zeroes the tables, totals, counters and lists and fills *pp but for the observed side (o_*,
+   validate, want), which the caller sets first; records the start event. */
+static int reconcile_prepare(regk_ctx *ctx, uint64_t n, uint64_t m, bool owned, ReconcileParams *pp)
 {
-    ctx->rc.valid = false;
-    ctx->rc.gen++;
-    if (in->flags & REGK_DECODE_LAST)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams", who);
-    if (ctx->pending)
-        return fail(ctx, REGK_ERR_STATE, "%s: batches are still in flight; finish them first", who);
-    if (!ctx->last.path_off || !ctx->last.json_off || ctx->last.n != ctx->last.json_n)
-        return fail(ctx, REGK_ERR_STATE, "%s: no finished batch with both a path and a payload stream on this context "
-                                         "(an empty batch or a REGK_JOB_STEP result leaves none)", who);
-    const uint64_t n = ctx->last.n, m = in->n;
-    if (n >= 0xFFFFFFFFull || m >= 0xFFFFFFFFull)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: %llu records and %llu nodes: both must be below 2^32 - 1", who,
-            (unsigned long long)n, (unsigned long long)m);
-    const bool in_dev = in->flags & REGK_IN_DEVICE, dev_out = flags & REGK_OUT_DEVICE;
-    const uint8_t *pb = in->path_bytes, *jb = in->json_bytes;
-    const uint64_t *po = in->path_off, *jo = in->json_off;
-    uint64_t path_total = m ? in->path_total : 0, json_total = m ? in->json_total : 0;
-    if (m && (!po || !jo))
-        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: a snapshot of %llu nodes needs path and data offsets", who, (unsigned long long)m);
-    const int32_t *sver = st ? st->version : nullptr;
-    const int64_t *sown = st ? st->ephemeral_owner : nullptr;
-    if (st && m && (!sver || !sown))
-        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: a snapshot of %llu nodes needs a version and an owner per node", who,
-            (unsigned long long)m);
-    if (st && m && in_dev && (((uintptr_t)sver & 3u) || ((uintptr_t)sown & 7u)))
-        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device stats (version needs 4-byte, ephemeral_owner 8-byte alignment)", who);
-    CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     regk_ctx::Reconcile &rb = ctx->rc;
+    ReconcileParams &p = *pp;
     int rc;
-    if (m && !in_dev) {
-        path_total = po[m];
-        json_total = jo[m];
-        /* offsets become memory ranges in the kernels: monotone, each node below 4 GiB, ending at the totals */
-        for (uint64_t j = 0; j < m; j++)
-            if (po[j] > po[j + 1] || jo[j] > jo[j + 1] || po[j + 1] - po[j] > 0xFFFFFFFFull || jo[j + 1] - jo[j] > 0xFFFFFFFFull)
-                return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets are not monotone at node %llu", who,
-                    (unsigned long long)j);
-        if ((path_total && !pb) || (json_total && !jb))
-            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets without bytes", who);
-        const void *src[6] = {pb, po, jb, jo, sver, sown};
-        const size_t sz[6] = {(size_t)path_total, (size_t)(m + 1) * 8, (size_t)json_total, (size_t)(m + 1) * 8, (size_t)m * 4, (size_t)m * 8};
-        for (int k = 0; k < (st ? 6 : 4); k++)
-            if ((rc = stage_in(ctx, rb.in[k], src[k], sz[k], s)))
-                return rc;
-        pb = (const uint8_t *)rb.in[0].p;
-        po = (const uint64_t *)rb.in[1].p;
-        jb = (const uint8_t *)rb.in[2].p;
-        jo = (const uint64_t *)rb.in[3].p;
-        if (st) {
-            sver = (const int32_t *)rb.in[4].p;
-            sown = (const int64_t *)rb.in[5].p;
-        }
-    } else if (m) {
-        if ((path_total && !pb) || (json_total && !jb))
-            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets without bytes", who);
-        if (((uintptr_t)pb & 3u) || ((uintptr_t)jb & 3u) || ((uintptr_t)po & 7u) || ((uintptr_t)jo & 7u))
-            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device snapshot (bytes need 4-byte, offsets 8-byte alignment)", who);
-    }
-    /* an empty stream is never read; its kernels still get a valid pointer */
-    if ((rc = ensure_dev(ctx, rb.in[0], 16)) || (rc = ensure_dev(ctx, rb.in[2], 16)))
-        return rc;
-    if (!pb)
-        pb = (const uint8_t *)rb.in[0].p;
-    if (!jb)
-        jb = (const uint8_t *)rb.in[2].p;
     /* the batch's totals */
     unsigned long long tot[2] = {0, 0};
     CK(cudaMemcpyAsync(&tot[0], ctx->last.path_off + n, 8, cudaMemcpyDeviceToHost, s));
@@ -3005,13 +2963,12 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
     for (int k = 0; k < RC_NGATHERS; k++)
         if ((rc = ensure_dev(ctx, rb.len[k], (k == RC_GDELETE ? m : n) * 4 + 8)))
             return rc;
-    for (int k = 0; st && k < RC_NVER; k++)
+    for (int k = 0; owned && k < RC_NVER; k++)
         if ((rc = ensure_dev(ctx, rb.ver[k], (k == RC_VDELETE ? m : n) * 4 + 8)))
             return rc;
     for (Event &ev : rb.ev)
         if ((rc = ensure_event(ctx, ev)))
             return rc;
-    ReconcileParams p{};
     p.n = n;
     p.m = m;
     p.d_path = ctx->last.path_bytes;
@@ -3020,20 +2977,8 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
     p.d_json_off = ctx->last.json_off;
     p.d_path_limit = tot[0] + 16;                   /* every stream buffer of this library has >= 16 bytes of slack */
     p.d_json_limit = tot[1] + 16;
-    p.o_path = pb;
-    p.o_path_off = (const unsigned long long *)po;
-    p.o_json = jb;
-    p.o_json_off = (const unsigned long long *)jo;
-    p.o_path_total = path_total;                    /* a caller's device buffers end where they end */
-    p.o_json_total = json_total;
-    p.validate = in_dev ? 1u : 0u;
-    if (st) {
-        p.o_version = sver;
-        p.o_owner = (const long long *)sown;
-        p.want = st->zk_flags == 1u ? (long long)st->session : 0ll;
-        for (int k = 0; k < RC_NVER; k++)
-            p.ver[k] = (int32_t *)rb.ver[k].p;
-    }
+    for (int k = 0; owned && k < RC_NVER; k++)
+        p.ver[k] = (int32_t *)rb.ver[k].p;
     p.mask_o = (uint32_t)(so - 1);
     p.mask_d = (uint32_t)(sd - 1);
     p.t_obs = (uint32_t *)rb.t_obs.p;
@@ -3061,26 +3006,19 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
     CK(cudaMemsetAsync(p.counters, 0, counters_bytes, s));
     CK(cudaMemsetAsync(p.counters, 0xFF, 16, s));   /* no bad node, no duplicate node */
     CK(cudaEventRecord(rb.ev[0], s));
-    uint32_t launches = 0;
-    if (m) {
-        regk_reconcile_insert_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(p);
-        launches++;
-    }
-    regk_reconcile_desired_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p);
-    regk_reconcile_mark_kernel<<<(unsigned)(tiles_r + tiles_o), RC_TILE, 0, s>>>(p);
-    regk_reconcile_compact_kernel<<<(unsigned)(tiles_r + tiles_o), RC_TILE, 0, s>>>(p);
-    CK(cudaGetLastError());
-    launches += 3;
-    unsigned long long *hc = (unsigned long long *)rb.h_count.p;
-    CK(cudaMemcpyAsync(hc, p.counters, counters_bytes, cudaMemcpyDeviceToHost, s));
-    if ((rc = sync_or_fail(ctx, s, who)))
-        return rc;
-    if (hc[RC_C_BAD] != ~0ull)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets are not monotone or reach past the totals at node %llu", who,
-            hc[RC_C_BAD]);
-    if (hc[RC_C_DUPNODE] != ~0ull)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot node %llu has the path of an earlier node; a registry cannot "
-                                               "hold two nodes with one path", who, hc[RC_C_DUPNODE]);
+    return REGK_OK;
+}
+
+/* What follows a reconcile's compact pass, given its counters on the host (hc): the request sets gathered into the
+   library's own streams, the stop event, the outputs on the side `flags` asks for, the context's record of the result. */
+static int reconcile_finish(regk_ctx *ctx, const ReconcileParams &p, const unsigned long long *hc, bool owned, uint32_t zk_flags,
+    uint32_t flags, uint32_t launches, regk_delta *out, const uint64_t **rep, uint64_t *n_rep, const char *who)
+{
+    cudaStream_t s = ctx->stream;
+    regk_ctx::Reconcile &rb = ctx->rc;
+    const uint64_t n = p.n, m = p.m;
+    const bool dev_out = flags & REGK_OUT_DEVICE;
+    int rc;
     uint64_t cnt[RC_NLISTS];
     for (int l = 0; l < RC_NLISTS; l++)
         cnt[l] = hc[RC_C_COUNT + l];
@@ -3150,8 +3088,8 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
         CK(cudaStreamSynchronize(s));
     }
     rb.valid = true;
-    rb.owned = st != nullptr;
-    rb.zk_flags = st ? st->zk_flags : 0u;
+    rb.owned = owned;
+    rb.zk_flags = zk_flags;
     for (int l = 0; l < RC_NLISTS; l++)
         rb.n_list[l] = cnt[l];
     out->n = n;
@@ -3176,6 +3114,116 @@ static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_nod
         *n_rep = cnt[RC_LREPLACE];
     }
     return REGK_OK;
+}
+
+/* regk_reconcile (st == NULL) and regk_reconcile_owned: one implementation, the same four passes; `rep` / `n_rep` receive
+   the replace list of the owned call */
+static int reconcile_run(regk_ctx *ctx, const regk_decode_in *in, const regk_node_stat *st, uint32_t flags, regk_delta *out,
+    const uint64_t **rep, uint64_t *n_rep, const char *who)
+{
+    ctx->rc.valid = false;
+    ctx->rc.gen++;
+    if (in->flags & REGK_DECODE_LAST)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams", who);
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "%s: batches are still in flight; finish them first", who);
+    if (!ctx->last.path_off || !ctx->last.json_off || ctx->last.n != ctx->last.json_n)
+        return fail(ctx, REGK_ERR_STATE, "%s: no finished batch with both a path and a payload stream on this context "
+                                         "(an empty batch or a REGK_JOB_STEP result leaves none)", who);
+    const uint64_t n = ctx->last.n, m = in->n;
+    if (n >= 0xFFFFFFFFull || m >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: %llu records and %llu nodes: both must be below 2^32 - 1", who,
+            (unsigned long long)n, (unsigned long long)m);
+    const bool in_dev = in->flags & REGK_IN_DEVICE;
+    const uint8_t *pb = in->path_bytes, *jb = in->json_bytes;
+    const uint64_t *po = in->path_off, *jo = in->json_off;
+    uint64_t path_total = m ? in->path_total : 0, json_total = m ? in->json_total : 0;
+    if (m && (!po || !jo))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: a snapshot of %llu nodes needs path and data offsets", who, (unsigned long long)m);
+    const int32_t *sver = st ? st->version : nullptr;
+    const int64_t *sown = st ? st->ephemeral_owner : nullptr;
+    if (st && m && (!sver || !sown))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: a snapshot of %llu nodes needs a version and an owner per node", who,
+            (unsigned long long)m);
+    if (st && m && in_dev && (((uintptr_t)sver & 3u) || ((uintptr_t)sown & 7u)))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device stats (version needs 4-byte, ephemeral_owner 8-byte alignment)", who);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    regk_ctx::Reconcile &rb = ctx->rc;
+    int rc;
+    if (m && !in_dev) {
+        path_total = po[m];
+        json_total = jo[m];
+        /* offsets become memory ranges in the kernels: monotone, each node below 4 GiB, ending at the totals */
+        for (uint64_t j = 0; j < m; j++)
+            if (po[j] > po[j + 1] || jo[j] > jo[j + 1] || po[j + 1] - po[j] > 0xFFFFFFFFull || jo[j + 1] - jo[j] > 0xFFFFFFFFull)
+                return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets are not monotone at node %llu", who,
+                    (unsigned long long)j);
+        if ((path_total && !pb) || (json_total && !jb))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets without bytes", who);
+        const void *src[6] = {pb, po, jb, jo, sver, sown};
+        const size_t sz[6] = {(size_t)path_total, (size_t)(m + 1) * 8, (size_t)json_total, (size_t)(m + 1) * 8, (size_t)m * 4, (size_t)m * 8};
+        for (int k = 0; k < (st ? 6 : 4); k++)
+            if ((rc = stage_in(ctx, rb.in[k], src[k], sz[k], s)))
+                return rc;
+        pb = (const uint8_t *)rb.in[0].p;
+        po = (const uint64_t *)rb.in[1].p;
+        jb = (const uint8_t *)rb.in[2].p;
+        jo = (const uint64_t *)rb.in[3].p;
+        if (st) {
+            sver = (const int32_t *)rb.in[4].p;
+            sown = (const int64_t *)rb.in[5].p;
+        }
+    } else if (m) {
+        if ((path_total && !pb) || (json_total && !jb))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets without bytes", who);
+        if (((uintptr_t)pb & 3u) || ((uintptr_t)jb & 3u) || ((uintptr_t)po & 7u) || ((uintptr_t)jo & 7u))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device snapshot (bytes need 4-byte, offsets 8-byte alignment)", who);
+    }
+    /* an empty stream is never read; its kernels still get a valid pointer */
+    if ((rc = ensure_dev(ctx, rb.in[0], 16)) || (rc = ensure_dev(ctx, rb.in[2], 16)))
+        return rc;
+    if (!pb)
+        pb = (const uint8_t *)rb.in[0].p;
+    if (!jb)
+        jb = (const uint8_t *)rb.in[2].p;
+    ReconcileParams p{};
+    p.o_path = pb;
+    p.o_path_off = (const unsigned long long *)po;
+    p.o_json = jb;
+    p.o_json_off = (const unsigned long long *)jo;
+    p.o_path_total = path_total;                    /* a caller's device buffers end where they end */
+    p.o_json_total = json_total;
+    p.validate = in_dev ? 1u : 0u;
+    if (st) {
+        p.o_version = sver;
+        p.o_owner = (const long long *)sown;
+        p.want = st->zk_flags == 1u ? (long long)st->session : 0ll;
+    }
+    if ((rc = reconcile_prepare(ctx, n, m, st != nullptr, &p)))
+        return rc;
+    const uint64_t tiles_r = p.tiles_r, tiles_o = (m + RC_TILE - 1) / RC_TILE;
+    uint32_t launches = 0;
+    if (m) {
+        regk_reconcile_insert_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(p);
+        launches++;
+    }
+    regk_reconcile_desired_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p);
+    regk_reconcile_mark_kernel<<<(unsigned)(tiles_r + tiles_o), RC_TILE, 0, s>>>(p);
+    regk_reconcile_compact_kernel<<<(unsigned)(tiles_r + tiles_o), RC_TILE, 0, s>>>(p);
+    CK(cudaGetLastError());
+    launches += 3;
+    unsigned long long *hc = (unsigned long long *)rb.h_count.p;
+    CK(cudaMemcpyAsync(hc, p.counters, RC_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    if (hc[RC_C_BAD] != ~0ull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets are not monotone or reach past the totals at node %llu", who,
+            hc[RC_C_BAD]);
+    if (hc[RC_C_DUPNODE] != ~0ull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot node %llu has the path of an earlier node; a registry cannot "
+                                               "hold two nodes with one path", who, hc[RC_C_DUPNODE]);
+    return reconcile_finish(ctx, p, hc, st != nullptr, st ? st->zk_flags : 0u, flags, launches, out, rep, n_rep, who);
 }
 
 int regk_reconcile(regk_ctx *ctx, const regk_decode_in *in, uint32_t flags, regk_delta *out)
@@ -4423,6 +4471,268 @@ int regk_read_results(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_
     out->aborted = (const uint64_t *)src[6];
     out->kernel_ms = ms;
     return REGK_OK;
+}
+
+static const char *stats_reason(uint32_t code)
+{
+    switch (code) {
+    case ST_TRUNC: return "the stream ends inside the frame";
+    case ST_BAD_LEN: return "a frame length below 16 (no room for a ReplyHeader)";
+    case ST_NEG_XID: return "a negative xid other than -1 (notification) or -2 (ping)";
+    case ST_XID_RANGE: return "an xid outside the framed requests";
+    case ST_ERR_BODY: return "an error reply with a body";
+    case ST_SUCC_LEN: return "a success frame whose length is not 84 (ReplyHeader + Stat)";
+    case ST_ORDER: return "a reply out of order, or for a record that already has one";
+    case ST_NEG_DLEN: return "a negative Stat.dataLength";
+    default: return "internal error";
+    }
+}
+
+int regk_read_stats(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, uint32_t flags, regk_stats *out)
+{
+    const char *who = "regk_read_stats";
+    if (!ctx || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_stats: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Stats &sq = ctx->sq;
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_stats: batches are still in flight; finish them first");
+    if (!ctx->ex_valid)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_stats: no exists framing (regk_jute_requests with REGK_ZK_EXISTS) of the "
+                                         "batch finished last");
+    if (ctx->ex_gen != ctx->last.gen || !ctx->last.path_off)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_stats: a batch finished after the exists framing; frame its exists "
+                                         "requests first");
+    if (!bytes && len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_stats: NULL stream of %llu bytes", (unsigned long long)len);
+    if (start > len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_stats: start %llu is past the stream's %llu bytes",
+            (unsigned long long)start, (unsigned long long)len);
+    const bool in_dev = flags & REGK_IN_DEVICE, dev_out = flags & REGK_OUT_DEVICE;
+    if (in_dev && ((uintptr_t)bytes & 15u))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_stats: misaligned device stream (16-byte alignment needed)");
+    const uint64_t n = ctx->ex_n;
+    const int32_t xb = ctx->ex_xid;
+    for (int32_t reserved : {-1, -2})
+        if ((uint64_t)((uint32_t)reserved - (uint32_t)xb) < n)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_stats: the framed xids [%d, %d + %llu) cover %d, which ZooKeeper "
+                                                   "uses for %s", xb, xb, (unsigned long long)n, reserved,
+                        reserved == -1 ? "watch notifications" : "pings");
+    if (n >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_stats: %llu records: must be below 2^32 - 1", (unsigned long long)n);
+    sq.read = false;                                    /* from here on the arrays of the last read are overwritten */
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    for (Event &ev : sq.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
+    const uint8_t *ds = bytes;
+    if (!in_dev && len) {
+        if ((rc = stage_in(ctx, sq.stream, bytes, len, s)))
+            return rc;
+        ds = (const uint8_t *)sq.stream.p;
+    }
+    const uint64_t nblk = (len + 15) / 16, tiles_s = (nblk + RP_TILE - 1) / RP_TILE;
+    const size_t totals_bytes = align16(tiles_s * 4) + (tiles_s / SUPER + 1) * 8;
+    const size_t n8 = n * 8 + 16, n4 = n * 4 + 16;
+    if ((rc = ensure_dev(ctx, sq.word, nblk * 4 + 16)) || (rc = ensure_dev(ctx, sq.totals, totals_bytes)) ||
+        (rc = ensure_dev(ctx, sq.tile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, sq.fpos, n8)) ||
+        (rc = ensure_dev(ctx, sq.err, n4)) || (rc = ensure_dev(ctx, sq.ver, n4)) || (rc = ensure_dev(ctx, sq.own, n8)) ||
+        (rc = ensure_dev(ctx, sq.dlen, n4)) || (rc = ensure_dev(ctx, sq.mzxid, n8)) ||
+        (rc = ensure_dev(ctx, sq.count, RQ_NCOUNTERS * 8)) || (rc = ensure_host(ctx, sq.h_count, RQ_NCOUNTERS * 8)))
+        return rc;
+    StatParams sp{};
+    RepParams &p = sp.r;
+    p.s = ds;
+    p.len = len;
+    p.xid_base = xb;
+    p.n = n;
+    p.word = (uint32_t *)sq.word.p;
+    p.tile_total = (uint32_t *)sq.totals.p;
+    p.super_total = (unsigned long long *)((uint8_t *)sq.totals.p + align16(tiles_s * 4));
+    p.tile_base = (unsigned long long *)sq.tile_base.p;
+    p.err = (int32_t *)sq.err.p;
+    p.ver = (int32_t *)sq.ver.p;
+    p.own = (long long *)sq.own.p;
+    p.counters = (unsigned long long *)sq.count.p;
+    sp.start = start;
+    sp.fpos = (unsigned long long *)sq.fpos.p;
+    sp.dlen = (int32_t *)sq.dlen.p;
+    sp.mzxid = (long long *)sq.mzxid.p;
+    unsigned long long *hc = (unsigned long long *)sq.h_count.p;
+    CK(cudaMemsetAsync(p.counters, 0, RQ_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(p.counters + RQ_ERR, 0xFF, 8, s));
+    CK(cudaMemsetAsync(p.tile_total, 0, totals_bytes, s));
+    CK(cudaEventRecord(sq.ev[0], s));
+    uint32_t launches = 0;
+    /* 1. the frame chain from `start`, 2. the replies of the n records */
+    RepParams pf = p;
+    if (n && len) {
+        if (opt_get(ctx, "stats_cand_shared", 0))
+            regk_stats_cand_shared_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(sp);
+        else
+            regk_stats_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(sp);
+        CK(cudaGetLastError());
+        launches++;
+        uint32_t *J = nullptr;
+        if ((rc = chain_pass(ctx, &pf, tiles_s, ~0ull, sq.cand, sq.mark, sq.jump, [&](const RepParams &q) {
+                regk_children_seed_kernel<<<1, 256, 0, s>>>(q, nullptr, nullptr, 1, start);
+            }, &J, &launches, who)))
+            return rc;
+        if (pf.C) {
+            const uint64_t tiles_c = (pf.C + RP_TILE - 1) / RP_TILE;
+            const size_t t2 = align16(tiles_c * 4) + (tiles_c / SUPER + 1) * 8;
+            if ((rc = ensure_dev(ctx, sq.totals2, t2)))
+                return rc;
+            sp.r = pf;
+            sp.r.tile_total = (uint32_t *)sq.totals2.p;
+            sp.r.super_total = (unsigned long long *)((uint8_t *)sq.totals2.p + align16(tiles_c * 4));
+            CK(cudaMemsetAsync(sq.totals2.p, 0, t2, s));
+            regk_replies_chain_count_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(sp.r);
+            regk_stats_chain_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(sp);
+            CK(cudaGetLastError());
+            launches += 3;
+        }
+    }
+    CK(cudaEventRecord(sq.ev[1], s));
+    CK(cudaMemcpyAsync(hc, p.counters, RQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    /* refusals: a chain is read front to back, so the smallest failing reply is the first fault */
+    if (hc[RQ_ERR] != ~0ull) {
+        const uint64_t k = hc[RQ_ERR] >> 8;
+        const uint32_t code = (uint32_t)(hc[RQ_ERR] & 0xFF);
+        unsigned long long pos = 0;
+        CK(cudaMemcpyAsync(&pos, sp.fpos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_stats: byte %llu: %s; expected the reply to record %llu (xid %d)",
+            pos, stats_reason(code), (unsigned long long)k, (int32_t)((uint32_t)xb + (uint32_t)k));
+    }
+    if (hc[RQ_NREP] < n) {
+        /* the chain stops before the n-th reply: the plausibility test where it stops names the reason */
+        uint64_t stop = start;
+        if (pf.C) {
+            regk_replies_stop_kernel<<<(unsigned)((pf.C + 255) / 256), 256, 0, s>>>(pf);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(hc + RQ_STOP, p.counters + RQ_STOP, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            stop = std::max<uint64_t>(stop, hc[RQ_STOP]);
+        }
+        const uint64_t done = hc[RQ_NREP];
+        uint8_t head[20] = {0};
+        const uint64_t avail = len - stop, take = std::min<uint64_t>(avail, sizeof head);
+        if (take) {
+            CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+        }
+        StatHead h;
+        const uint32_t code = stat_head(head, avail, xb, n, &h);   /* reads at most 20 bytes, all of them in head */
+        const int32_t want = (int32_t)((uint32_t)xb + (uint32_t)done);
+        if (code == ST_TRUNC)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_stats: byte %llu: the stream ends before the reply to record %llu "
+                                                   "(xid %d) is complete; %llu of %llu replies complete", (unsigned long long)stop,
+                        (unsigned long long)done, want, (unsigned long long)done, (unsigned long long)n);
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_stats: byte %llu: %s (len %d, xid %d); expected the reply to record "
+                                               "%llu (xid %d)", (unsigned long long)stop, code ? stats_reason(code) : "internal error",
+                    h.len, h.xid, (unsigned long long)done, want);
+    }
+    float ms = 0;
+    cudaEventElapsedTime(&ms, sq.ev[0], sq.ev[1]);
+    const void *src[5] = {sq.err.p, sq.ver.p, sq.own.p, sq.dlen.p, sq.mzxid.p};
+    if (!dev_out) {
+        HostBuf *hb[5] = {&sq.h_err, &sq.h_ver, &sq.h_own, &sq.h_dlen, &sq.h_mzxid};
+        const size_t sz[5] = {n * 4, n * 4, n * 8, n * 4, n * 8};
+        for (int k = 0; k < 5; k++) {
+            if ((rc = to_host(ctx, *hb[k], src[k], sz[k], s)))
+                return rc;
+            src[k] = hb[k]->p;
+        }
+        CK(cudaStreamSynchronize(s));
+    }
+    sq.read = true;
+    sq.gen = ctx->last.gen;
+    sq.n = n;
+    out->n = n;
+    out->n_found = hc[RQ_FOUND];
+    out->n_missing = hc[RQ_MISSING];
+    out->n_error = hc[RQ_ERROR];
+    out->n_skipped = hc[RQ_SKIP];
+    out->consumed = n ? hc[RQ_CONSUMED] : start;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->err = (const int32_t *)src[0];
+    out->version = (const int32_t *)src[1];
+    out->ephemeral_owner = (const int64_t *)src[2];
+    out->data_length = (const int32_t *)src[3];
+    out->mzxid = (const int64_t *)src[4];
+    out->kernel_ms = ms;
+    return REGK_OK;
+}
+
+int regk_reconcile_stats(regk_ctx *ctx, const regk_stat_opts *o, uint32_t flags, regk_delta_owned *out)
+{
+    const char *who = "regk_reconcile_stats";
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_stats: NULL argument");
+    memset(out, 0, sizeof *out);
+    ctx->rc.valid = false;
+    ctx->rc.gen++;
+    if (o->zk_flags > 1u)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_stats: zk_flags %u is not 0 (persistent) or 1 (EPHEMERAL); a "
+                                               "sequential or container mode makes a path key meaningless", o->zk_flags);
+    if (o->zk_flags == 1u && o->session == 0)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_stats: EPHEMERAL nodes need the session id they are sent on");
+    const bool in_dev = flags & REGK_IN_DEVICE;
+    if (o->known_mzxid && in_dev && ((uintptr_t)o->known_mzxid & 7u))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_stats: misaligned device known_mzxid (8-byte alignment needed)");
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_reconcile_stats: batches are still in flight; finish them first");
+    regk_ctx::Stats &sq = ctx->sq;
+    if (!sq.read)
+        return fail(ctx, REGK_ERR_STATE, "regk_reconcile_stats: no stats on this context; call regk_read_stats first");
+    if (sq.gen != ctx->last.gen || !ctx->last.path_off || !ctx->last.json_off || ctx->last.n != sq.n)
+        return fail(ctx, REGK_ERR_STATE, "regk_reconcile_stats: a batch finished after regk_read_stats; its stats answer "
+                                         "another batch's records");
+    const uint64_t n = sq.n;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    StatClassParams sp{};
+    sp.err = (const int32_t *)sq.err.p;
+    sp.own = (const long long *)sq.own.p;
+    sp.dlen = (const int32_t *)sq.dlen.p;
+    sp.mzxid = (const long long *)sq.mzxid.p;
+    sp.known_mzxid = (const long long *)o->known_mzxid;
+    if (o->known_mzxid && !in_dev) {
+        if ((rc = stage_in(ctx, sq.known, o->known_mzxid, n * 8, s)))
+            return rc;
+        sp.known_mzxid = (const long long *)sq.known.p;
+    }
+    /* no observed side: m = 0; the compact pass takes each update / replace entry's version from the stats, through
+       match[i] = the record itself */
+    ReconcileParams &p = sp.rc;
+    p.o_version = (const int32_t *)sq.ver.p;
+    p.want = o->zk_flags == 1u ? (long long)o->session : 0ll;
+    if ((rc = reconcile_prepare(ctx, n, 0, true, &p)))
+        return rc;
+    regk_stats_class_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(sp);
+    regk_stats_mark_kernel<<<p.tiles_r, RC_TILE, 0, s>>>(sp);
+    regk_reconcile_compact_kernel<<<p.tiles_r, RC_TILE, 0, s>>>(p);
+    CK(cudaGetLastError());
+    unsigned long long *hc = (unsigned long long *)ctx->rc.h_count.p;
+    CK(cudaMemcpyAsync(hc, p.counters, RC_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    if (hc[RC_C_BAD] != ~0ull) {
+        int32_t e = 0;
+        CK(cudaMemcpy(&e, sp.err + hc[RC_C_BAD], 4, cudaMemcpyDeviceToHost));
+        return fail(ctx, REGK_ERR_STATE, "regk_reconcile_stats: record %llu's reply carries error %d: the state of its node is "
+                                         "unknown, and no repair over it is right", hc[RC_C_BAD], e);
+    }
+    rc = reconcile_finish(ctx, p, hc, true, o->zk_flags, flags, 3, &out->d, &out->replace, &out->n_replace, who);
+    out->d.obs_cls = nullptr;
+    return rc;
 }
 
 int regk_release(regk_ctx *ctx, regk_result *res)
