@@ -597,6 +597,12 @@ int         regk_reconcile(regk_ctx *ctx, const regk_decode_in *snapshot, uint32
  */
 #define REGK_ZK_REPLACE          256u       /* regk_jute_opts.op: not a ZooKeeper OpCode */
 #define REGK_ZK_VERSION_OBSERVED (1u << 9)  /* regk_jute_opts.flags */
+/* regk_jute_opts.flags: the read framings (regk_jute_requests with REGK_ZK_EXISTS / REGK_ZK_GETDATA,
+   regk_children_requests with REGK_ZK_GETCHILDREN) write the request's trailing watch byte as 1 instead of 0, so the
+   server arms a one-shot watch on each node or directory and later pushes a WatcherEvent when it changes (read by
+   regk_read_events).  Without the flag every frame is byte for byte what it was.  With any write op (create, delete,
+   setData, replace; regk_reconcile_requests; regk_children_requests' delete) it is REGK_ERR_INVALID_ARG. */
+#define REGK_ZK_WATCH            (1u << 10)
 
 int         regk_reconcile_requests(regk_ctx *ctx, const regk_jute_opts *opts, regk_frames *out);
 
@@ -936,6 +942,99 @@ typedef struct regk_stat_opts {
 } regk_stat_opts;
 
 int         regk_reconcile_stats(regk_ctx *ctx, const regk_stat_opts *opts, uint32_t flags, regk_delta_owned *out);
+
+/*
+ * ---- the watched heartbeat: arm each node and service directory once (REGK_ZK_WATCH), read the notifications the
+ * server pushes for what changed, and re-check and re-arm only that.  An additional route: the reference polls every
+ * node with zk.stat (lib/zk.js:21-44), and the stat round above stays as it is ----------------------------------------
+ * regk_read_events: bytes[start, len) = what the caller read off the session; host memory, or device memory with
+ * REGK_IN_DEVICE in opts->flags (bytes 16-byte aligned; start need not be).  Positions, consumed included, count from
+ * bytes.  Every complete frame from start on is walked:
+ *   notification  int len | ReplyHeader{int xid = -1; long zxid; int err = 0} | WatcherEvent{int type; int state;
+ *                 ustring path}, so len == 28 + P (P = the path's length word, the path at +32 from the frame's first
+ *                 byte).  The header's zxid is reported, not checked: server versions differ in what they put there.
+ *   ping          xid -2, len == 16.
+ *   reply         an xid in [opts->xid_base, opts->xid_base + opts->n_xids) (wrapping): a reply to an outstanding
+ *                 request, skipped by its length whatever its body and counted, so one session stream can go through
+ *                 this call and through the reply readers, each reading its own frames and skipping the other's.
+ * A trailing partial frame is not an error (a socket read can end mid-frame): consumed stops at its start and
+ * out->partial = 1; feed the rest with the next call.  Without one, consumed == len.
+ * Event e (in stream order) has pos, type, state, zxid and a subject, mapped by the event's path (compared byte for byte;
+ * a hash only picks a table slot):
+ *   NodeCreated (1), NodeDeleted (2), NodeDataChanged (3)  the first record of the batch finished last with that path
+ *                                                          (REGK_EV_RECORD; a DUP record is never a subject itself)
+ *   NodeChildrenChanged (4), and NodeDeleted (2) of a path that is no record's
+ *                                                          service directory k of the batch, in the order and by the
+ *                                                          rule regk_children_requests lists them (REGK_EV_DIR)
+ *   anything else, or a path in neither set               REGK_EV_NONE, subject UINT64_MAX
+ * n_unmatched counts the REGK_EV_NONE events; n_other counts types -1 and 5 .. 7 (session events and watch removals),
+ * which are also unmatched.  Each mapped record event ORs its type's bit into its record's mark and each directory event
+ * marks its directory; a record or directory not yet pending joins the pending set, which accumulates over the calls of
+ * one batch generation (feed each recv separately) until regk_events_requests takes it.  A new batch drops it.  The
+ * tables are built on the first call after a batch finishes (work proportional to n); every later call's work is
+ * proportional to its stream and its events.  n_dirty_recs / n_dirty_dirs = what is pending after the call.
+ * pos .. subject are pinned host arrays, or device arrays with REGK_OUT_DEVICE; valid until the next call.
+ * REGK_ERR_STATE: no finished batch with a path stream, a pending batch.  REGK_ERR_INVALID_ARG (the message names the
+ * byte position; nothing is marked): len < 16, an xid other than -1 / -2 outside the reply range, a notification whose
+ * length is not 28 + P, P < 0, a notification with err != 0 or a type outside -1 .. 7, a ping with a body; a reply range
+ * that covers -1 or -2; start > len; NULL pointers; a misaligned device stream.
+ *
+ * regk_events_requests: frame the pending set of op, in ascending order, and clear it.  Watches are one-shot, so every
+ * frame carries watch = 1 whatever opts->flags says (only REGK_OUT_DEVICE is read from it); group must be 0.
+ *   REGK_ZK_EXISTS       one ExistsRequest per pending record (an exists watch arms a missing node as well as a present
+ *                        one).  Recorded as a SUBSET exists framing: regk_read_stats reads its replies unchanged, reply k
+ *                        answering pending record k and its arrays holding one entry per pending record; then
+ *                        regk_reconcile_stats classes the whole batch: a pending record by its stat, as always, every
+ *                        other record SAME (its watch has not fired), DUP detection over all n.  known_mzxid with a
+ *                        subset is REGK_ERR_INVALID_ARG: the repair's own writes fire the library's watches and move
+ *                        mzxid, so an mzxid baseline would never settle.  What a stat cannot see stays unseen: a
+ *                        same-length rewrite still fires NodeDataChanged, and the re-check then reads it as SAME.
+ *   REGK_ZK_GETCHILDREN  one GetChildrenRequest per pending directory, recorded as the last getChildren framing:
+ *                        regk_read_children reads it unchanged over that subset (dir_rec / dir_len are the subset's,
+ *                        n_unlisted == 0, the keep table still holds every directory of the batch), and
+ *                        regk_children_requests(REGK_ZK_DELETE) frames the stale children it finds.
+ * An empty pending set frames 0 requests and succeeds.  Any other op, group != 0: REGK_ERR_INVALID_ARG.  No
+ * regk_read_events call since the batch finished last, a pending batch, an exists framing of a batch without its payload
+ * stream: REGK_ERR_STATE.  flags: REGK_OUT_DEVICE as regk_jute_requests; the frames stay valid until the next call with
+ * that op.
+ * CONVERGENCE: the repair's own writes fire the library's own watches, so the next regk_read_events makes those records
+ * dirty; their re-check says SAME and re-arms them (a replaced node included).  Every byte the session delivers must pass
+ * through regk_read_events once.  After a reconnect that would need SetWatches, or a session expiry, run the full armed
+ * round again (the read framings with REGK_ZK_WATCH).
+ * PARITY UNPINNED: the layouts are restated from zookeeper.jute (ReplyHeader, WatcherEvent, ExistsRequest,
+ * GetChildrenRequest) and tested against an independent restatement, not against a server.
+ */
+#define REGK_EV_NONE    0u          /* regk_events.subject_kind[] */
+#define REGK_EV_RECORD  1u
+#define REGK_EV_DIR     2u
+
+typedef struct regk_events_opts {
+    int32_t  xid_base;              /* the replies still outstanding on the session: [xid_base, xid_base + n_xids) */
+    uint32_t n_xids;
+    uint32_t flags;                 /* REGK_IN_DEVICE | REGK_OUT_DEVICE */
+    uint32_t reserved;
+} regk_events_opts;
+
+typedef struct regk_events {
+    uint64_t n_events, n_pings, n_replies;
+    uint64_t n_unmatched, n_other;
+    uint64_t consumed;              /* end of the last complete frame (start when none) */
+    uint64_t n_dirty_recs, n_dirty_dirs;    /* pending after the call */
+    uint32_t partial;               /* 1: a frame starts at consumed and the stream ends inside it */
+    uint32_t flags, launches;       /* REGK_OUT_DEVICE */
+    uint32_t reserved;
+    const uint64_t *pos;            /* [n_events] the frame's first byte */
+    const int32_t  *type;           /* WatcherEvent.type */
+    const int32_t  *state;          /* WatcherEvent.state */
+    const int64_t  *zxid;           /* ReplyHeader.zxid */
+    const uint8_t  *subject_kind;   /* REGK_EV_* */
+    const uint64_t *subject;        /* record, directory, or UINT64_MAX */
+    float kernel_ms;
+} regk_events;
+
+int         regk_read_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, const regk_events_opts *opts,
+                             regk_events *out);
+int         regk_events_requests(regk_ctx *ctx, const regk_jute_opts *opts, regk_frames *out);
 
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);

@@ -100,6 +100,7 @@ ZK_GETDATA = 4                      # jute_requests: GetDataRequest{path, watch 
 ZK_GETCHILDREN = 8                  # children_requests: GetChildrenRequest{dir, watch = false}; replies go to read_children()
 ZK_REPLACE = 256                    # reconcile_requests after reconcile_owned: delete + create in one multi transaction
 FLAG_ZK_VERSION_OBSERVED = 1 << 9   # regk_jute_opts.flags: each frame carries its node's Stat.version
+FLAG_ZK_WATCH = 1 << 10             # regk_jute_opts.flags: a read framing arms a one-shot watch (watch byte = 1)
 
 
 class CDecodeIn(C.Structure):        # regk_decode_in
@@ -388,6 +389,43 @@ class Stats:
         self.mzxid = _as_np(out.mzxid, n, np.int64).copy()
 
 
+EV_NONE, EV_RECORD, EV_DIR = 0, 1, 2                                # Events.subject_kind
+
+
+class CEventsOpts(C.Structure):      # regk_events_opts
+    _fields_ = [("xid_base", C.c_int32), ("n_xids", C.c_uint32), ("flags", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class CEvents(C.Structure):          # regk_events
+    _fields_ = [("n_events", C.c_uint64), ("n_pings", C.c_uint64), ("n_replies", C.c_uint64),
+                ("n_unmatched", C.c_uint64), ("n_other", C.c_uint64), ("consumed", C.c_uint64),
+                ("n_dirty_recs", C.c_uint64), ("n_dirty_dirs", C.c_uint64), ("partial", C.c_uint32),
+                ("flags", C.c_uint32), ("launches", C.c_uint32), ("reserved", C.c_uint32), ("pos", C.c_void_p),
+                ("type", C.c_void_p), ("state", C.c_void_p), ("zxid", C.c_void_p), ("subject_kind", C.c_void_p),
+                ("subject", C.c_void_p), ("kernel_ms", C.c_float)]
+
+
+class Events:
+    """What read_events() made of one piece of the session stream: event e (stream order) has pos[e] (its frame's first
+    byte), type, state, zxid and subject_kind[e] / subject[e] (EV_RECORD: the record, EV_DIR: the service directory,
+    EV_NONE: UINT64_MAX).  Counts n_events, n_pings, n_replies, n_unmatched, n_other; `consumed` and `partial` (a frame
+    starts at consumed and is still arriving); n_dirty_recs / n_dirty_dirs pending after the call."""
+
+    def __init__(self, out):
+        n = int(out.n_events)
+        self.n_events, self.n_pings, self.n_replies = n, int(out.n_pings), int(out.n_replies)
+        self.n_unmatched, self.n_other = int(out.n_unmatched), int(out.n_other)
+        self.consumed, self.partial = int(out.consumed), bool(out.partial)
+        self.n_dirty_recs, self.n_dirty_dirs = int(out.n_dirty_recs), int(out.n_dirty_dirs)
+        self.launches, self.kernel_ms = int(out.launches), float(out.kernel_ms)
+        self.pos = _as_np(out.pos, n, np.uint64).copy()
+        self.type = _as_np(out.type, n, np.int32).copy()
+        self.state = _as_np(out.state, n, np.int32).copy()
+        self.zxid = _as_np(out.zxid, n, np.int64).copy()
+        self.subject_kind = _as_np(out.subject_kind, n, np.uint8).copy()
+        self.subject = _as_np(out.subject, n, np.uint64).copy()
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -401,7 +439,7 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records", "regk_mkdirp_dirs",
            "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned",
            "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results", "regk_read_stats",
-           "regk_reconcile_stats"]
+           "regk_reconcile_stats", "regk_read_events", "regk_events_requests"]
 
 _lib = None
 
@@ -464,6 +502,8 @@ def load_library():
     lib.regk_read_results.argtypes = [vp, vp, u64, u64, C.POINTER(CResultsOpts), C.POINTER(CResults)]
     lib.regk_read_stats.argtypes = [vp, vp, u64, u64, u32, C.POINTER(CStats)]
     lib.regk_reconcile_stats.argtypes = [vp, C.POINTER(CStatOpts), u32, C.POINTER(CDeltaOwned)]
+    lib.regk_read_events.argtypes = [vp, vp, u64, u64, C.POINTER(CEventsOpts), C.POINTER(CEvents)]
+    lib.regk_events_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     _lib = lib
     return lib
 
@@ -674,11 +714,13 @@ class Context:
                 float(out.kernel_ms))
 
     def jute_requests(self, op: int = ZK_CREATE, xid_base: int = 1, zk_flags: int = 1, version: int = -1, group: int = 0,
-                      device: bool = False):
+                      device: bool = False, watch: bool = False):
         """regk_jute_requests: create / delete / setData requests of the batch finished last, one per record
-        (group=0) or as multi transactions of `group` operations.  Returns (frame_bytes, frame_off uint64[frames+1],
-        kernel_ms), or the raw CFrames with device=True."""
-        o = CJuteOpts(int(op), FLAG_OUT_DEVICE if device else 0, int(xid_base), int(zk_flags), int(version), int(group))
+        (group=0) or as multi transactions of `group` operations.  watch=True arms a watch with each exists / getData
+        request (a write op refuses it).  Returns (frame_bytes, frame_off uint64[frames+1], kernel_ms), or the raw
+        CFrames with device=True."""
+        flags = (FLAG_OUT_DEVICE if device else 0) | (FLAG_ZK_WATCH if watch else 0)
+        o = CJuteOpts(int(op), flags, int(xid_base), int(zk_flags), int(version), int(group))
         out = CFrames()
         self._check(self._lib.regk_jute_requests(self._h, C.byref(o), C.byref(out)))
         if device:
@@ -865,14 +907,15 @@ class Context:
 
     # -- the batch's service directories listed, and the children it does not produce --
     def children_requests(self, op: int = ZK_GETCHILDREN, xid_base: int = 1, version: int = -1, group: int = 0,
-                          device: bool = False):
+                          device: bool = False, watch: bool = False):
         """regk_children_requests: ZK_GETCHILDREN frames one GetChildrenRequest per service directory of the batch
         finished last (its distinct parent directories but "/" and rejected ones, in order of first record); ZK_DELETE
         frames a DeleteRequest at `version` for every stale child of the last read_children(), singly or as multi
-        transactions of `group`.  Returns (frame_bytes, frame_off uint64[frames+1], kernel_ms), or the raw CFrames with
-        device=True."""
+        transactions of `group`.  watch=True arms a child watch with each getChildren request.  Returns (frame_bytes,
+        frame_off uint64[frames+1], kernel_ms), or the raw CFrames with device=True."""
         xid = (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31
-        o = CJuteOpts(int(op), FLAG_OUT_DEVICE if device else 0, xid, 0, int(version), int(group))
+        flags = (FLAG_OUT_DEVICE if device else 0) | (FLAG_ZK_WATCH if watch else 0)
+        o = CJuteOpts(int(op), flags, xid, 0, int(version), int(group))
         out = CFrames()
         self._check(self._lib.regk_children_requests(self._h, C.byref(o), C.byref(out)))
         if device:
@@ -982,6 +1025,48 @@ class Context:
         del keep
         self._check(rc)
         return out if device else Delta(out.d, out.replace, out.n_replace)
+
+    # -- the watched heartbeat: notifications read on the GPU, and re-checks of only what fired --
+    def read_events(self, stream, start: int = 0, xid_base: int = 0, n_xids: int = 0, device: bool = False):
+        """regk_read_events: `stream` (a NumPy uint8 array, or a contiguous CUDA uint8 tensor) holds, from byte `start`
+        on, bytes read off the session: watch notifications, pings, and replies to the [xid_base, xid_base + n_xids)
+        requests still outstanding (skipped).  Maps each notification to its record or service directory of the batch
+        finished last and adds it to the pending sets events_requests() frames.  Returns an Events, or the raw CEvents
+        (its arrays on the device) with device=True."""
+        flags = FLAG_OUT_DEVICE if device else 0
+        if hasattr(stream, "data_ptr"):
+            import torch
+            if not stream.is_cuda or stream.dtype != torch.uint8 or not stream.is_contiguous():
+                raise ValueError("a device stream is a contiguous CUDA uint8 tensor")
+            keep, ptr, n = stream, stream.data_ptr() or None, stream.numel()
+            flags |= FLAG_IN_DEVICE
+        else:
+            keep = np.ascontiguousarray(stream)
+            if keep.dtype != np.uint8 or keep.ndim != 1:
+                raise ValueError("a host stream is a one-dimensional uint8 array")
+            ptr, n = _np_ptr(keep), keep.size
+        xid = (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31
+        o = CEventsOpts(xid, int(n_xids), flags, 0)
+        out = CEvents()
+        rc = self._lib.regk_read_events(self._h, ptr, n, int(start), C.byref(o), C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else Events(out)
+
+    def events_requests(self, op: int, xid_base: int = 1, device: bool = False):
+        """regk_events_requests: the pending records (ZK_EXISTS) or service directories (ZK_GETCHILDREN) of the
+        read_events() calls since the last such call, one request each in ascending order, every one re-arming its
+        watch; the set is then empty.  read_stats() / reconcile_stats() and read_children() read the replies as a
+        subset.  Returns (frame_bytes, frame_off uint64[frames+1], kernel_ms), or the raw CFrames with device=True."""
+        xid = (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31
+        o = CJuteOpts(int(op), FLAG_OUT_DEVICE if device else 0, xid, 0, -1, 0)
+        out = CFrames()
+        self._check(self._lib.regk_events_requests(self._h, C.byref(o), C.byref(out)))
+        if device:
+            return out
+        n = int(out.n)
+        return (_as_np(out.frame_bytes, int(out.total), np.uint8).copy(), _as_np(out.frame_off, n + 1, np.uint64).copy(),
+                float(out.kernel_ms))
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

@@ -36,6 +36,7 @@
 #include "regk_children.cuh"
 #include "regk_results.cuh"
 #include "regk_stats.cuh"
+#include "regk_events.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -245,6 +246,11 @@ struct regk_ctx {
         bool read = false;                      /* the stale list of the last regk_read_children is in stale .. soff */
         uint64_t n_stale = 0;
         uint64_t read_gen = 0;                  /* bumped by every regk_read_children */
+        /* the directories whose prefixes go into the keep table: the framed ones, or the batch's whole set when
+           regk_events_requests framed a subset of it */
+        const unsigned long long *keep_drec = nullptr;
+        const uint32_t *keep_dlen = nullptr;
+        uint64_t keep_d = 0;
     } ch;
     /* regk_read_results (regk_results.cuh): what each write framing framed (one record per source, four for the
        reconcile ops), and the last read's chain, per-frame and per-entry arrays and lists */
@@ -273,7 +279,34 @@ struct regk_ctx {
         Event ev[2];
         bool read = false;                      /* the arrays of the last regk_read_stats are in err .. mzxid */
         uint64_t gen = 0, n = 0;                /* the batch generation and the records they answer */
+        /* a subset read (regk_events_requests): record k of the arrays is sub_rec[k] of a batch of batch_n records;
+           regk_reconcile_stats spreads it over f_err .. f_dlen */
+        bool sub = false;
+        uint64_t batch_n = 0;
+        DevBuf sub_rec, f_err, f_ver, f_own, f_dlen;
     } sq;
+    /* the subset of the last REGK_ZK_EXISTS framing of regk_events_requests (ex_sub; ex_n records, listed in ex_rec) */
+    bool ex_sub = false;
+    const unsigned long long *ex_rec = nullptr;
+    /* regk_read_events / regk_events_requests (regk_events.cuh).  Per batch generation: the directory set (the members
+       children_dirs fills), the record and directory tables, the marks and the pending counts.  Per call: the staged
+       stream, the chain, the events.  Per framing: the pending set compacted and its packed paths. */
+    struct Events {
+        ParentPass pass;
+        DevBuf totals, count, unlisted, drec, dlen, dbytes, doff;
+        HostBuf h_count;
+        uint64_t d = 0, n_unlisted = 0, prefixes = 0;
+        bool built = false, read = false;       /* tables of batch generation `gen`; events read for it */
+        uint64_t gen = 0, n = 0;
+        uint32_t rec_epoch = 1, dir_epoch = 1, mask_r = 0, mask_d = 0;
+        DevBuf zero, slot, t_rec, t_dir, rec_mark, dir_mark, dirty;
+        DevBuf stream, word, ftotals, tile_base, cand, mark, jump, ntotals, ecount;
+        DevBuf pos, type, state, zxid, kind, subject;
+        HostBuf h_ecount, h_pos, h_type, h_state, h_zxid, h_kind, h_subject;
+        Event ev[2];
+        DevBuf ptotals, pcount, item[2], prec[2], plen[2], pbytes, poff;
+        FrameBufs frames;
+    } evq;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     struct Skip {
@@ -946,7 +979,8 @@ static int frame_requests(regk_ctx *ctx, const FrameSrc &src, const regk_jute_op
     /* what follows the data: create - acl vector [OPEN_ACL_UNSAFE] + flags; delete / setData - the expected version */
     uint8_t tail[48] = {0};
     if (o->op == REGK_ZK_GETDATA || o->op == REGK_ZK_GETCHILDREN || o->op == REGK_ZK_EXISTS) {
-        p.tail_len = 1;                                 /* watch = false */
+        tail[0] = (o->flags & REGK_ZK_WATCH) ? 1u : 0u;  /* the watch byte */
+        p.tail_len = 1;
     } else if (o->op == REGK_ZK_CREATE) {
         static const uint8_t acl[27] = {0, 0, 0, 1, 0, 0, 0, 31, 0, 0, 0, 5, 'w', 'o', 'r', 'l', 'd', 0, 0, 0, 6, 'a', 'n', 'y', 'o', 'n', 'e'};
         memcpy(tail, acl, 27);
@@ -2480,6 +2514,9 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
     if (o->op != REGK_ZK_CREATE && o->op != REGK_ZK_DELETE && o->op != REGK_ZK_SETDATA && !getdata && !exists)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: op %u is not create (1), delete (2), exists (3), getData (4) "
                                                "or setData (5)", o->op);
+    if ((o->flags & REGK_ZK_WATCH) && !getdata && !exists)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: REGK_ZK_WATCH arms a watch with a read; op %u is a write",
+            o->op);
     if (o->group > 65536)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_jute_requests: at most 65536 operations per multi transaction");
     if ((getdata || exists) && o->group != 0)
@@ -2506,6 +2543,7 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
         ctx->ex_gen = ctx->last.gen;
         ctx->ex_xid = o->xid_base;
         ctx->ex_n = ctx->last.n;
+        ctx->ex_sub = false;
     } else if (rc == REGK_OK) {
         record_framing(ctx->rs.batch, src, o, o->op, o->group != 0, out->n, nullptr, ctx->last.gen);
     }
@@ -3262,6 +3300,9 @@ int regk_reconcile_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames 
                                                "replace (256)", o->op);
     if (observed && o->op == REGK_ZK_CREATE)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: a CreateRequest carries no version to observe");
+    if (o->flags & REGK_ZK_WATCH)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: REGK_ZK_WATCH arms a watch with a read; op %u is a "
+                                               "write", o->op);
     if (o->group > 65536)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_requests: at most 65536 operations per multi transaction");
     if (replace && o->group > 32768)
@@ -3636,11 +3677,14 @@ static int pack_strings(regk_ctx *ctx, uint64_t m, const uint8_t *path_bytes, co
     return REGK_OK;
 }
 
-/* The directory set of the batch finished last (n >= 1 records) into ctx->ch: its distinct parents in parent order,
-   listed (valid, not "/") to drec / dlen and packed to dbytes / doff, the others' first records to unlisted. */
-static int children_dirs(regk_ctx *ctx)
+/* The directory set of the batch finished last (n >= 1 records) into `ch` (ctx->ch, or ctx->evq for regk_read_events):
+   its distinct parents in parent order, listed (valid, not "/") to drec / dlen and, with `pack`, packed to dbytes /
+   doff, the others' first records to unlisted. */
+extern "C++" {
+namespace {
+template <class Dirs>
+int children_dirs(regk_ctx *ctx, Dirs &ch, bool pack)
 {
-    regk_ctx::Children &ch = ctx->ch;
     cudaStream_t s = ctx->stream;
     const uint64_t n = ctx->last.n;
     int rc;
@@ -3685,11 +3729,15 @@ static int children_dirs(regk_ctx *ctx)
     ch.d = hc[CQ_LISTED];
     ch.n_unlisted = hc[CQ_UNLISTED];
     ch.prefixes = hc[CQ_PREFIXES];
+    if (!pack)
+        return REGK_OK;
     uint64_t bytes = 0;
     uint32_t launches = 0;
     return pack_strings(ctx, ch.d, ctx->last.path_bytes, ctx->last.path_off, (const unsigned long long *)ch.drec.p,
         (const uint32_t *)ch.dlen.p, ch.totals, ch.dbytes, ch.doff, &bytes, &launches);
 }
+}  // namespace
+}  /* extern "C++" */
 
 int regk_children_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
 {
@@ -3698,6 +3746,9 @@ int regk_children_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *
     memset(out, 0, sizeof *out);
     regk_ctx::Children &ch = ctx->ch;
     if (o->op == REGK_ZK_DELETE) {
+        if (o->flags & REGK_ZK_WATCH)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_children_requests: REGK_ZK_WATCH arms a watch with a read; delete (2) "
+                                                   "is a write");
         if (o->group > 65536)
             return fail(ctx, REGK_ERR_INVALID_ARG, "regk_children_requests: at most 65536 operations per multi transaction");
         if (ctx->pending)
@@ -3731,7 +3782,7 @@ int regk_children_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *
     CK(cudaSetDevice(ctx->device));
     ch.framed = false;
     int rc;
-    if ((rc = children_dirs(ctx)))
+    if ((rc = children_dirs(ctx, ch, true)))
         return rc;
     FrameSrc src{ch.d, (const uint8_t *)ch.dbytes.p, (const unsigned long long *)ch.doff.p, nullptr, nullptr};
     src.who = "regk_children_requests";
@@ -3741,6 +3792,9 @@ int regk_children_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *
     ch.gen = ctx->last.gen;
     ch.n = ctx->last.n;
     ch.xid = o->xid_base;
+    ch.keep_drec = (const unsigned long long *)ch.drec.p;
+    ch.keep_dlen = (const uint32_t *)ch.dlen.p;
+    ch.keep_d = ch.d;
     return REGK_OK;
 }
 
@@ -4107,9 +4161,9 @@ int regk_read_children(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64
         kp.path_bytes = ctx->last.path_bytes;
         kp.path_off = ctx->last.path_off;
         kp.n = ch.n;
-        kp.dir_rec = (const unsigned long long *)ch.drec.p;
-        kp.dir_len = (const uint32_t *)ch.dlen.p;
-        kp.d = d;
+        kp.dir_rec = ch.keep_drec;
+        kp.dir_len = ch.keep_dlen;
+        kp.d = ch.keep_d;
         kp.table = (unsigned long long *)ch.table.p;
         kp.mask = (uint32_t)(slots - 1);
         kp.lst_bytes = (const uint8_t *)ch.lst_bytes.p;
@@ -4124,12 +4178,12 @@ int regk_read_children(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64
         CK(cudaMemsetAsync(kp.table, 0, slots * 8, s));
         CK(cudaMemsetAsync(ch.stotals.p, 0, st_bytes, s));
         regk_children_keep_paths_kernel<<<(unsigned)((ch.n + 255) / 256), 256, 0, s>>>(kp);
-        if (d)
-            regk_children_keep_dirs_kernel<<<(unsigned)((d + 255) / 256), 256, 0, s>>>(kp);
+        if (kp.d)
+            regk_children_keep_dirs_kernel<<<(unsigned)((kp.d + 255) / 256), 256, 0, s>>>(kp);
         regk_children_probe_kernel<<<(unsigned)tiles_l, MK_TILE, 0, s>>>(kp);
         regk_children_stale_kernel<<<(unsigned)tiles_l, MK_TILE, 0, s>>>(kp);
         CK(cudaGetLastError());
-        launches += d ? 4 : 3;
+        launches += kp.d ? 4 : 3;
         CK(cudaMemcpyAsync(hc + CQ_STALE, p.counters + CQ_STALE, 8, cudaMemcpyDeviceToHost, s));
         if ((rc = sync_or_fail(ctx, s, who)))
             return rc;
@@ -4650,6 +4704,16 @@ int regk_read_stats(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t 
         }
         CK(cudaStreamSynchronize(s));
     }
+    /* a subset framing's record list, kept with the read (the next regk_events_requests rewrites the framing's own) */
+    sq.sub = ctx->ex_sub;
+    sq.batch_n = ctx->last.n;
+    if (sq.sub) {
+        if ((rc = ensure_dev(ctx, sq.sub_rec, n * 8 + 16)))
+            return rc;
+        if (n)
+            CK(cudaMemcpyAsync(sq.sub_rec.p, ctx->ex_rec, n * 8, cudaMemcpyDeviceToDevice, s));
+        CK(cudaStreamSynchronize(s));
+    }
     sq.read = true;
     sq.gen = ctx->last.gen;
     sq.n = n;
@@ -4691,10 +4755,13 @@ int regk_reconcile_stats(regk_ctx *ctx, const regk_stat_opts *o, uint32_t flags,
     regk_ctx::Stats &sq = ctx->sq;
     if (!sq.read)
         return fail(ctx, REGK_ERR_STATE, "regk_reconcile_stats: no stats on this context; call regk_read_stats first");
-    if (sq.gen != ctx->last.gen || !ctx->last.path_off || !ctx->last.json_off || ctx->last.n != sq.n)
+    if (sq.gen != ctx->last.gen || !ctx->last.path_off || !ctx->last.json_off || ctx->last.n != (sq.sub ? sq.batch_n : sq.n))
         return fail(ctx, REGK_ERR_STATE, "regk_reconcile_stats: a batch finished after regk_read_stats; its stats answer "
                                          "another batch's records");
-    const uint64_t n = sq.n;
+    if (sq.sub && o->known_mzxid)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_reconcile_stats: known_mzxid with the stats of a regk_events_requests "
+                                               "subset: the repair's own writes fire its watches and move mzxid");
+    const uint64_t n = sq.sub ? sq.batch_n : sq.n;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->stream;
     int rc;
@@ -4703,6 +4770,39 @@ int regk_reconcile_stats(regk_ctx *ctx, const regk_stat_opts *o, uint32_t flags,
     sp.own = (const long long *)sq.own.p;
     sp.dlen = (const int32_t *)sq.dlen.p;
     sp.mzxid = (const long long *)sq.mzxid.p;
+    const int32_t *ver = (const int32_t *)sq.ver.p;
+    uint32_t launches = 3;
+    if (sq.sub) {
+        /* the records whose watches did not fire read as SAME: a node the batch owns at its payload length */
+        EvStatFill f{};
+        f.n = n;
+        f.m = sq.n;
+        f.json_off = ctx->last.json_off;
+        f.want = o->zk_flags == 1u ? (long long)o->session : 0ll;
+        f.rec = (const unsigned long long *)sq.sub_rec.p;
+        f.s_err = sp.err;
+        f.s_ver = ver;
+        f.s_dlen = sp.dlen;
+        f.s_own = sp.own;
+        if ((rc = ensure_dev(ctx, sq.f_err, n * 4 + 16)) || (rc = ensure_dev(ctx, sq.f_ver, n * 4 + 16)) ||
+            (rc = ensure_dev(ctx, sq.f_own, n * 8 + 16)) || (rc = ensure_dev(ctx, sq.f_dlen, n * 4 + 16)))
+            return rc;
+        f.err = (int32_t *)sq.f_err.p;
+        f.ver = (int32_t *)sq.f_ver.p;
+        f.own = (long long *)sq.f_own.p;
+        f.dlen = (int32_t *)sq.f_dlen.p;
+        if (n)
+            regk_events_stat_fill_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(f);
+        if (f.m)
+            regk_events_stat_scatter_kernel<<<(unsigned)((f.m + 255) / 256), 256, 0, s>>>(f);
+        CK(cudaGetLastError());
+        launches += (n ? 1 : 0) + (f.m ? 1 : 0);
+        sp.err = f.err;
+        sp.own = f.own;
+        sp.dlen = f.dlen;
+        sp.mzxid = nullptr;                         /* read only against known_mzxid */
+        ver = f.ver;
+    }
     sp.known_mzxid = (const long long *)o->known_mzxid;
     if (o->known_mzxid && !in_dev) {
         if ((rc = stage_in(ctx, sq.known, o->known_mzxid, n * 8, s)))
@@ -4712,7 +4812,7 @@ int regk_reconcile_stats(regk_ctx *ctx, const regk_stat_opts *o, uint32_t flags,
     /* no observed side: m = 0; the compact pass takes each update / replace entry's version from the stats, through
        match[i] = the record itself */
     ReconcileParams &p = sp.rc;
-    p.o_version = (const int32_t *)sq.ver.p;
+    p.o_version = ver;
     p.want = o->zk_flags == 1u ? (long long)o->session : 0ll;
     if ((rc = reconcile_prepare(ctx, n, 0, true, &p)))
         return rc;
@@ -4730,9 +4830,400 @@ int regk_reconcile_stats(regk_ctx *ctx, const regk_stat_opts *o, uint32_t flags,
         return fail(ctx, REGK_ERR_STATE, "regk_reconcile_stats: record %llu's reply carries error %d: the state of its node is "
                                          "unknown, and no repair over it is right", hc[RC_C_BAD], e);
     }
-    rc = reconcile_finish(ctx, p, hc, true, o->zk_flags, flags, 3, &out->d, &out->replace, &out->n_replace, who);
+    rc = reconcile_finish(ctx, p, hc, true, o->zk_flags, flags, launches, &out->d, &out->replace, &out->n_replace, who);
     out->d.obs_cls = nullptr;
     return rc;
+}
+
+static const char *events_reason(uint32_t code)
+{
+    switch (code) {
+    case EV_TRUNC: return "the stream ends inside the frame";
+    case EV_BAD_LEN: return "a frame length below 16 (no room for a ReplyHeader)";
+    case EV_NEG_XID: return "a negative xid other than -1 (notification) or -2 (ping), outside the reply range";
+    case EV_XID_RANGE: return "an xid outside the reply range";
+    case EV_NOTE_LEN: return "a notification whose length is not 28 + its path length";
+    case EV_NEG_PATH: return "a notification with a negative path length";
+    case EV_NOTE_ERR: return "a notification with err != 0";
+    case EV_TYPE: return "a notification whose type is outside -1 .. 7";
+    case EV_PING_BODY: return "a ping with a body";
+    default: return "internal error";
+    }
+}
+
+/* The tables regk_read_events maps paths with, for the batch finished last: the record table, the directory set and
+   its table, zeroed marks and pending counts.  Once per batch generation. */
+static int events_build(regk_ctx *ctx, const char *who)
+{
+    regk_ctx::Events &ev = ctx->evq;
+    cudaStream_t s = ctx->stream;
+    const uint64_t n = ctx->last.n;
+    int rc;
+    ev.built = ev.read = false;
+    ev.d = ev.prefixes = ev.n_unlisted = 0;
+    if (n && !ctx->last.alias && (rc = children_dirs(ctx, ev, false)))
+        return rc;
+    const uint64_t d = ev.d;
+    uint64_t sr = 1024, sd = 1024;
+    while (sr < 2 * n)
+        sr <<= 1;
+    while (sd < 2 * d)
+        sd <<= 1;
+    if (sr > (1ull << 32))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: %llu records are too many for one table", who, (unsigned long long)n);
+    if ((rc = ensure_dev(ctx, ev.zero, n * 4 + 16)) || (rc = ensure_dev(ctx, ev.slot, n * 4 + 16)) ||
+        (rc = ensure_dev(ctx, ev.t_rec, sr * 4)) || (rc = ensure_dev(ctx, ev.t_dir, sd * 4)) ||
+        (rc = ensure_dev(ctx, ev.rec_mark, n * 4 + 16)) || (rc = ensure_dev(ctx, ev.dir_mark, d * 4 + 16)) ||
+        (rc = ensure_dev(ctx, ev.dirty, 16)))
+        return rc;
+    CK(cudaMemsetAsync(ev.zero.p, 0, n * 4 + 16, s));
+    CK(cudaMemsetAsync(ev.t_rec.p, 0, sr * 4, s));
+    CK(cudaMemsetAsync(ev.t_dir.p, 0, sd * 4, s));
+    CK(cudaMemsetAsync(ev.rec_mark.p, 0, n * 4 + 16, s));
+    CK(cudaMemsetAsync(ev.dir_mark.p, 0, d * 4 + 16, s));
+    CK(cudaMemsetAsync(ev.dirty.p, 0, 16, s));
+    if (n) {
+        /* every record "found": the first record with a path keeps its slot */
+        RepParams rp{};
+        rp.n = n;
+        rp.err = (int32_t *)ev.zero.p;
+        rp.d_path = ctx->last.path_bytes;
+        rp.d_path_off = ctx->last.path_off;
+        rp.table = (uint32_t *)ev.t_rec.p;
+        rp.mask_t = (uint32_t)(sr - 1);
+        rp.slot = (uint32_t *)ev.slot.p;
+        regk_replies_insert_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(rp);
+    }
+    if (d) {
+        EvDirParams dp{};
+        dp.d_path = ctx->last.path_bytes;
+        dp.d_path_off = ctx->last.path_off;
+        dp.dir_rec = (const unsigned long long *)ev.drec.p;
+        dp.dir_len = (const uint32_t *)ev.dlen.p;
+        dp.d = d;
+        dp.table = (uint32_t *)ev.t_dir.p;
+        dp.mask = (uint32_t)(sd - 1);
+        regk_events_dir_insert_kernel<<<(unsigned)((d + 255) / 256), 256, 0, s>>>(dp);
+    }
+    CK(cudaGetLastError());
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    ev.mask_r = (uint32_t)(sr - 1);
+    ev.mask_d = (uint32_t)(sd - 1);
+    ev.rec_epoch = ev.dir_epoch = 1;
+    ev.n = n;
+    ev.gen = ctx->last.gen;
+    ev.built = true;
+    return REGK_OK;
+}
+
+int regk_read_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, const regk_events_opts *o,
+    regk_events *out)
+{
+    const char *who = "regk_read_events";
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_events: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Events &ev = ctx->evq;
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_events: batches are still in flight; finish them first");
+    if (!ctx->last.path_off || !ctx->last.path_bytes)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_events: no finished batch with a path stream on this context: events "
+                                         "map to the records of the batch finished last");
+    if (ctx->last.n >= 0xFFFFFFFEull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_events: batch too large");
+    if (!bytes && len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_events: NULL stream of %llu bytes", (unsigned long long)len);
+    if (start > len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_events: start %llu is past the stream's %llu bytes",
+            (unsigned long long)start, (unsigned long long)len);
+    const bool in_dev = o->flags & REGK_IN_DEVICE, dev_out = o->flags & REGK_OUT_DEVICE;
+    if (in_dev && ((uintptr_t)bytes & 15u))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_events: misaligned device stream (16-byte alignment needed)");
+    const int32_t xb = o->xid_base;
+    const uint64_t nx = o->n_xids;
+    for (int32_t reserved : {-1, -2})
+        if ((uint64_t)((uint32_t)reserved - (uint32_t)xb) < nx)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_events: the reply xids [%d, %d + %llu) cover %d, which ZooKeeper "
+                                                   "uses for %s", xb, xb, (unsigned long long)nx, reserved,
+                        reserved == -1 ? "watch notifications" : "pings");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    if (!ev.built || ev.gen != ctx->last.gen) {
+        if ((rc = events_build(ctx, who)))
+            return rc;
+    }
+    for (Event &e : ev.ev)
+        if ((rc = ensure_event(ctx, e)))
+            return rc;
+    const uint8_t *ds = bytes;
+    if (!in_dev && len) {
+        if ((rc = stage_in(ctx, ev.stream, bytes, len, s)))
+            return rc;
+        ds = (const uint8_t *)ev.stream.p;
+    }
+    const uint64_t nblk = (len + 15) / 16, tiles_s = (nblk + RP_TILE - 1) / RP_TILE;
+    const size_t totals_bytes = align16(tiles_s * 4) + (tiles_s / SUPER + 1) * 8;
+    if ((rc = ensure_dev(ctx, ev.word, nblk * 4 + 16)) || (rc = ensure_dev(ctx, ev.ftotals, totals_bytes)) ||
+        (rc = ensure_dev(ctx, ev.tile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, ev.ecount, EQ_NCOUNTERS * 8)) ||
+        (rc = ensure_host(ctx, ev.h_ecount, EQ_NCOUNTERS * 8 + 16)))
+        return rc;
+    EvParams ep{};
+    RepParams &p = ep.r;
+    p.s = ds;
+    p.len = len;
+    p.xid_base = xb;
+    p.n = nx;
+    p.word = (uint32_t *)ev.word.p;
+    p.tile_total = (uint32_t *)ev.ftotals.p;
+    p.super_total = (unsigned long long *)((uint8_t *)ev.ftotals.p + align16(tiles_s * 4));
+    p.tile_base = (unsigned long long *)ev.tile_base.p;
+    p.counters = (unsigned long long *)ev.ecount.p;
+    ep.start = start;
+    ep.d_path = ctx->last.path_bytes;
+    ep.d_path_off = ctx->last.path_off;
+    ep.t_rec = (const uint32_t *)ev.t_rec.p;
+    ep.mask_r = ev.mask_r;
+    ep.t_dir = (const uint32_t *)ev.t_dir.p;
+    ep.mask_d = ev.mask_d;
+    ep.dir_rec = (const unsigned long long *)ev.drec.p;
+    ep.dir_len = (const uint32_t *)ev.dlen.p;
+    ep.rec_mark = (uint32_t *)ev.rec_mark.p;
+    ep.dir_mark = (uint32_t *)ev.dir_mark.p;
+    ep.rec_epoch = ev.rec_epoch;
+    ep.dir_epoch = ev.dir_epoch;
+    ep.dirty = (unsigned long long *)ev.dirty.p;
+    unsigned long long *hc = (unsigned long long *)ev.h_ecount.p;
+    CK(cudaMemsetAsync(p.counters, 0, EQ_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(p.tile_total, 0, totals_bytes, s));
+    CK(cudaEventRecord(ev.ev[0], s));
+    uint32_t launches = 0;
+    /* 1. the frame chain from `start` and where it stops */
+    RepParams pf = p;
+    if (len > start) {
+        regk_events_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(ep);
+        CK(cudaGetLastError());
+        launches++;
+        uint32_t *J = nullptr;
+        if ((rc = chain_pass(ctx, &pf, tiles_s, ~0ull, ev.cand, ev.mark, ev.jump, [&](const RepParams &q) {
+                regk_children_seed_kernel<<<1, 256, 0, s>>>(q, nullptr, nullptr, 1, start);
+            }, &J, &launches, who)))
+            return rc;
+        if (pf.C) {
+            regk_replies_stop_kernel<<<(unsigned)((pf.C + 255) / 256), 256, 0, s>>>(pf);
+            CK(cudaGetLastError());
+            launches++;
+        }
+    }
+    CK(cudaMemcpyAsync(hc, p.counters, EQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    const uint64_t stop = std::max<uint64_t>(start, hc[RQ_STOP]);
+    bool partial = false;
+    if (stop < len) {
+        /* the first position the chain does not pass: a frame still arriving, or a fault.  Nothing has been marked. */
+        uint8_t head[32] = {0};
+        const uint64_t avail = len - stop, take = std::min<uint64_t>(avail, sizeof head);
+        CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        EvHead h;
+        const uint32_t code = ev_head(head, avail, xb, nx, &h);   /* reads at most 32 bytes, all of them in head */
+        if (code != EV_TRUNC)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_events: byte %llu: %s (len %d, xid %d)", (unsigned long long)stop,
+                code ? events_reason(code) : "internal error", h.len, h.xid);
+        partial = true;
+    }
+    /* 2. the events of the chain, mapped and marked */
+    const uint64_t C = pf.C;
+    if ((rc = ensure_dev(ctx, ev.pos, C * 8 + 16)) || (rc = ensure_dev(ctx, ev.subject, C * 8 + 16)) ||
+        (rc = ensure_dev(ctx, ev.zxid, C * 8 + 16)) || (rc = ensure_dev(ctx, ev.type, C * 4 + 16)) ||
+        (rc = ensure_dev(ctx, ev.state, C * 4 + 16)) || (rc = ensure_dev(ctx, ev.kind, C + 16)))
+        return rc;
+    ep.r = pf;
+    ep.pos = (unsigned long long *)ev.pos.p;
+    ep.subject = (unsigned long long *)ev.subject.p;
+    ep.zxid = (long long *)ev.zxid.p;
+    ep.type = (int32_t *)ev.type.p;
+    ep.state = (int32_t *)ev.state.p;
+    ep.kind = (uint8_t *)ev.kind.p;
+    if (C) {
+        const uint64_t tiles_c = (C + RP_TILE - 1) / RP_TILE;
+        const size_t t2 = align16(tiles_c * 4) + (tiles_c / SUPER + 1) * 8;
+        if ((rc = ensure_dev(ctx, ev.ntotals, t2)))
+            return rc;
+        ep.tile_total = (uint32_t *)ev.ntotals.p;
+        ep.super_total = (unsigned long long *)((uint8_t *)ev.ntotals.p + align16(tiles_c * 4));
+        CK(cudaMemsetAsync(ev.ntotals.p, 0, t2, s));
+        regk_events_count_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(ep);
+        regk_events_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(ep);
+        CK(cudaGetLastError());
+        launches += 2;
+    }
+    CK(cudaEventRecord(ev.ev[1], s));
+    CK(cudaMemcpyAsync(hc, p.counters, EQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(hc + EQ_NCOUNTERS, ev.dirty.p, 16, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    const uint64_t ne = C ? hc[EQ_NEV] : 0;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, ev.ev[0], ev.ev[1]);
+    const void *src[6] = {ev.pos.p, ev.type.p, ev.state.p, ev.zxid.p, ev.kind.p, ev.subject.p};
+    if (!dev_out) {
+        HostBuf *hb[6] = {&ev.h_pos, &ev.h_type, &ev.h_state, &ev.h_zxid, &ev.h_kind, &ev.h_subject};
+        const size_t sz[6] = {ne * 8, ne * 4, ne * 4, ne * 8, ne, ne * 8};
+        for (int k = 0; k < 6; k++) {
+            if ((rc = to_host(ctx, *hb[k], src[k], sz[k], s)))
+                return rc;
+            src[k] = hb[k]->p;
+        }
+        CK(cudaStreamSynchronize(s));
+    }
+    ev.read = true;
+    out->n_events = ne;
+    out->n_pings = hc[EQ_PING];
+    out->n_replies = hc[EQ_REPLY];
+    out->n_unmatched = hc[EQ_UNMATCHED];
+    out->n_other = hc[EQ_OTHER];
+    out->consumed = stop;
+    out->n_dirty_recs = hc[EQ_NCOUNTERS];
+    out->n_dirty_dirs = hc[EQ_NCOUNTERS + 1];
+    out->partial = partial ? 1u : 0u;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->pos = (const uint64_t *)src[0];
+    out->type = (const int32_t *)src[1];
+    out->state = (const int32_t *)src[2];
+    out->zxid = (const int64_t *)src[3];
+    out->subject_kind = (const uint8_t *)src[4];
+    out->subject = (const uint64_t *)src[5];
+    out->kernel_ms = ms;
+    return REGK_OK;
+}
+
+/* The pending records (dirs == false) or directories of the current epoch, ascending, into evq.item / prec / plen[dirs];
+   *m = their number. */
+static int events_pending(regk_ctx *ctx, bool dirs, uint64_t *m, uint32_t *launches, const char *who)
+{
+    regk_ctx::Events &ev = ctx->evq;
+    cudaStream_t s = ctx->stream;
+    const int w = dirs ? 1 : 0;
+    const uint64_t N = dirs ? ev.d : ev.n;
+    const uint64_t tiles = (N + RP_TILE - 1) / RP_TILE;
+    const size_t tb = align16(tiles * 4) + (tiles / SUPER + 1) * 8;
+    int rc;
+    if ((rc = ensure_dev(ctx, ev.ptotals, tb + 16)) || (rc = ensure_dev(ctx, ev.pcount, 16)) ||
+        (rc = ensure_dev(ctx, ev.item[w], N * 8 + 16)) || (rc = ensure_dev(ctx, ev.prec[w], N * 8 + 16)) ||
+        (rc = ensure_dev(ctx, ev.plen[w], N * 4 + 16)))
+        return rc;
+    *m = 0;
+    if (!N)
+        return REGK_OK;
+    EvPendParams pp{};
+    pp.n = N;
+    pp.mark = (const uint32_t *)(dirs ? ev.dir_mark.p : ev.rec_mark.p);
+    pp.shift = dirs ? 0u : 3u;
+    pp.epoch = dirs ? ev.dir_epoch : ev.rec_epoch;
+    pp.path_off = ctx->last.path_off;
+    pp.dir_rec = dirs ? (const unsigned long long *)ev.drec.p : nullptr;
+    pp.dir_len = dirs ? (const uint32_t *)ev.dlen.p : nullptr;
+    pp.tile_total = (uint32_t *)ev.ptotals.p;
+    pp.super_total = (unsigned long long *)((uint8_t *)ev.ptotals.p + align16(tiles * 4));
+    pp.item = (unsigned long long *)ev.item[w].p;
+    pp.rec = (unsigned long long *)ev.prec[w].p;
+    pp.len = (uint32_t *)ev.plen[w].p;
+    pp.count = (unsigned long long *)ev.pcount.p;
+    CK(cudaMemsetAsync(ev.ptotals.p, 0, tb, s));
+    regk_events_pending_count_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(pp);
+    regk_events_pending_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(pp);
+    CK(cudaGetLastError());
+    *launches += 2;
+    unsigned long long cnt = 0;
+    CK(cudaMemcpyAsync(&cnt, pp.count, 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    *m = cnt;
+    return REGK_OK;
+}
+
+int regk_events_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
+{
+    const char *who = "regk_events_requests";
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_events_requests: NULL argument");
+    memset(out, 0, sizeof *out);
+    const bool exists = o->op == REGK_ZK_EXISTS;
+    if (!exists && o->op != REGK_ZK_GETCHILDREN)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_events_requests: op %u is not exists (3) or getChildren (8)", o->op);
+    if (o->group != 0)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_events_requests: reads cannot go in a multi transaction (group %u)", o->group);
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_events_requests: batches are still in flight; finish them first");
+    regk_ctx::Events &ev = ctx->evq;
+    if (!ev.read || ev.gen != ctx->last.gen || !ctx->last.path_off)
+        return fail(ctx, REGK_ERR_STATE, "regk_events_requests: no regk_read_events call for the batch finished last");
+    if (exists && (!ctx->last.json_off || ctx->last.n != ctx->last.json_n))
+        return fail(ctx, REGK_ERR_STATE, "regk_events_requests: no finished batch with both a path and a payload stream on "
+                                         "this context: the exists replies are classed against the payload lengths");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    uint64_t m = 0, total = 0;
+    uint32_t launches = 0;
+    const int w = exists ? 0 : 1;
+    if ((rc = events_pending(ctx, !exists, &m, &launches, who)))
+        return rc;
+    regk_jute_opts oo = *o;
+    oo.flags = (o->flags & REGK_OUT_DEVICE) | REGK_ZK_WATCH;    /* watches are one-shot: every re-check re-arms */
+    FrameSrc src{};
+    src.who = who;
+    if (exists) {
+        ctx->ex_valid = false;
+        if ((rc = pack_strings(ctx, m, ctx->last.path_bytes, ctx->last.path_off, (const unsigned long long *)ev.prec[w].p,
+                 (const uint32_t *)ev.plen[w].p, ev.ptotals, ev.pbytes, ev.poff, &total, &launches)))
+            return rc;
+        src = FrameSrc{m, (const uint8_t *)ev.pbytes.p, (const unsigned long long *)ev.poff.p, nullptr, nullptr, who};
+        if ((rc = frame_requests(ctx, src, &oo, ev.frames, out)))
+            return rc;
+        ctx->ex_valid = true;
+        ctx->ex_gen = ctx->last.gen;
+        ctx->ex_xid = o->xid_base;
+        ctx->ex_n = m;
+        ctx->ex_sub = true;
+        ctx->ex_rec = (const unsigned long long *)ev.item[w].p;
+        ev.rec_epoch++;
+    } else {
+        regk_ctx::Children &ch = ctx->ch;
+        ch.framed = false;
+        if ((rc = ensure_dev(ctx, ch.drec, m * 8 + 8)) || (rc = ensure_dev(ctx, ch.dlen, m * 4 + 8)) ||
+            (rc = ensure_dev(ctx, ch.unlisted, 8)))
+            return rc;
+        if (m) {
+            CK(cudaMemcpyAsync(ch.drec.p, ev.prec[w].p, m * 8, cudaMemcpyDeviceToDevice, s));
+            CK(cudaMemcpyAsync(ch.dlen.p, ev.plen[w].p, m * 4, cudaMemcpyDeviceToDevice, s));
+        }
+        if ((rc = pack_strings(ctx, m, ctx->last.path_bytes, ctx->last.path_off, (const unsigned long long *)ch.drec.p,
+                 (const uint32_t *)ch.dlen.p, ch.totals, ch.dbytes, ch.doff, &total, &launches)))
+            return rc;
+        src = FrameSrc{m, (const uint8_t *)ch.dbytes.p, (const unsigned long long *)ch.doff.p, nullptr, nullptr, who};
+        if ((rc = frame_requests(ctx, src, &oo, ch.frames[0], out)))
+            return rc;
+        ch.framed = true;
+        ch.gen = ctx->last.gen;
+        ch.n = ctx->last.n;
+        ch.d = m;
+        ch.n_unlisted = 0;
+        ch.prefixes = ev.prefixes;
+        ch.xid = o->xid_base;
+        ch.keep_drec = (const unsigned long long *)ev.drec.p;
+        ch.keep_dlen = (const uint32_t *)ev.dlen.p;
+        ch.keep_d = ev.d;
+        ev.dir_epoch++;
+    }
+    CK(cudaMemsetAsync((unsigned long long *)ev.dirty.p + w, 0, 8, s));
+    CK(cudaStreamSynchronize(s));
+    out->launches += launches;
+    return REGK_OK;
 }
 
 int regk_release(regk_ctx *ctx, regk_result *res)
