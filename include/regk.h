@@ -999,8 +999,8 @@ int         regk_reconcile_stats(regk_ctx *ctx, const regk_stat_opts *opts, uint
  * that op.
  * CONVERGENCE: the repair's own writes fire the library's own watches, so the next regk_read_events makes those records
  * dirty; their re-check says SAME and re-arms them (a replaced node included).  Every byte the session delivers must pass
- * through regk_read_events once.  After a reconnect that would need SetWatches, or a session expiry, run the full armed
- * round again (the read framings with REGK_ZK_WATCH).
+ * through regk_read_events once.  After a reconnect, regk_setwatches_requests below carries the watches over; after a
+ * session expiry, run the full armed round again (the read framings with REGK_ZK_WATCH).
  * PARITY UNPINNED: the layouts are restated from zookeeper.jute (ReplyHeader, WatcherEvent, ExistsRequest,
  * GetChildrenRequest) and tested against an independent restatement, not against a server.
  */
@@ -1035,6 +1035,64 @@ typedef struct regk_events {
 int         regk_read_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, const regk_events_opts *opts,
                              regk_events *out);
 int         regk_events_requests(regk_ctx *ctx, const regk_jute_opts *opts, regk_frames *out);
+
+/*
+ * ---- the watched heartbeat across a reconnect: ZooKeeper forgets a connection's watches when it drops, though the
+ * session survives.  regk_setwatches_requests frames SetWatches (op 101) for the watches the session holds, so the
+ * server re-arms them on the new connection or fires what the client missed, and re-pends everything else -----------
+ * The context keeps, per batch generation, the watch kind each first-of-path record and each service directory holds:
+ *   regk_read_stats of an exists framing with the watch byte (REGK_ZK_WATCH, or an regk_events_requests subset): err 0
+ *   gives DATA, NONODE gives EXIST (an exists watch arms a missing node too), any other err NONE.
+ *   regk_read_children of a getChildren framing with the watch byte: err 0 gives CHILD, anything else NONE (ZooKeeper
+ *   leaves no child watch on a missing node).
+ * Unwatched reads leave the kinds alone; a new batch resets them all to NONE.  A watched framing whose replies have not
+ * been read is in flight: its requests die with the connection, so its items count as NONE.  The bookkeeping after a
+ * watched read is one kernel that the read's `launches` and kernel_ms do not include.
+ * The session zxid is the largest ReplyHeader.zxid of every complete reply a successful regk_read_events call walked
+ * (replies in the outstanding xid range and SetWatches replies; not notifications or pings), 0 at first, kept for the
+ * context's whole life.  It is safe as relativeZxid: a reply with zxid R leaves the server after every notification of
+ * a change at or below R, and TCP keeps that order, so an event the client missed is one the session never delivered,
+ * and then R was not read either.  Underestimating is always safe: the server only fires spurious events, which cost
+ * re-checks.
+ *
+ * regk_setwatches_requests: call it when the connection drops, before reconnecting; relative_zxid is also the
+ * lastZxidSeen of the ConnectRequest.  The lists, each without the pending records and directories (their re-check
+ * re-arms them):
+ *   D  the records of kind DATA, ascending          E  the records of kind EXIST, ascending
+ *   C  the directories of kind CHILD, in the order regk_children_requests lists them
+ * Every other first-of-path record and every other directory joins the current pending set (NONE, in flight, never
+ * armed; n_repend_*), so after the call each one is either listed or pending and regk_events_requests re-checks the
+ * rest.  With no watched round read, nothing is listed and everything is pending.
+ * Frames, big endian: int len | int xid = -8 | int type = 101 | long relativeZxid | int nD | nD x (int P | path) | int nE
+ * | ... | int nC | ..., 32 bytes of header and count words each.  The split, in closed form: with S = D ++ E ++ C, s_j the
+ * exclusive prefix of the entry sizes 4 + P, Lmax = 4 + the batch's longest path and B = max_frame - 32 - Lmax, entry j
+ * goes into frame floor(s_j / B).  Every frame holds at least one entry and is shorter than max_frame (len + 4 bytes).
+ * max_frame 0 means 131072 (the Java client's 128 KiB); below 32 + 2 Lmax, or 2^31 or more, it is refused (the message
+ * names the minimum).  The server closes the connection when a frame's len exceeds its jute.maxbuffer (1048575 by
+ * default).  frames.frame_bytes / frame_off are pinned host arrays, or device arrays with REGK_OUT_DEVICE in
+ * opts->flags; valid until the next call.  Empty lists frame 0 frames.
+ * After a successful call regk_read_events, for this batch generation, also accepts a SetWatches reply (xid -8, len 16,
+ * err 0: skipped and counted in n_replies, its zxid entering the high-water mark); a -8 frame with a body or an err is
+ * refused.  Without the call, -8 is refused as any negative xid.
+ * REGK_ERR_STATE: a pending batch, no finished batch with a path stream.  REGK_ERR_INVALID_ARG: NULL pointers, a bad
+ * max_frame, unknown flag bits.  The tables are built on demand, as regk_read_events builds them.
+ * PARITY UNPINNED: the layout is restated from zookeeper.jute (SetWatches) and the server's re-arming from ZooKeeper
+ * 3.4's DataTree.setWatches, tested against an independent restatement, not against a server.
+ */
+typedef struct regk_setwatches_opts {
+    uint32_t max_frame;             /* bytes per frame, len word included; 0 = 131072 */
+    uint32_t flags;                 /* REGK_OUT_DEVICE */
+} regk_setwatches_opts;
+
+typedef struct regk_setwatches {
+    uint64_t n_data, n_exist, n_child;          /* paths listed */
+    uint64_t n_repend_recs, n_repend_dirs;      /* made pending by this call */
+    uint64_t n_dirty_recs, n_dirty_dirs;        /* pending after the call, as regk_read_events reports them */
+    int64_t  relative_zxid;
+    regk_frames frames;
+} regk_setwatches;
+
+int         regk_setwatches_requests(regk_ctx *ctx, const regk_setwatches_opts *opts, regk_setwatches *out);
 
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);

@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import struct
 from typing import Optional
 
 import numpy as np
@@ -426,6 +427,46 @@ class Events:
         self.subject = _as_np(out.subject, n, np.uint64).copy()
 
 
+class CSetWatchesOpts(C.Structure):  # regk_setwatches_opts
+    _fields_ = [("max_frame", C.c_uint32), ("flags", C.c_uint32)]
+
+
+class CSetWatches(C.Structure):      # regk_setwatches
+    _fields_ = [("n_data", C.c_uint64), ("n_exist", C.c_uint64), ("n_child", C.c_uint64),
+                ("n_repend_recs", C.c_uint64), ("n_repend_dirs", C.c_uint64), ("n_dirty_recs", C.c_uint64),
+                ("n_dirty_dirs", C.c_uint64), ("relative_zxid", C.c_int64), ("frames", CFrames)]
+
+
+class SetWatches:
+    """What setwatches_requests() framed: SetWatches frames (frames uint8[total], frame_off uint64[n_frames+1]) for the
+    n_data / n_exist / n_child watches the session holds, relative_zxid (also the ConnectRequest's lastZxidSeen), and
+    n_repend_recs / n_repend_dirs made pending instead, n_dirty_recs / n_dirty_dirs pending after the call."""
+
+    def __init__(self, out):
+        f = out.frames
+        self.n_frames, self.launches, self.kernel_ms = int(f.n), int(f.launches), float(f.kernel_ms)
+        self.frames = _as_np(f.frame_bytes, int(f.total), np.uint8).copy()
+        self.frame_off = _as_np(f.frame_off, self.n_frames + 1, np.uint64).copy()
+        self.n_data, self.n_exist, self.n_child = int(out.n_data), int(out.n_exist), int(out.n_child)
+        self.n_repend_recs, self.n_repend_dirs = int(out.n_repend_recs), int(out.n_repend_dirs)
+        self.n_dirty_recs, self.n_dirty_dirs = int(out.n_dirty_recs), int(out.n_dirty_dirs)
+        self.relative_zxid = int(out.relative_zxid)
+
+    def lists(self):
+        """(D, E, C): the data, exist and child watch paths, in frame order, read back out of the frames"""
+        b, out = self.frames.tobytes(), ([], [], [])
+        for f in range(self.n_frames):
+            k = int(self.frame_off[f]) + 20
+            for lst in out:
+                (cnt,) = struct.unpack_from(">i", b, k)
+                k += 4
+                for _ in range(cnt):
+                    (pl,) = struct.unpack_from(">i", b, k)
+                    lst.append(b[k + 4:k + 4 + pl])
+                    k += 4 + pl
+        return out
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -439,7 +480,8 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_jute_frames", "regk_jute_requests", "regk_decode", "regk_skipped_records", "regk_mkdirp_dirs",
            "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned",
            "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results", "regk_read_stats",
-           "regk_reconcile_stats", "regk_read_events", "regk_events_requests"]
+           "regk_reconcile_stats", "regk_read_events", "regk_events_requests",
+           "regk_setwatches_requests"]
 
 _lib = None
 
@@ -504,6 +546,7 @@ def load_library():
     lib.regk_reconcile_stats.argtypes = [vp, C.POINTER(CStatOpts), u32, C.POINTER(CDeltaOwned)]
     lib.regk_read_events.argtypes = [vp, vp, u64, u64, C.POINTER(CEventsOpts), C.POINTER(CEvents)]
     lib.regk_events_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
+    lib.regk_setwatches_requests.argtypes = [vp, C.POINTER(CSetWatchesOpts), C.POINTER(CSetWatches)]
     _lib = lib
     return lib
 
@@ -1067,6 +1110,15 @@ class Context:
         n = int(out.n)
         return (_as_np(out.frame_bytes, int(out.total), np.uint8).copy(), _as_np(out.frame_off, n + 1, np.uint64).copy(),
                 float(out.kernel_ms))
+
+    def setwatches_requests(self, max_frame: int = 0, device: bool = False):
+        """regk_setwatches_requests: after the connection dropped, SetWatches frames for the watches the session holds
+        (frames of at most max_frame bytes; 0 = 131072), with every other record and service directory made pending
+        for events_requests().  Returns a SetWatches, or the raw CSetWatches (frames on the device) with device=True."""
+        o = CSetWatchesOpts(int(max_frame), FLAG_OUT_DEVICE if device else 0)
+        out = CSetWatches()
+        self._check(self._lib.regk_setwatches_requests(self._h, C.byref(o), C.byref(out)))
+        return out if device else SetWatches(out)
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

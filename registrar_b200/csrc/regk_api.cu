@@ -37,6 +37,7 @@
 #include "regk_results.cuh"
 #include "regk_stats.cuh"
 #include "regk_events.cuh"
+#include "regk_setwatches.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -251,6 +252,9 @@ struct regk_ctx {
         const unsigned long long *keep_drec = nullptr;
         const uint32_t *keep_dlen = nullptr;
         uint64_t keep_d = 0;
+        /* a subset framing of regk_events_requests: directory k of the framing is directory sub_item[k] of the batch's
+           whole set (NULL: the framing lists the whole set) */
+        const unsigned long long *sub_item = nullptr;
     } ch;
     /* regk_read_results (regk_results.cuh): what each write framing framed (one record per source, four for the
        reconcile ops), and the last read's chain, per-frame and per-entry arrays and lists */
@@ -307,6 +311,24 @@ struct regk_ctx {
         DevBuf ptotals, pcount, item[2], prec[2], plen[2], pbytes, poff;
         FrameBufs frames;
     } evq;
+    /* the watches the session holds (regk_setwatches.cuh), for batch generation `gen`: the kind each watched read armed
+       per record and per directory of evq's set, whether the last exists / getChildren framing carried the watch byte
+       and whether its replies are still unread (in flight), and regk_read_events' SetWatches gate.  zxid: the session's
+       high-water mark, kept for the context's whole life.  The framing's working arrays and frames. */
+    struct Watch {
+        uint64_t gen = 0;
+        DevBuf rec_kind, dir_kind;
+        uint64_t rec_n = 0, dir_d = 0;          /* kinds held for this generation; 0: none yet (all NONE) */
+        bool ex_watch = false, ch_watch = false;
+        bool ex_fly = false, ch_fly = false;
+        bool gate = false;
+        bool lmax_ok = false;
+        uint32_t lmax = 0;                      /* the batch's longest path */
+        long long zxid = 0;
+        DevBuf zmax, lmax_d, cls, totals, count, ent_src, ent_s, ent_len;
+        FrameBufs frames;
+        Event ev[2];
+    } wq;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     struct Skip {
@@ -2495,6 +2517,103 @@ int regk_service_records(regk_ctx *ctx, const regk_service_batch *b, regk_result
     return REGK_OK;
 }
 
+/* The watch state of the batch finished last: a new batch generation starts with no kinds, nothing in flight and the
+   SetWatches gate closed (the zxid high-water mark stays). */
+static regk_ctx::Watch &watch_state(regk_ctx *ctx)
+{
+    regk_ctx::Watch &w = ctx->wq;
+    if (w.gen != ctx->last.gen) {
+        w.gen = ctx->last.gen;
+        w.rec_n = w.dir_d = 0;
+        w.ex_watch = w.ch_watch = w.ex_fly = w.ch_fly = w.gate = w.lmax_ok = false;
+    }
+    return w;
+}
+
+/* the kinds of the generation's `count` records (dirs == false) or directories, all NONE when first asked for */
+static int watch_kinds(regk_ctx *ctx, bool dirs, uint64_t count, uint8_t **kind)
+{
+    regk_ctx::Watch &w = watch_state(ctx);
+    DevBuf &b = dirs ? w.dir_kind : w.rec_kind;
+    uint64_t &have = dirs ? w.dir_d : w.rec_n;
+    if (have != count || !b.p) {
+        const int rc = ensure_dev(ctx, b, count + 16);
+        if (rc)
+            return rc;
+        CK(cudaMemsetAsync(b.p, 0, count + 16, ctx->stream));
+        have = count;
+    }
+    *kind = (uint8_t *)b.p;
+    return REGK_OK;
+}
+
+/* The items of the last watched exists (dirs == false) or getChildren framing, if its replies are unread, are in
+   flight: their kinds become NONE (a subset's items, or every kind when the framing's list is gone).  Called before a
+   framing overwrites that list, and by regk_setwatches_requests; *launches (if given) counts the launch. */
+static int watch_forget_unread(regk_ctx *ctx, bool dirs, uint32_t *launches)
+{
+    regk_ctx::Watch &w = watch_state(ctx);
+    bool &fly = dirs ? w.ch_fly : w.ex_fly;
+    const uint64_t have = dirs ? w.dir_d : w.rec_n;
+    if (!fly || !have) {
+        fly = false;
+        return REGK_OK;
+    }
+    uint8_t *kind = (uint8_t *)(dirs ? w.dir_kind : w.rec_kind).p;
+    const regk_ctx::Children &ch = ctx->ch;
+    const unsigned long long *items = nullptr;
+    uint64_t m = 0;
+    if (!dirs && ctx->ex_valid && ctx->ex_gen == ctx->last.gen && ctx->ex_sub) {
+        items = ctx->ex_rec;
+        m = ctx->ex_n;
+    } else if (dirs && ch.framed && ch.gen == ctx->last.gen && ch.sub_item) {
+        items = ch.sub_item;
+        m = ch.d;
+    } else {
+        CK(cudaMemsetAsync(kind, 0, have, ctx->stream));
+    }
+    if (items && m) {
+        regk_watch_forget_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(items, m, kind);
+        CK(cudaGetLastError());
+        if (launches)
+            ++*launches;
+    }
+    fly = false;
+    return REGK_OK;
+}
+
+/* an exists (dirs == false) or getChildren framing was made, with the watch byte or without */
+static int watch_framed(regk_ctx *ctx, bool dirs, bool watched)
+{
+    const int rc = watch_forget_unread(ctx, dirs, nullptr);
+    if (rc)
+        return rc;
+    regk_ctx::Watch &w = ctx->wq;
+    (dirs ? w.ch_watch : w.ex_watch) = watched;
+    (dirs ? w.ch_fly : w.ex_fly) = watched;
+    return REGK_OK;
+}
+
+/* a read of the last exists / getChildren framing succeeded: with the watch byte, reply k (err[k], k < m) gives item
+   sub[k] (or k) of the generation's `count` its kind.  The launch is the bookkeeping's, not the read's. */
+static int watch_read(regk_ctx *ctx, bool dirs, const int32_t *err, uint64_t m, const unsigned long long *sub, uint64_t count)
+{
+    regk_ctx::Watch &w = watch_state(ctx);
+    if (!(dirs ? w.ch_watch : w.ex_watch))
+        return REGK_OK;
+    uint8_t *kind = nullptr;
+    const int rc = watch_kinds(ctx, dirs, count, &kind);
+    if (rc)
+        return rc;
+    if (m) {
+        const WatchKindParams kp{m, err, sub, kind, dirs};
+        regk_watch_kind_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(kp);
+        CK(cudaGetLastError());
+    }
+    (dirs ? w.ch_fly : w.ex_fly) = false;
+    return REGK_OK;
+}
+
 int regk_jute_frames(regk_ctx *ctx, uint32_t flags, int32_t xid_base, uint32_t zk_flags, regk_frames *out)
 {
     regk_jute_opts o{};
@@ -2532,7 +2651,10 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
             need_json ? "both a path and a payload stream" : "a path stream");
     const FrameSrc src{ctx->last.n, ctx->last.path_bytes, ctx->last.path_off, has_data ? ctx->last.json_bytes : nullptr,
                        has_data ? ctx->last.json_off : nullptr};
-    const int rc = frame_requests(ctx, src, o, ctx->frames, out);
+    int rc = exists ? watch_forget_unread(ctx, false, nullptr) : REGK_OK;
+    if (rc)
+        return rc;
+    rc = frame_requests(ctx, src, o, ctx->frames, out);
     if (rc == REGK_OK && getdata) {
         ctx->gd_valid = true;
         ctx->gd_gen = ctx->last.gen;
@@ -2544,6 +2666,7 @@ int regk_jute_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *out)
         ctx->ex_xid = o->xid_base;
         ctx->ex_n = ctx->last.n;
         ctx->ex_sub = false;
+        rc = watch_framed(ctx, false, o->flags & REGK_ZK_WATCH);
     } else if (rc == REGK_OK) {
         record_framing(ctx->rs.batch, src, o, o->op, o->group != 0, out->n, nullptr, ctx->last.gen);
     }
@@ -3780,8 +3903,10 @@ int regk_children_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *
     if (ctx->last.n >= 0xFFFFFFFEull)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_children_requests: batch too large");
     CK(cudaSetDevice(ctx->device));
-    ch.framed = false;
     int rc;
+    if ((rc = watch_forget_unread(ctx, true, nullptr)))
+        return rc;
+    ch.framed = false;
     if ((rc = children_dirs(ctx, ch, true)))
         return rc;
     FrameSrc src{ch.d, (const uint8_t *)ch.dbytes.p, (const unsigned long long *)ch.doff.p, nullptr, nullptr};
@@ -3795,7 +3920,8 @@ int regk_children_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *
     ch.keep_drec = (const unsigned long long *)ch.drec.p;
     ch.keep_dlen = (const uint32_t *)ch.dlen.p;
     ch.keep_d = ch.d;
-    return REGK_OK;
+    ch.sub_item = nullptr;
+    return watch_framed(ctx, true, o->flags & REGK_ZK_WATCH);
 }
 
 static const char *children_reason(uint32_t code)
@@ -4221,6 +4347,8 @@ int regk_read_children(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64
         }
         CK(cudaStreamSynchronize(s));
     }
+    if ((rc = watch_read(ctx, true, (const int32_t *)ch.err.p, d, ch.sub_item, ch.keep_d)))
+        return rc;
     ch.read = true;
     ch.n_stale = n_stale;
     out->n_dirs = d;
@@ -4714,6 +4842,8 @@ int regk_read_stats(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t 
             CK(cudaMemcpyAsync(sq.sub_rec.p, ctx->ex_rec, n * 8, cudaMemcpyDeviceToDevice, s));
         CK(cudaStreamSynchronize(s));
     }
+    if ((rc = watch_read(ctx, false, (const int32_t *)sq.err.p, n, ctx->ex_sub ? ctx->ex_rec : nullptr, ctx->last.n)))
+        return rc;
     sq.read = true;
     sq.gen = ctx->last.gen;
     sq.n = n;
@@ -4847,6 +4977,8 @@ static const char *events_reason(uint32_t code)
     case EV_NOTE_ERR: return "a notification with err != 0";
     case EV_TYPE: return "a notification whose type is outside -1 .. 7";
     case EV_PING_BODY: return "a ping with a body";
+    case EV_SW_BODY: return "a SetWatches reply (xid -8) with a body";
+    case EV_SW_ERR: return "a SetWatches reply (xid -8) with err != 0";
     default: return "internal error";
     }
 }
@@ -4957,6 +5089,10 @@ int regk_read_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
     for (Event &e : ev.ev)
         if ((rc = ensure_event(ctx, e)))
             return rc;
+    regk_ctx::Watch &wq = watch_state(ctx);
+    const bool sw = wq.gate;                    /* SetWatches replies are frames of the stream */
+    if ((rc = ensure_dev(ctx, wq.zmax, 16)))
+        return rc;
     const uint8_t *ds = bytes;
     if (!in_dev && len) {
         if ((rc = stage_in(ctx, ev.stream, bytes, len, s)))
@@ -5002,7 +5138,10 @@ int regk_read_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
     /* 1. the frame chain from `start` and where it stops */
     RepParams pf = p;
     if (len > start) {
-        regk_events_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(ep);
+        if (sw)
+            regk_events_sw_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(ep);
+        else
+            regk_events_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(ep);
         CK(cudaGetLastError());
         launches++;
         uint32_t *J = nullptr;
@@ -5028,7 +5167,8 @@ int regk_read_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
         CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         EvHead h;
-        const uint32_t code = ev_head(head, avail, xb, nx, &h);   /* reads at most 32 bytes, all of them in head */
+        /* reads at most 32 bytes, all of them in head */
+        const uint32_t code = sw ? ev_sw_head(head, avail, xb, nx, &h) : ev_head(head, avail, xb, nx, &h);
         if (code != EV_TRUNC)
             return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_events: byte %llu: %s (len %d, xid %d)", (unsigned long long)stop,
                 code ? events_reason(code) : "internal error", h.len, h.xid);
@@ -5055,14 +5195,19 @@ int regk_read_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
         ep.tile_total = (uint32_t *)ev.ntotals.p;
         ep.super_total = (unsigned long long *)((uint8_t *)ev.ntotals.p + align16(tiles_c * 4));
         CK(cudaMemsetAsync(ev.ntotals.p, 0, t2, s));
+        CK(cudaMemsetAsync(wq.zmax.p, 0, 8, s));
         regk_events_count_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(ep);
         regk_events_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(ep);
+        regk_events_zxid_kernel<<<(unsigned)((C + 255) / 256), 256, 0, s>>>(pf, (long long *)wq.zmax.p);
         CK(cudaGetLastError());
-        launches += 2;
+        launches += 3;
     }
     CK(cudaEventRecord(ev.ev[1], s));
     CK(cudaMemcpyAsync(hc, p.counters, EQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(hc + EQ_NCOUNTERS, ev.dirty.p, 16, cudaMemcpyDeviceToHost, s));
+    long long zmax = 0;
+    if (C)
+        CK(cudaMemcpyAsync(&zmax, wq.zmax.p, 8, cudaMemcpyDeviceToHost, s));
     if ((rc = sync_or_fail(ctx, s, who)))
         return rc;
     const uint64_t ne = C ? hc[EQ_NEV] : 0;
@@ -5080,6 +5225,7 @@ int regk_read_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
         CK(cudaStreamSynchronize(s));
     }
     ev.read = true;
+    wq.zxid = std::max(wq.zxid, zmax);
     out->n_events = ne;
     out->n_pings = hc[EQ_PING];
     out->n_replies = hc[EQ_REPLY];
@@ -5171,6 +5317,8 @@ int regk_events_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *ou
     uint64_t m = 0, total = 0;
     uint32_t launches = 0;
     const int w = exists ? 0 : 1;
+    if ((rc = watch_forget_unread(ctx, !exists, nullptr)))
+        return rc;
     if ((rc = events_pending(ctx, !exists, &m, &launches, who)))
         return rc;
     regk_jute_opts oo = *o;
@@ -5192,6 +5340,8 @@ int regk_events_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *ou
         ctx->ex_sub = true;
         ctx->ex_rec = (const unsigned long long *)ev.item[w].p;
         ev.rec_epoch++;
+        if ((rc = watch_framed(ctx, false, true)))
+            return rc;
     } else {
         regk_ctx::Children &ch = ctx->ch;
         ch.framed = false;
@@ -5218,11 +5368,216 @@ int regk_events_requests(regk_ctx *ctx, const regk_jute_opts *o, regk_frames *ou
         ch.keep_drec = (const unsigned long long *)ev.drec.p;
         ch.keep_dlen = (const uint32_t *)ev.dlen.p;
         ch.keep_d = ev.d;
+        ch.sub_item = (const unsigned long long *)ev.item[w].p;
         ev.dir_epoch++;
+        if ((rc = watch_framed(ctx, true, true)))
+            return rc;
     }
     CK(cudaMemsetAsync((unsigned long long *)ev.dirty.p + w, 0, 8, s));
     CK(cudaStreamSynchronize(s));
     out->launches += launches;
+    return REGK_OK;
+}
+
+int regk_setwatches_requests(regk_ctx *ctx, const regk_setwatches_opts *o, regk_setwatches *out)
+{
+    const char *who = "regk_setwatches_requests";
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_setwatches_requests: NULL argument");
+    memset(out, 0, sizeof *out);
+    if (o->flags & ~(uint32_t)REGK_OUT_DEVICE)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_setwatches_requests: unknown flag bits 0x%x (only REGK_OUT_DEVICE)",
+            o->flags & ~(uint32_t)REGK_OUT_DEVICE);
+    if (o->max_frame >= 0x80000000u)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_setwatches_requests: max_frame %u is 2^31 or more; a frame's length is "
+                                               "a signed 32-bit int", o->max_frame);
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "regk_setwatches_requests: batches are still in flight; finish them first");
+    if (!ctx->last.path_off || !ctx->last.path_bytes)
+        return fail(ctx, REGK_ERR_STATE, "regk_setwatches_requests: no finished batch with a path stream on this context: the "
+                                         "watches are the ones its reads armed");
+    if (ctx->last.n >= 0xFFFFFFFEull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_setwatches_requests: batch too large");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    regk_ctx::Events &ev = ctx->evq;
+    int rc;
+    if (!ev.built || ev.gen != ctx->last.gen) {
+        if ((rc = events_build(ctx, who)))
+            return rc;
+    }
+    regk_ctx::Watch &w = watch_state(ctx);
+    for (Event &e : w.ev)
+        if ((rc = ensure_event(ctx, e)))
+            return rc;
+    const uint64_t n = ctx->last.n, d = ev.d;
+    uint32_t launches = 0;
+    /* 1. the split's bound: the longest path, once per batch generation */
+    if (!w.lmax_ok) {
+        if ((rc = ensure_dev(ctx, w.lmax_d, 16)))
+            return rc;
+        CK(cudaMemsetAsync(w.lmax_d.p, 0, 4, s));
+        if (n) {
+            regk_sw_lmax_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(ctx->last.path_off, n, (uint32_t *)w.lmax_d.p);
+            CK(cudaGetLastError());
+            launches++;
+        }
+        uint32_t lm = 0;
+        CK(cudaMemcpyAsync(&lm, w.lmax_d.p, 4, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        w.lmax = lm;
+        w.lmax_ok = true;
+    }
+    const uint64_t Lmax = 4ull + w.lmax, mf = o->max_frame ? o->max_frame : 131072u;
+    if (mf < SW_OVERHEAD + 2 * Lmax)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_setwatches_requests: max_frame %llu is below this batch's minimum of %llu "
+                                               "(32 + 2 x (4 + its longest path, %u bytes))", (unsigned long long)mf,
+                    (unsigned long long)(SW_OVERHEAD + 2 * Lmax), w.lmax);
+    const uint64_t B = mf - SW_OVERHEAD - Lmax;
+    /* 2. what is in flight counts as NONE */
+    uint8_t *rk = nullptr, *dk = nullptr;
+    if ((rc = watch_kinds(ctx, false, n, &rk)) || (rc = watch_kinds(ctx, true, d, &dk)))
+        return rc;
+    if ((rc = watch_forget_unread(ctx, false, &launches)) || (rc = watch_forget_unread(ctx, true, &launches)))
+        return rc;
+    /* 3. classify: the lists, the re-pend marks, per-tile counts and bytes */
+    const uint64_t tiles_r = (n + RP_TILE - 1) / RP_TILE, tiles_d = (d + RP_TILE - 1) / RP_TILE;
+    const size_t reg_r = align16(tiles_r * 4) + (tiles_r / SUPER + 1) * 8, reg_d = align16(tiles_d * 4) + (tiles_d / SUPER + 1) * 8;
+    const size_t totals_bytes = 4 * reg_r + 2 * reg_d;
+    if ((rc = ensure_dev(ctx, w.totals, totals_bytes)) || (rc = ensure_dev(ctx, w.count, SWQ_N * 8 + 16)) ||
+        (rc = ensure_dev(ctx, w.cls, n + d + 16)))
+        return rc;
+    SwParams sp{};
+    sp.n = n;
+    sp.d = d;
+    sp.tiles_r = (uint32_t)tiles_r;
+    sp.path_off = ctx->last.path_off;
+    sp.slot = (const uint32_t *)ev.slot.p;
+    sp.t_rec = (const uint32_t *)ev.t_rec.p;
+    sp.dir_rec = (const unsigned long long *)ev.drec.p;
+    sp.dir_len = (const uint32_t *)ev.dlen.p;
+    sp.rec_kind = rk;
+    sp.dir_kind = dk;
+    sp.rec_mark = (uint32_t *)ev.rec_mark.p;
+    sp.dir_mark = (uint32_t *)ev.dir_mark.p;
+    sp.rec_epoch = ev.rec_epoch;
+    sp.dir_epoch = ev.dir_epoch;
+    sp.dirty = (unsigned long long *)ev.dirty.p;
+    sp.counters = (unsigned long long *)w.count.p;
+    sp.cls = (uint8_t *)w.cls.p;
+    {
+        uint8_t *t = (uint8_t *)w.totals.p;
+        for (int k = 0; k < SWT_N; k++) {
+            const bool dr = k >= SWT_CC;
+            const uint64_t tiles = dr ? tiles_d : tiles_r;
+            sp.tt[k] = (uint32_t *)t;
+            sp.st[k] = (unsigned long long *)(t + align16(tiles * 4));
+            t += dr ? reg_d : reg_r;
+        }
+    }
+    CK(cudaMemsetAsync(w.totals.p, 0, totals_bytes, s));
+    CK(cudaMemsetAsync(w.count.p, 0, SWQ_N * 8, s));
+    CK(cudaEventRecord(w.ev[0], s));
+    const unsigned grid = (unsigned)(tiles_r + tiles_d);
+    if (grid) {
+        regk_sw_classify_kernel<<<grid, RP_TILE, 0, s>>>(sp);
+        CK(cudaGetLastError());
+        launches++;
+    }
+    uint64_t sums[SWT_N] = {};
+    std::vector<unsigned long long> sup(4 * (tiles_r / SUPER + 1) + 2 * (tiles_d / SUPER + 1));
+    for (int k = 0, at = 0; k < SWT_N; k++) {
+        const uint64_t ns = (k >= SWT_CC ? tiles_d : tiles_r) / SUPER + 1;
+        CK(cudaMemcpyAsync(sup.data() + at, sp.st[k], ns * 8, cudaMemcpyDeviceToHost, s));
+        at += (int)ns;
+    }
+    unsigned long long hq[SWQ_N + 2] = {};
+    CK(cudaMemcpyAsync(hq, w.count.p, SWQ_N * 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(hq + SWQ_N, ev.dirty.p, 16, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    for (int k = 0, at = 0; k < SWT_N; k++) {
+        const uint64_t ns = (k >= SWT_CC ? tiles_d : tiles_r) / SUPER + 1;
+        for (uint64_t q = 0; q < ns; q++)
+            sums[k] += sup[at + q];
+        at += (int)ns;
+    }
+    const uint64_t nD = sums[SWT_DC], nE = sums[SWT_EC], nC = sums[SWT_CC], m = nD + nE + nC;
+    const uint64_t total_s = sums[SWT_DB] + sums[SWT_EB] + sums[SWT_CB];
+    /* 4. place: entry j's path, length and prefix s_j */
+    if ((rc = ensure_dev(ctx, w.ent_src, m * 8 + 16)) || (rc = ensure_dev(ctx, w.ent_s, m * 8 + 16)) ||
+        (rc = ensure_dev(ctx, w.ent_len, m * 4 + 16)))
+        return rc;
+    sp.nD = nD;
+    sp.nE = nE;
+    sp.m = m;
+    sp.bD = sums[SWT_DB];
+    sp.bE = sums[SWT_EB];
+    sp.total_s = total_s;
+    sp.B = B;
+    sp.zxid = w.zxid;
+    sp.ent_src = (unsigned long long *)w.ent_src.p;
+    sp.ent_s = (unsigned long long *)w.ent_s.p;
+    sp.ent_len = (uint32_t *)w.ent_len.p;
+    sp.path_bytes = ctx->last.path_bytes;
+    uint64_t F = 0;
+    if (m) {
+        regk_sw_place_kernel<<<grid, RP_TILE, 0, s>>>(sp);
+        CK(cudaGetLastError());
+        launches++;
+        unsigned long long last_s = 0;
+        CK(cudaMemcpyAsync(&last_s, sp.ent_s + (m - 1), 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        F = last_s / B + 1;
+    }
+    /* 5. the frames: entries, then headers and count words over the bytes between them */
+    const uint64_t total = SW_OVERHEAD * F + total_s;
+    FrameBufs &fb = w.frames;
+    if ((rc = ensure_dev(ctx, fb.bytes, total + 16)) || (rc = ensure_dev(ctx, fb.off, (F + 1) * 8)))
+        return rc;
+    sp.out = (uint8_t *)fb.bytes.p;
+    sp.frame_off = (unsigned long long *)fb.off.p;
+    sp.F = F;
+    if (m) {
+        regk_sw_write_kernel<<<(unsigned)((m + RP_TILE - 1) / RP_TILE), RP_TILE, 0, s>>>(sp);
+        regk_sw_head_kernel<<<(unsigned)((F + 255) / 256), 256, 0, s>>>(sp);
+        CK(cudaGetLastError());
+        launches += 2;
+    } else {
+        CK(cudaMemsetAsync(fb.off.p, 0, 8, s));
+    }
+    CK(cudaEventRecord(w.ev[1], s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, w.ev[0], w.ev[1]);
+    const bool dev_out = o->flags & REGK_OUT_DEVICE;
+    const void *src[2] = {fb.bytes.p, fb.off.p};
+    if (!dev_out) {
+        if ((rc = to_host(ctx, fb.h_bytes, fb.bytes.p, total, s)) || (rc = to_host(ctx, fb.h_off, fb.off.p, (F + 1) * 8, s)))
+            return rc;
+        CK(cudaStreamSynchronize(s));
+        src[0] = fb.h_bytes.p;
+        src[1] = fb.h_off.p;
+    }
+    w.gate = true;
+    out->n_data = nD;
+    out->n_exist = nE;
+    out->n_child = nC;
+    out->n_repend_recs = hq[SWQ_REPEND_R];
+    out->n_repend_dirs = hq[SWQ_REPEND_D];
+    out->n_dirty_recs = hq[SWQ_N];
+    out->n_dirty_dirs = hq[SWQ_N + 1];
+    out->relative_zxid = w.zxid;
+    out->frames.n = F;
+    out->frames.total = total;
+    out->frames.flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->frames.launches = launches;
+    out->frames.frame_bytes = (const uint8_t *)src[0];
+    out->frames.frame_off = (const uint64_t *)src[1];
+    out->frames.kernel_ms = ms;
     return REGK_OK;
 }
 
