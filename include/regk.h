@@ -1094,6 +1094,77 @@ typedef struct regk_setwatches {
 
 int         regk_setwatches_requests(regk_ctx *ctx, const regk_setwatches_opts *opts, regk_setwatches *out);
 
+/*
+ * ---- what DNS answers for a registry snapshot: the A and SRV sets its host and service records define (the contract
+ * between registrar and Binder, README.md:441-755 of the reference), restricted to the canonical forms this library
+ * writes ------------------------------------------------------------------------------------------------------------
+ * Snapshot: m nodes in the layout regk_reconcile takes (host streams, or device streams with REGK_IN_DEVICE, e.g.
+ * regk_replies.snapshot as it stands); host_nodes is ignored; REGK_DECODE_LAST, unknown opts->flags bits, a nonzero
+ * reserved, a negative default TTL and m >= 2^32 - 1 are REGK_ERR_INVALID_ARG.  A device snapshot's offsets are checked
+ * as regk_reconcile checks them, and two nodes with one path are refused as there (the message names the later node).
+ *   name(j)   node j's path components reversed and joined by '.' (regk_decode's domain with host_nodes = 0):
+ *             /us/joyent/example/b44c74d6 -> b44c74d6.example.joyent.us.  Valid: every label 1-63 bytes of
+ *             [A-Za-z0-9_-], at most 253 bytes.  A service record's SRV owner <srvce>.<proto>.name(s) (srvce and proto
+ *             verbatim, README.md:432) must be valid too.
+ *   node_cls  the first failing rule decides, in the order of REGK_RSV_* below.  Type tables (README.md:274-282,
+ *             type bytes compared raw): queryable db_host host load_balancer moray_host redis_host; usable for a
+ *             service load_balancer moray_host ops_host redis_host rr_host.
+ *   children  a host record c of class OK and a usable type is a child of service node s when dirname(path(c)) is
+ *             s's path byte for byte and s is a service record of class OK; children in ascending node order.
+ *   TTLs      a_ttl(c) = c's ttl, else default_host_ttl; srv_ttl(s) = s's service.service.ttl, else default_srv_ttl
+ *             (README.md:670-755; in canonical form only the innermost ttl exists).
+ * Queries, in ascending node order (a service's A query before its SRV query):
+ *   REGK_Q_HOST_A       every OK host record of a queryable type: name(c). a_ttl(c) IN A addr(c)
+ *   REGK_Q_SERVICE_A    every OK service record, with or without children: per child
+ *                       name(s). min(srv_ttl(s), a_ttl(c)) IN A addr(c)
+ *   REGK_Q_SERVICE_SRV  per child, per port of its ports in payload order ([port(s)] without a ports key):
+ *                       <srvce>.<proto>.name(s). srv_ttl(s) IN SRV 0 10 port name(c).  (README.md:432,705); additional:
+ *                       per child with >= 1 SRV answer, name(c). a_ttl(c) IN A addr(c).  ports: [] gives neither.
+ * Text: one record per line, LF-terminated; owner, TTL, IN, type and rdata separated by one TAB, SRV rdata fields by
+ * one space: dig's presentation format with single tabs.
+ * Results are pinned host arrays, or device arrays with REGK_OUT_DEVICE; valid until the next regk_resolve call.
+ * launches counts the radix sort that groups the children as one; kernel_ms spans every pass but the host's reads.
+ * PARITY UNPINNED: Binder's default TTLs are parameters (the README's SRV example implies a host default of 30:
+ * README.md:383-392 sets no ttl and :433 shows 30); Binder's answer order; a service record with a middle-level ttl
+ * (the README's authcache example, :511-523) is not a form this library writes and is REGK_RSV_NOT_RECORD here.
+ */
+typedef struct regk_resolve_opts {
+    uint32_t flags;                 /* REGK_OUT_DEVICE */
+    int32_t  default_host_ttl;      /* A TTL of a host record without "ttl" (>= 0) */
+    int32_t  default_srv_ttl;       /* SRV TTL of a service record without "ttl" (>= 0) */
+    uint32_t reserved;              /* 0 */
+} regk_resolve_opts;
+
+#define REGK_Q_HOST_A      1u       /* A    <name of node>                 */
+#define REGK_Q_SERVICE_A   2u       /* A    <name of service node>         */
+#define REGK_Q_SERVICE_SRV 3u       /* SRV  <srvce>.<proto>.<service name> */
+
+#define REGK_RSV_OK           0u    /* node_cls[]; first failing rule decides, in this order: */
+#define REGK_RSV_EMPTY        1u    /* empty data: a directory node; answers nothing; not listed */
+#define REGK_RSV_NOT_RECORD   2u    /* regk_decode found no canonical host or service record, or a bad path */
+#define REGK_RSV_BAD_NAME     3u    /* a DNS name it would own is not a valid name */
+#define REGK_RSV_UNKNOWN_TYPE 4u    /* host record whose type bytes are not one of the README's seven */
+#define REGK_RSV_BAD_ADDRESS  5u    /* host record address not a dotted-quad IPv4 (no leading zeros) */
+#define REGK_RSV_BAD_TTL      6u    /* ttl < 0 */
+#define REGK_RSV_BAD_PORT     7u    /* a port > 65535 (host ports, or the service's port) */
+
+typedef struct regk_answers {
+    uint64_t m;                     /* snapshot nodes */
+    uint64_t n_queries, n_answers, n_additional, n_unresolved;
+    uint64_t text_total;
+    uint32_t flags, launches;
+    const uint8_t  *q_kind;         /* [n_queries] REGK_Q_* */
+    const uint64_t *q_node;         /* [n_queries] snapshot node whose name is asked, ascending */
+    const uint64_t *sec_off;        /* [2 n_queries + 1]: answer section of q = text[sec_off[2q], sec_off[2q+1]),
+                                       additional section = text[sec_off[2q+1], sec_off[2q+2]) */
+    const uint8_t  *text;           /* [text_total] */
+    const uint8_t  *node_cls;       /* [m] REGK_RSV_* */
+    const uint64_t *unresolved;     /* [n_unresolved] ascending nodes with class >= REGK_RSV_NOT_RECORD */
+    float kernel_ms;
+} regk_answers;
+
+int         regk_resolve(regk_ctx *ctx, const regk_decode_in *snapshot, const regk_resolve_opts *opts, regk_answers *out);
+
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);
 int64_t     regk_get_option(const regk_ctx *ctx, const char *name);

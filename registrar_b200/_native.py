@@ -467,6 +467,49 @@ class SetWatches:
         return out
 
 
+class CResolveOpts(C.Structure):     # regk_resolve_opts
+    _fields_ = [("flags", C.c_uint32), ("default_host_ttl", C.c_int32), ("default_srv_ttl", C.c_int32),
+                ("reserved", C.c_uint32)]
+
+
+class CAnswers(C.Structure):         # regk_answers
+    _fields_ = [("m", C.c_uint64), ("n_queries", C.c_uint64), ("n_answers", C.c_uint64), ("n_additional", C.c_uint64),
+                ("n_unresolved", C.c_uint64), ("text_total", C.c_uint64), ("flags", C.c_uint32), ("launches", C.c_uint32),
+                ("q_kind", C.c_void_p), ("q_node", C.c_void_p), ("sec_off", C.c_void_p), ("text", C.c_void_p),
+                ("node_cls", C.c_void_p), ("unresolved", C.c_void_p), ("kernel_ms", C.c_float)]
+
+
+Q_HOST_A, Q_SERVICE_A, Q_SERVICE_SRV = 1, 2, 3                       # Answers.q_kind
+(RSV_OK, RSV_EMPTY, RSV_NOT_RECORD, RSV_BAD_NAME, RSV_UNKNOWN_TYPE, RSV_BAD_ADDRESS, RSV_BAD_TTL,
+ RSV_BAD_PORT) = range(8)                                            # Answers.node_cls
+
+
+class Answers:
+    """Host copy of a regk_answers: what DNS answers for a snapshot.  Query q asks q_kind[q] (Q_HOST_A, Q_SERVICE_A,
+    Q_SERVICE_SRV) for the name of snapshot node q_node[q]; answer(q) / additional(q) are its sections as
+    LF-terminated, tab-separated presentation lines.  node_cls[j] is RSV_* of node j, unresolved the ascending nodes of
+    class RSV_NOT_RECORD or worse."""
+
+    def __init__(self, out):
+        self.m, self.n_queries = int(out.m), int(out.n_queries)
+        self.n_answers, self.n_additional = int(out.n_answers), int(out.n_additional)
+        self.n_unresolved, self.text_total = int(out.n_unresolved), int(out.text_total)
+        self.launches, self.kernel_ms = int(out.launches), float(out.kernel_ms)
+        nq = self.n_queries
+        self.q_kind = _as_np(out.q_kind, nq, np.uint8).copy()
+        self.q_node = _as_np(out.q_node, nq, np.uint64).copy()
+        self.sec_off = _as_np(out.sec_off, 2 * nq + 1, np.uint64).copy()
+        self.text = _as_np(out.text, self.text_total, np.uint8).copy()
+        self.node_cls = _as_np(out.node_cls, self.m, np.uint8).copy()
+        self.unresolved = _as_np(out.unresolved, self.n_unresolved, np.uint64).copy()
+
+    def answer(self, q: int) -> bytes:
+        return self.text[int(self.sec_off[2 * q]):int(self.sec_off[2 * q + 1])].tobytes()
+
+    def additional(self, q: int) -> bytes:
+        return self.text[int(self.sec_off[2 * q + 1]):int(self.sec_off[2 * q + 2])].tobytes()
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -481,7 +524,7 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned",
            "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results", "regk_read_stats",
            "regk_reconcile_stats", "regk_read_events", "regk_events_requests",
-           "regk_setwatches_requests"]
+           "regk_setwatches_requests", "regk_resolve"]
 
 _lib = None
 
@@ -547,6 +590,7 @@ def load_library():
     lib.regk_read_events.argtypes = [vp, vp, u64, u64, C.POINTER(CEventsOpts), C.POINTER(CEvents)]
     lib.regk_events_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     lib.regk_setwatches_requests.argtypes = [vp, C.POINTER(CSetWatchesOpts), C.POINTER(CSetWatches)]
+    lib.regk_resolve.argtypes = [vp, C.POINTER(CDecodeIn), C.POINTER(CResolveOpts), C.POINTER(CAnswers)]
     _lib = lib
     return lib
 
@@ -1119,6 +1163,19 @@ class Context:
         out = CSetWatches()
         self._check(self._lib.regk_setwatches_requests(self._h, C.byref(o), C.byref(out)))
         return out if device else SetWatches(out)
+
+    # -- what DNS answers for a snapshot --
+    def resolve(self, snapshot, default_host_ttl: int, default_srv_ttl: int, device: bool = False):
+        """regk_resolve: the A and SRV answers the host and service records of `snapshot` define (a batch.Snapshot,
+        host or CUDA, or anything with cdecode_in(), such as a Replies).  Returns an Answers, or the raw CAnswers
+        (device pointers) with device=True."""
+        cin, keep = snapshot.cdecode_in()
+        o = CResolveOpts(FLAG_OUT_DEVICE if device else 0, int(default_host_ttl), int(default_srv_ttl), 0)
+        out = CAnswers()
+        rc = self._lib.regk_resolve(self._h, C.byref(cin), C.byref(o), C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else Answers(out)
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

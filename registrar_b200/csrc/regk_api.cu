@@ -7,6 +7,7 @@
  * implementation of the path in this library.
  */
 #include <cuda_runtime.h>
+#include <cub/device/device_radix_sort.cuh>
 
 #include <algorithm>
 #include <cstdarg>
@@ -38,6 +39,7 @@
 #include "regk_stats.cuh"
 #include "regk_events.cuh"
 #include "regk_setwatches.cuh"
+#include "regk_resolve.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -329,6 +331,14 @@ struct regk_ctx {
         FrameBufs frames;
         Event ev[2];
     } wq;
+    /* regk_resolve (regk_resolve.cuh): staged snapshot, table, decode outputs, per-node and per-child arrays, sort
+       buffers, totals, the answers and their pinned copies */
+    struct Resolve {
+        DevBuf in[4], table, slot, hash, rec, dom, ports, cls, roles, ttl, key, val, skey, sval, first, end, cum[3], totals,
+            count, node_q, q_kind, q_node, sec_off, unres, text, sort_tmp;
+        HostBuf h_count, h_q_kind, h_q_node, h_sec_off, h_text, h_cls, h_unres;
+        Event ev[5];
+    } rsv;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     struct Skip {
@@ -5578,6 +5588,266 @@ int regk_setwatches_requests(regk_ctx *ctx, const regk_setwatches_opts *o, regk_
     out->frames.frame_bytes = (const uint8_t *)src[0];
     out->frames.frame_off = (const uint64_t *)src[1];
     out->frames.kernel_ms = ms;
+    return REGK_OK;
+}
+
+int regk_resolve(regk_ctx *ctx, const regk_decode_in *in, const regk_resolve_opts *o, regk_answers *out)
+{
+    const char *who = "regk_resolve";
+    if (!ctx || !in || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_resolve: NULL argument");
+    memset(out, 0, sizeof *out);
+    if (in->flags & REGK_DECODE_LAST)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams", who);
+    if (o->flags & ~REGK_OUT_DEVICE)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: unknown flag bits 0x%x", who, o->flags & ~REGK_OUT_DEVICE);
+    if (o->reserved)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: reserved must be 0", who);
+    if (o->default_host_ttl < 0 || o->default_srv_ttl < 0)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: default TTLs must be >= 0 (host %d, srv %d)", who, o->default_host_ttl,
+            o->default_srv_ttl);
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "%s: batches are still in flight; finish them first", who);
+    const uint64_t m = in->n;
+    if (m >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: %llu nodes: must be below 2^32 - 1", who, (unsigned long long)m);
+    const bool in_dev = in->flags & REGK_IN_DEVICE, dev_out = o->flags & REGK_OUT_DEVICE;
+    const uint8_t *pb = in->path_bytes, *jb = in->json_bytes;
+    const uint64_t *po = in->path_off, *jo = in->json_off;
+    uint64_t path_total = m ? in->path_total : 0, json_total = m ? in->json_total : 0;
+    if (m && (!po || !jo))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: a snapshot of %llu nodes needs path and data offsets", who, (unsigned long long)m);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    regk_ctx::Resolve &rb = ctx->rsv;
+    int rc;
+    if (m && !in_dev) {
+        path_total = po[m];
+        json_total = jo[m];
+        /* offsets become memory ranges in the kernels: monotone, each node below 4 GiB, ending at the totals */
+        for (uint64_t j = 0; j < m; j++)
+            if (po[j] > po[j + 1] || jo[j] > jo[j + 1] || po[j + 1] - po[j] > 0xFFFFFFFFull || jo[j + 1] - jo[j] > 0xFFFFFFFFull)
+                return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets are not monotone at node %llu", who, (unsigned long long)j);
+        if ((path_total && !pb) || (json_total && !jb))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets without bytes", who);
+        const void *src[4] = {pb, po, jb, jo};
+        const size_t sz[4] = {(size_t)path_total, (size_t)(m + 1) * 8, (size_t)json_total, (size_t)(m + 1) * 8};
+        for (int k = 0; k < 4; k++)
+            if ((rc = stage_in(ctx, rb.in[k], src[k], sz[k], s)))
+                return rc;
+        pb = (const uint8_t *)rb.in[0].p;
+        po = (const uint64_t *)rb.in[1].p;
+        jb = (const uint8_t *)rb.in[2].p;
+        jo = (const uint64_t *)rb.in[3].p;
+    } else if (m) {
+        if ((path_total && !pb) || (json_total && !jb))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets without bytes", who);
+        if (((uintptr_t)pb & 3u) || ((uintptr_t)jb & 3u) || ((uintptr_t)po & 7u) || ((uintptr_t)jo & 7u))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device snapshot (bytes need 4-byte, offsets 8-byte alignment)", who);
+    }
+    /* an empty stream is never read; its kernels still get a valid pointer */
+    if ((rc = ensure_dev(ctx, rb.in[0], 16)) || (rc = ensure_dev(ctx, rb.in[2], 16)))
+        return rc;
+    if (!pb)
+        pb = (const uint8_t *)rb.in[0].p;
+    if (!jb)
+        jb = (const uint8_t *)rb.in[2].p;
+    for (Event &ev : rb.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
+    /* sizes: the table at most half full; per-node and per-position arrays; totals of both scans */
+    uint64_t slots = 1024;
+    while (slots < 2 * m)
+        slots <<= 1;
+    const uint64_t tiles = (m + RV_TILE - 1) / RV_TILE, nsup = tiles / SUPER + 1;
+    const size_t totals_bytes = 6 * (tiles + nsup) * 8;
+    const uint32_t end_bit = m ? 32u - (uint32_t)__builtin_clz((uint32_t)m) : 1u;
+    size_t sort_bytes = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const uint32_t *)nullptr,
+        (uint32_t *)nullptr, (int)std::max<uint64_t>(m, 1), 0, (int)end_bit, s));
+    if ((rc = ensure_dev(ctx, rb.table, slots * 4)) || (rc = ensure_dev(ctx, rb.slot, m * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb.hash, m * 4 + 16)) || (rc = ensure_dev(ctx, rb.rec, (m + 1) * sizeof(Decoded))) ||
+        (rc = ensure_dev(ctx, rb.dom, path_total + 16)) || (rc = ensure_dev(ctx, rb.ports, (json_total / 2 + 1) * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb.cls, m + 16)) || (rc = ensure_dev(ctx, rb.roles, m + 16)) || (rc = ensure_dev(ctx, rb.ttl, m * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb.key, m * 4 + 16)) || (rc = ensure_dev(ctx, rb.val, m * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb.skey, m * 4 + 16)) || (rc = ensure_dev(ctx, rb.sval, m * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb.first, m * 4 + 16)) || (rc = ensure_dev(ctx, rb.end, m * 4 + 16)) ||
+        (rc = ensure_dev(ctx, rb.totals, totals_bytes)) || (rc = ensure_dev(ctx, rb.count, RV_NCOUNTERS * 8)) ||
+        (rc = ensure_dev(ctx, rb.node_q, m * 8 + 16)) || (rc = ensure_dev(ctx, rb.q_kind, 2 * m + 16)) ||
+        (rc = ensure_dev(ctx, rb.q_node, 2 * m * 8 + 16)) || (rc = ensure_dev(ctx, rb.sec_off, (4 * m + 1) * 8)) ||
+        (rc = ensure_dev(ctx, rb.unres, m * 8 + 16)) || (rc = ensure_dev(ctx, rb.sort_tmp, sort_bytes + 16)) ||
+        (rc = ensure_host(ctx, rb.h_count, RV_NCOUNTERS * 8)))
+        return rc;
+    for (int k = 0; k < 3; k++)
+        if ((rc = ensure_dev(ctx, rb.cum[k], (m + 1) * 8)))
+            return rc;
+    CK(cudaMemsetAsync(rb.table.p, 0, slots * 4, s));
+    CK(cudaMemsetAsync(rb.totals.p, 0, totals_bytes, s));
+    CK(cudaMemsetAsync(rb.count.p, 0, RV_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(rb.count.p, 0xFF, 16, s));           /* no bad node, no duplicate node */
+    CK(cudaMemsetAsync(rb.first.p, 0, m * 4 + 16, s));      /* a service without children: [0, 0) */
+    CK(cudaMemsetAsync(rb.end.p, 0, m * 4 + 16, s));
+    CK(cudaMemsetAsync(rb.sec_off.p, 0, 8, s));
+    unsigned long long *hc = (unsigned long long *)rb.h_count.p;
+    uint32_t launches = 0;
+    float ms = 0, part = 0;
+    /* 1. offsets check (device snapshots) and every path into the table: regk_reconcile's insert pass */
+    ReconcileParams ip{};
+    ip.m = m;
+    ip.o_path = pb;
+    ip.o_path_off = (const unsigned long long *)po;
+    ip.o_json = jb;
+    ip.o_json_off = (const unsigned long long *)jo;
+    ip.o_path_total = path_total;
+    ip.o_json_total = json_total;
+    ip.validate = in_dev ? 1u : 0u;
+    ip.mask_o = (uint32_t)(slots - 1);
+    ip.t_obs = (uint32_t *)rb.table.p;
+    ip.slot_obs = (uint32_t *)rb.slot.p;
+    ip.hash_obs = (uint32_t *)rb.hash.p;
+    ip.counters = (unsigned long long *)rb.count.p;
+    CK(cudaEventRecord(rb.ev[0], s));
+    if (m) {
+        regk_reconcile_insert_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(ip);
+        CK(cudaGetLastError());
+        launches++;
+    }
+    CK(cudaEventRecord(rb.ev[1], s));
+    if (m && in_dev) {                                      /* the decode pass reads every node's bytes: refuse first */
+        CK(cudaMemcpyAsync(hc, rb.count.p, 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        if (hc[RV_C_BAD] != ~0ull)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot offsets are not monotone or reach past the totals at node %llu", who,
+                hc[RV_C_BAD]);
+    }
+    CK(cudaEventRecord(rb.ev[2], s));
+    ResolveParams p{};
+    p.m = m;
+    p.path = pb;
+    p.path_off = (const unsigned long long *)po;
+    p.json = jb;
+    p.json_off = (const unsigned long long *)jo;
+    p.path_total = path_total;
+    p.dec = (const Decoded *)rb.rec.p;
+    p.dom = (const uint8_t *)rb.dom.p;
+    p.ports = (const uint32_t *)rb.ports.p;
+    p.dflt_host = o->default_host_ttl;
+    p.dflt_srv = o->default_srv_ttl;
+    p.mask = (uint32_t)(slots - 1);
+    p.table = (const uint32_t *)rb.table.p;
+    p.slot = (const uint32_t *)rb.slot.p;
+    p.cls = (uint8_t *)rb.cls.p;
+    p.roles = (uint8_t *)rb.roles.p;
+    p.ttl = (int32_t *)rb.ttl.p;
+    p.key = (uint32_t *)rb.key.p;
+    p.val = (uint32_t *)rb.val.p;
+    p.skey = (const uint32_t *)rb.skey.p;
+    p.sval = (const uint32_t *)rb.sval.p;
+    p.first = (uint32_t *)rb.first.p;
+    p.end = (uint32_t *)rb.end.p;
+    unsigned long long *tb = (unsigned long long *)rb.totals.p;
+    for (int k = 0; k < 3; k++) {
+        p.cum[k] = (unsigned long long *)rb.cum[k].p;
+        p.ctile[k] = tb + (size_t)k * (tiles + nsup);
+        p.csuper[k] = p.ctile[k] + tiles;
+        p.ntile[k] = tb + (size_t)(3 + k) * (tiles + nsup);
+        p.nsuper[k] = p.ntile[k] + tiles;
+    }
+    p.node_q = (unsigned long long *)rb.node_q.p;
+    p.q_kind = (uint8_t *)rb.q_kind.p;
+    p.q_node = (unsigned long long *)rb.q_node.p;
+    p.sec_off = (unsigned long long *)rb.sec_off.p;
+    p.unresolved = (unsigned long long *)rb.unres.p;
+    p.counters = (unsigned long long *)rb.count.p;
+    if (m) {
+        /* 2. decode (host_nodes = 0): regk_decode's kernel and staging budgets */
+        DecodeParams dp{};
+        dp.n = m;
+        dp.path_bytes = pb;
+        dp.path_off = (const unsigned long long *)po;
+        dp.json_bytes = jb;
+        dp.json_off = (const unsigned long long *)jo;
+        dp.host_nodes = 0;
+        dp.out = (Decoded *)rb.rec.p;
+        dp.dom_bytes = (uint8_t *)rb.dom.p;
+        dp.ports = (uint32_t *)rb.ports.p;
+        dp.path_cap = (uint32_t)align16(std::min<uint64_t>(path_total * DEC_TILE / m * 9 / 8 + 1024, 49152));
+        dp.json_cap = (uint32_t)align16(std::min<uint64_t>(json_total * DEC_TILE / m * 9 / 8 + 1024, 65536));
+        const uint64_t slack = in_dev ? 0 : 16;             /* a caller's own device buffers end where they end */
+        dp.path_limit = path_total + slack;
+        dp.json_limit = json_total + slack;
+        const size_t dsmem = std::max<size_t>((size_t)dp.path_cap + 32, DEC_TILE * sizeof(Decoded)) + ((dp.path_cap / 8 + 47) & ~15u) +
+            std::max<size_t>(dp.json_cap, dp.path_cap) + 32 + 16;
+        if ((rc = set_smem_limit(ctx, (const void *)regk_decode_kernel, dsmem)))
+            return rc;
+        regk_decode_kernel<<<(unsigned)((m + DEC_TILE - 1) / DEC_TILE), DEC_TILE, dsmem, s>>>(dp);
+        /* 3. classify, 4. join, 5. group, 6. size and place */
+        const unsigned g256 = (unsigned)((m + 255) / 256);
+        regk_resolve_classify_kernel<<<g256, 256, 0, s>>>(p);
+        regk_resolve_join_kernel<<<g256, 256, 0, s>>>(p);
+        CK(cudaGetLastError());
+        size_t tmp = rb.sort_tmp.cap;
+        CK(cub::DeviceRadixSort::SortPairs(rb.sort_tmp.p, tmp, (const uint32_t *)p.key, (uint32_t *)rb.skey.p, (const uint32_t *)p.val,
+            (uint32_t *)rb.sval.p, (int)m, 0, (int)end_bit, s));
+        regk_resolve_child_len_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p);
+        regk_resolve_child_scan_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p);
+        regk_resolve_qlen_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p);
+        regk_resolve_place_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p);
+        CK(cudaGetLastError());
+        launches += 8;                                      /* the radix sort counted as one */
+    }
+    CK(cudaEventRecord(rb.ev[3], s));
+    CK(cudaMemcpyAsync(hc, rb.count.p, RV_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    if (m && hc[RV_C_DUP] != ~0ull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: snapshot node %llu has the path of an earlier node; a registry cannot "
+                                               "hold two nodes with one path", who, hc[RV_C_DUP]);
+    cudaEventElapsedTime(&ms, rb.ev[0], rb.ev[1]);
+    cudaEventElapsedTime(&part, rb.ev[2], rb.ev[3]);
+    ms += part;
+    const uint64_t nq = m ? hc[RV_C_QUERIES] : 0, text_total = m ? hc[RV_C_TEXT] : 0, n_unres = m ? hc[RV_C_UNRESOLVED] : 0;
+    /* 7. emit */
+    if ((rc = ensure_dev(ctx, rb.text, text_total + 16)))
+        return rc;
+    p.text = (uint8_t *)rb.text.p;
+    CK(cudaEventRecord(rb.ev[3], s));
+    if (m && text_total) {
+        regk_resolve_emit_kernel<<<(unsigned)((2 * m + 255) / 256), 256, 0, s>>>(p);
+        CK(cudaGetLastError());
+        launches++;
+    }
+    CK(cudaEventRecord(rb.ev[4], s));
+    const void *dsrc[6] = {rb.q_kind.p, rb.q_node.p, rb.sec_off.p, rb.text.p, rb.cls.p, rb.unres.p};
+    if (!dev_out) {
+        HostBuf *hb[6] = {&rb.h_q_kind, &rb.h_q_node, &rb.h_sec_off, &rb.h_text, &rb.h_cls, &rb.h_unres};
+        const size_t sz[6] = {(size_t)nq, (size_t)nq * 8, (size_t)(2 * nq + 1) * 8, (size_t)text_total, (size_t)m, (size_t)n_unres * 8};
+        for (int k = 0; k < 6; k++) {
+            if ((rc = to_host(ctx, *hb[k], dsrc[k], sz[k], s)))
+                return rc;
+            dsrc[k] = hb[k]->p;
+        }
+    }
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    cudaEventElapsedTime(&part, rb.ev[3], rb.ev[4]);
+    ms += part;
+    out->m = m;
+    out->n_queries = nq;
+    out->n_answers = m ? hc[RV_C_ANSWERS] : 0;
+    out->n_additional = m ? hc[RV_C_ADDITIONAL] : 0;
+    out->n_unresolved = n_unres;
+    out->text_total = text_total;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->q_kind = (const uint8_t *)dsrc[0];
+    out->q_node = (const uint64_t *)dsrc[1];
+    out->sec_off = (const uint64_t *)dsrc[2];
+    out->text = (const uint8_t *)dsrc[3];
+    out->node_cls = (const uint8_t *)dsrc[4];
+    out->unresolved = (const uint64_t *)dsrc[5];
+    out->kernel_ms = ms;
     return REGK_OK;
 }
 
