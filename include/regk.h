@@ -1165,6 +1165,93 @@ typedef struct regk_answers {
 
 int         regk_resolve(regk_ctx *ctx, const regk_decode_in *snapshot, const regk_resolve_opts *opts, regk_answers *out);
 
+/*
+ * ---- DNS responses from the last regk_resolve: RFC 1035 query messages in, wire-format A and SRV responses out ------
+ * Answers against the last regk_resolve on the context; REGK_ERR_STATE when there was none or it failed.  A device
+ * snapshot passed to that resolve must stay allocated and unchanged until the last regk_dns_answer on it (a host
+ * snapshot was staged by the resolve).  Results stay valid until the next regk_dns_answer or regk_resolve.
+ * Input: k messages back to back, no TCP length prefix; message i = msgs[off[i], off[i+1]).  Host memory, or device
+ * memory with REGK_IN_DEVICE (off 8-byte aligned, total = off[k]).  REGK_ERR_INVALID_ARG: a NULL pointer, unknown flag
+ * bits, a nonzero reserved, udp_payload outside 512..65535, misaligned device offsets, offsets that are not monotone
+ * or reach past total, a message longer than 65535 bytes; the message names the smallest bad message (device offsets
+ * are checked on the device before any message byte is read).
+ * Message handling, the first rule that applies decides:
+ *   1. shorter than 12 bytes, or QR = 1: REGK_DNS_DROPPED, no response bytes
+ *   2. opcode != 0: NOTIMP
+ *   3. QDCOUNT != 1, ANCOUNT != 0, NSCOUNT != 0 or ARCOUNT > 1: FORMERR
+ *   4. the question must parse, else FORMERR: labels of 1-63 bytes (a length byte with either top bit set, a
+ *      compression pointer or an extended label type, is FORMERR), a wire name of at most 255 bytes, QTYPE and QCLASS
+ *      inside the message
+ *   5. ARCOUNT = 1: an OPT record (root owner, TYPE 41, RDATA inside the message), else FORMERR; its CLASS is the
+ *      requester's UDP size, its TTL ext-rcode, version and flags; options are ignored
+ *   6. bytes after the last record: FORMERR
+ *   7. OPT version != 0: BADVERS (extended rcode 1 in the response OPT, header rcode 0)
+ *   8. QCLASS != IN: REFUSED
+ *   9. lookup.  Names compare after ASCII lower-casing; a name with a label byte outside [A-Za-z0-9_-], or the root,
+ *      owns nothing.  node(name) = the snapshot node whose path is '/' + the lower-cased labels reversed, joined by
+ *      '/' (a node whose path has an upper-case letter is the node of no name).  A name owns A when node(name) has a
+ *      REGK_Q_HOST_A or REGK_Q_SERVICE_A query; it owns SRV when it has >= 3 labels and node(name without its first
+ *      two labels) is a class-OK service record whose srvce and proto equal those two labels, case-insensitively.
+ *      QTYPE A on an A owner, QTYPE SRV (33) on an SRV owner: ANSWER with that regk_resolve query's answers (and, for
+ *      SRV, additionals); any other QTYPE on a name that owns A or SRV: NODATA; otherwise NXDOMAIN.  A service without
+ *      children answers A with NOERROR and no RRs.  node[i] is the answering node for ANSWER, else ~0.
+ * Response: ID copied, QR = 1, opcode and RD copied, RA Z AD CD 0, AA = 1 for ANSWER, NODATA and NXDOMAIN.  NOTIMP and
+ * FORMERR: the 12-byte header only, QDCOUNT 0.  Every other response echoes the question byte for byte and, when the
+ * query had OPT, ends with an OPT record: root owner, TYPE 41, CLASS udp_payload, TTL ext-rcode << 24 | the query's
+ * DO bit, RDLENGTH 0.  RRs in the order and with the TTLs of the matching regk_resolve query, ports in payload order:
+ *   A      owner 0xC00C, 16 bytes
+ *   SRV    owner 0xC00C, priority 0, weight 10, port, the child's name uncompressed (RFC 2782): 20 + L bytes for a
+ *          name of L text bytes
+ *   additional A of a child: owner a pointer to the target name in the child's first SRV RR (RR start + 18), 16 bytes
+ * Size limit L: 65535 with REGK_DNS_TCP, else clamp(requester's OPT size, 512, udp_payload) with OPT and 512 without.
+ * Header, question and OPT always; then the longest prefix of the answers that fits in L; only if every answer fit,
+ * the longest prefix of the additionals that fits and whose owner pointer is below 0x4000 (a pointer's 14 bits).
+ * tc[i] (and the header's TC) is 1 exactly when an answer was left out.
+ * launches counts the once-per-resolve preparation (two kernels) on the first call after a resolve only; kernel_ms
+ * spans every pass of the call but the host's reads.
+ * PARITY UNPINNED (Binder is absent): its rcode for empty non-terminals and names outside its zones; AA and the
+ * header bits; answer order and shuffling; its truncation policy; case handling; the form of error responses.  The
+ * wire format is RFC 1035, 2782 and 6891.
+ */
+#define REGK_DNS_TCP (1u << 8)      /* regk_dns_opts.flags: a 65535-byte limit (no TCP length prefix is written) */
+
+typedef struct regk_dns_in {
+    const uint8_t  *msgs;           /* k query messages, back to back */
+    const uint64_t *off;            /* [k + 1], monotone; message i = msgs[off[i], off[i+1]) */
+    uint64_t k, total;              /* total = off[k] (required for device input) */
+    uint32_t flags;                 /* REGK_IN_DEVICE */
+    uint32_t reserved;              /* 0 */
+} regk_dns_in;
+
+typedef struct regk_dns_opts {
+    uint32_t flags;                 /* REGK_OUT_DEVICE | REGK_DNS_TCP */
+    uint32_t udp_payload;           /* the server's EDNS0 UDP size, 512..65535 (e.g. 1232) */
+} regk_dns_opts;
+
+#define REGK_DNS_ANSWER   0u
+#define REGK_DNS_NODATA   1u
+#define REGK_DNS_NXDOMAIN 2u
+#define REGK_DNS_FORMERR  3u
+#define REGK_DNS_NOTIMP   4u
+#define REGK_DNS_REFUSED  5u
+#define REGK_DNS_BADVERS  6u
+#define REGK_DNS_DROPPED  7u
+
+typedef struct regk_dns_out {
+    uint64_t k, resp_total;
+    uint64_t n_status[8];           /* per REGK_DNS_* */
+    uint64_t n_truncated;
+    uint32_t flags, launches;       /* REGK_OUT_DEVICE */
+    const uint64_t *resp_off;       /* [k + 1]; a dropped message has an empty range */
+    const uint8_t  *resp;           /* [resp_total] */
+    const uint8_t  *status;         /* [k] REGK_DNS_* */
+    const uint8_t  *tc;             /* [k] 1 when answers were dropped to fit */
+    const uint64_t *node;           /* [k] snapshot node whose records answered, ~0 if none */
+    float kernel_ms;
+} regk_dns_out;
+
+int         regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *opts, regk_dns_out *out);
+
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);
 int64_t     regk_get_option(const regk_ctx *ctx, const char *name);

@@ -510,6 +510,44 @@ class Answers:
         return self.text[int(self.sec_off[2 * q + 1]):int(self.sec_off[2 * q + 2])].tobytes()
 
 
+class CDnsIn(C.Structure):           # regk_dns_in
+    _fields_ = [("msgs", C.c_void_p), ("off", C.c_void_p), ("k", C.c_uint64), ("total", C.c_uint64),
+                ("flags", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class CDnsOpts(C.Structure):         # regk_dns_opts
+    _fields_ = [("flags", C.c_uint32), ("udp_payload", C.c_uint32)]
+
+
+class CDnsOut(C.Structure):          # regk_dns_out
+    _fields_ = [("k", C.c_uint64), ("resp_total", C.c_uint64), ("n_status", C.c_uint64 * 8), ("n_truncated", C.c_uint64),
+                ("flags", C.c_uint32), ("launches", C.c_uint32), ("resp_off", C.c_void_p), ("resp", C.c_void_p),
+                ("status", C.c_void_p), ("tc", C.c_void_p), ("node", C.c_void_p), ("kernel_ms", C.c_float)]
+
+
+(DNS_ANSWER, DNS_NODATA, DNS_NXDOMAIN, DNS_FORMERR, DNS_NOTIMP, DNS_REFUSED, DNS_BADVERS,
+ DNS_DROPPED) = range(8)                                             # DnsResponses.status
+FLAG_DNS_TCP = 1 << 8                                                # CDnsOpts.flags
+
+
+class DnsResponses:
+    """Host copy of a regk_dns_out: response(i) is the wire-format response to message i (b"" when it was dropped);
+    status[i] is DNS_*, tc[i] 1 when answers were left out to fit, node[i] the snapshot node that answered (~0: none)."""
+
+    def __init__(self, out):
+        self.k, self.resp_total = int(out.k), int(out.resp_total)
+        self.n_status = [int(x) for x in out.n_status]
+        self.n_truncated, self.launches, self.kernel_ms = int(out.n_truncated), int(out.launches), float(out.kernel_ms)
+        self.resp_off = _as_np(out.resp_off, self.k + 1, np.uint64).copy()
+        self.resp = _as_np(out.resp, self.resp_total, np.uint8).copy()
+        self.status = _as_np(out.status, self.k, np.uint8).copy()
+        self.tc = _as_np(out.tc, self.k, np.uint8).copy()
+        self.node = _as_np(out.node, self.k, np.uint64).copy()
+
+    def response(self, i: int) -> bytes:
+        return self.resp[int(self.resp_off[i]):int(self.resp_off[i + 1])].tobytes()
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -524,7 +562,7 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned",
            "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results", "regk_read_stats",
            "regk_reconcile_stats", "regk_read_events", "regk_events_requests",
-           "regk_setwatches_requests", "regk_resolve"]
+           "regk_setwatches_requests", "regk_resolve", "regk_dns_answer"]
 
 _lib = None
 
@@ -591,6 +629,7 @@ def load_library():
     lib.regk_events_requests.argtypes = [vp, C.POINTER(CJuteOpts), C.POINTER(CFrames)]
     lib.regk_setwatches_requests.argtypes = [vp, C.POINTER(CSetWatchesOpts), C.POINTER(CSetWatches)]
     lib.regk_resolve.argtypes = [vp, C.POINTER(CDecodeIn), C.POINTER(CResolveOpts), C.POINTER(CAnswers)]
+    lib.regk_dns_answer.argtypes = [vp, C.POINTER(CDnsIn), C.POINTER(CDnsOpts), C.POINTER(CDnsOut)]
     _lib = lib
     return lib
 
@@ -1176,6 +1215,32 @@ class Context:
         del keep
         self._check(rc)
         return out if device else Answers(out)
+
+    def answer_dns(self, msgs, off, udp_payload: int = 1232, tcp: bool = False, device: bool = False):
+        """regk_dns_answer: responses to the query messages msgs[off[i]:off[i+1]] (NumPy uint8 bytes and int64 / uint64
+        offsets, or contiguous CUDA uint8 and int64 tensors), answered from the last resolve() on this context.
+        udp_payload is the server's EDNS0 UDP size; tcp=True allows 65535 bytes.  Returns a DnsResponses, or the raw
+        CDnsOut (arrays on the device) with device=True."""
+        flags = (FLAG_OUT_DEVICE if device else 0) | (FLAG_DNS_TCP if tcp else 0)
+        if hasattr(msgs, "data_ptr"):
+            import torch
+            if not msgs.is_cuda or msgs.dtype != torch.uint8 or not msgs.is_contiguous():
+                raise ValueError("device messages are a contiguous CUDA uint8 tensor")
+            if not off.is_cuda or off.dtype != torch.int64 or not off.is_contiguous():
+                raise ValueError("device offsets are a contiguous CUDA int64 tensor")
+            keep = (msgs, off)
+            cin = CDnsIn(msgs.data_ptr() or None, off.data_ptr() or None, off.numel() - 1, msgs.numel(), FLAG_IN_DEVICE, 0)
+        else:
+            m = np.ascontiguousarray(msgs, np.uint8).reshape(-1)
+            o = np.ascontiguousarray(off).astype(np.uint64, copy=False)
+            keep = (m, o)
+            cin = CDnsIn(_np_ptr(m), _np_ptr(o), o.size - 1, int(o[-1]) if o.size else 0, 0, 0)
+        opts = CDnsOpts(flags, int(udp_payload))
+        out = CDnsOut()
+        rc = self._lib.regk_dns_answer(self._h, C.byref(cin), C.byref(opts), C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else DnsResponses(out)
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

@@ -40,6 +40,7 @@
 #include "regk_events.cuh"
 #include "regk_setwatches.cuh"
 #include "regk_resolve.cuh"
+#include "regk_dns.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -338,7 +339,21 @@ struct regk_ctx {
             count, node_q, q_kind, q_node, sec_off, unres, text, sort_tmp;
         HostBuf h_count, h_q_kind, h_q_node, h_sec_off, h_text, h_cls, h_unres;
         Event ev[5];
+        /* the last call succeeded: regk_dns_answer answers against it (the snapshot streams it read, its table size) */
+        bool valid = false;
+        uint64_t gen = 0, m = 0, path_total = 0, slots = 0;
+        const uint8_t *pb = nullptr, *jb = nullptr;
+        const uint64_t *po = nullptr, *jo = nullptr;
     } rsv;
+    /* regk_dns_answer (regk_dns.cuh): the per-resolve preparation (of resolve generation prep_gen), the staged queries,
+       the per-query arrays and the responses */
+    struct Dns {
+        uint64_t prep_gen = 0;
+        DevBuf ip4, cum[3], ptotals, in[2], scratch, status, tc, node, meta, nans, nadd, ans_bytes, qtotals, resp_off, rr_base,
+            count, resp;
+        HostBuf h_count, h_resp_off, h_resp, h_status, h_tc, h_node;
+        Event ev[4];
+    } dns;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     struct Skip {
@@ -5597,6 +5612,7 @@ int regk_resolve(regk_ctx *ctx, const regk_decode_in *in, const regk_resolve_opt
     if (!ctx || !in || !o || !out)
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_resolve: NULL argument");
     memset(out, 0, sizeof *out);
+    ctx->rsv.valid = false;
     if (in->flags & REGK_DECODE_LAST)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams", who);
     if (o->flags & ~REGK_OUT_DEVICE)
@@ -5847,6 +5863,226 @@ int regk_resolve(regk_ctx *ctx, const regk_decode_in *in, const regk_resolve_opt
     out->text = (const uint8_t *)dsrc[3];
     out->node_cls = (const uint8_t *)dsrc[4];
     out->unresolved = (const uint64_t *)dsrc[5];
+    out->kernel_ms = ms;
+    rb.valid = true;
+    rb.gen++;
+    rb.m = m;
+    rb.path_total = path_total;
+    rb.slots = slots;
+    rb.pb = pb;
+    rb.po = po;
+    rb.jb = jb;
+    rb.jo = jo;
+    return REGK_OK;
+}
+
+int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o, regk_dns_out *out)
+{
+    const char *who = "regk_dns_answer";
+    if (!ctx || !in || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_dns_answer: NULL argument");
+    memset(out, 0, sizeof *out);
+    if (in->flags & ~REGK_IN_DEVICE)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: unknown input flag bits 0x%x", who, in->flags & ~REGK_IN_DEVICE);
+    if (in->reserved)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: reserved must be 0", who);
+    if (o->flags & ~(REGK_OUT_DEVICE | REGK_DNS_TCP))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: unknown flag bits 0x%x", who, o->flags & ~(REGK_OUT_DEVICE | REGK_DNS_TCP));
+    if (o->udp_payload < 512u || o->udp_payload > 65535u)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: udp_payload %u outside 512..65535", who, o->udp_payload);
+    const regk_ctx::Resolve &rb = ctx->rsv;
+    if (!rb.valid)
+        return fail(ctx, REGK_ERR_STATE, "%s: no successful regk_resolve on this context to answer from", who);
+    if (ctx->pending)
+        return fail(ctx, REGK_ERR_STATE, "%s: batches are still in flight; finish them first", who);
+    const uint64_t k = in->k, m = rb.m;
+    const bool in_dev = in->flags & REGK_IN_DEVICE, dev_out = o->flags & REGK_OUT_DEVICE;
+    if (k && !in->off)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: %llu messages need offsets", who, (unsigned long long)k);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    regk_ctx::Dns &db = ctx->dns;
+    int rc;
+    uint64_t total = k ? in->total : 0;
+    const uint8_t *mb = in->msgs;
+    const uint64_t *mo = in->off;
+    if (k && !in_dev) {
+        total = mo[k];
+        for (uint64_t i = 0; i < k; i++)
+            if (mo[i] > mo[i + 1] || mo[i + 1] > total || mo[i + 1] - mo[i] > 65535u)
+                return fail(ctx, REGK_ERR_INVALID_ARG, "%s: message %llu: offsets not monotone, past total or longer than 65535 "
+                                                       "bytes", who, (unsigned long long)i);
+        if (total && !mb)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: offsets without message bytes", who);
+        if ((rc = stage_in(ctx, db.in[0], mb, total, s)) || (rc = stage_in(ctx, db.in[1], mo, (k + 1) * 8, s)))
+            return rc;
+        mb = (const uint8_t *)db.in[0].p;
+        mo = (const uint64_t *)db.in[1].p;
+    } else if (k) {
+        if (total && !mb)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: offsets without message bytes", who);
+        if ((uintptr_t)mo & 7u)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: misaligned device offsets (8-byte alignment)", who);
+    }
+    if ((rc = ensure_dev(ctx, db.in[0], 16)))
+        return rc;
+    if (!mb)
+        mb = (const uint8_t *)db.in[0].p;
+    for (Event &ev : db.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
+    const uint64_t ptiles = (m + RV_TILE - 1) / RV_TILE, pnsup = ptiles / SUPER + 1;
+    const uint64_t tiles = (k + RV_TILE - 1) / RV_TILE, nsup = tiles / SUPER + 1;
+    if ((rc = ensure_dev(ctx, db.ip4, m * 4 + 16)) || (rc = ensure_dev(ctx, db.ptotals, 3 * (ptiles + pnsup) * 8)) ||
+        (rc = ensure_dev(ctx, db.scratch, total + 16)) || (rc = ensure_dev(ctx, db.status, k + 16)) ||
+        (rc = ensure_dev(ctx, db.tc, k + 16)) || (rc = ensure_dev(ctx, db.node, k * 8 + 16)) ||
+        (rc = ensure_dev(ctx, db.meta, k * 4 + 16)) || (rc = ensure_dev(ctx, db.nans, k * 4 + 16)) ||
+        (rc = ensure_dev(ctx, db.nadd, k * 4 + 16)) || (rc = ensure_dev(ctx, db.ans_bytes, k * 4 + 16)) ||
+        (rc = ensure_dev(ctx, db.qtotals, 2 * (tiles + nsup) * 8)) || (rc = ensure_dev(ctx, db.resp_off, (k + 1) * 8)) ||
+        (rc = ensure_dev(ctx, db.rr_base, (k + 1) * 8)) || (rc = ensure_dev(ctx, db.count, DNS_NCOUNTERS * 8)) ||
+        (rc = ensure_host(ctx, db.h_count, DNS_NCOUNTERS * 8)))
+        return rc;
+    for (int j = 0; j < 3; j++)
+        if ((rc = ensure_dev(ctx, db.cum[j], (m + 1) * 8)))
+            return rc;
+    DnsParams p{};
+    p.m = m;
+    p.path = rb.pb;
+    p.path_off = (const unsigned long long *)rb.po;
+    p.path_total = rb.path_total;
+    p.json = rb.jb;
+    p.json_off = (const unsigned long long *)rb.jo;
+    p.dec = (const Decoded *)rb.rec.p;
+    p.dom = (const uint8_t *)rb.dom.p;
+    p.ports = (const uint32_t *)rb.ports.p;
+    p.mask = (uint32_t)(rb.slots - 1);
+    p.table = (const uint32_t *)rb.table.p;
+    p.cls = (const uint8_t *)rb.cls.p;
+    p.roles = (const uint8_t *)rb.roles.p;
+    p.ttl = (const int32_t *)rb.ttl.p;
+    p.skey = (const uint32_t *)rb.skey.p;
+    p.sval = (const uint32_t *)rb.sval.p;
+    p.first = (const uint32_t *)rb.first.p;
+    p.end = (const uint32_t *)rb.end.p;
+    p.ip4 = (uint32_t *)db.ip4.p;
+    unsigned long long *pt = (unsigned long long *)db.ptotals.p, *qt = (unsigned long long *)db.qtotals.p;
+    for (int j = 0; j < 3; j++) {
+        p.cum[j] = (unsigned long long *)db.cum[j].p;
+        p.ctile[j] = pt + (size_t)j * (ptiles + pnsup);
+        p.csuper[j] = p.ctile[j] + ptiles;
+        p.qtile[j] = qt + (size_t)(j < 2 ? j : 1) * (tiles + nsup);
+        p.qsuper[j] = p.qtile[j] + tiles;
+    }
+    p.k = k;
+    p.msgs = mb;
+    p.off = (const unsigned long long *)mo;
+    p.total = total;
+    p.scratch = (uint8_t *)db.scratch.p;
+    p.udp_payload = o->udp_payload;
+    p.tcp = (o->flags & REGK_DNS_TCP) ? 1u : 0u;
+    p.status = (uint8_t *)db.status.p;
+    p.tc = (uint8_t *)db.tc.p;
+    p.node = (unsigned long long *)db.node.p;
+    p.meta = (uint32_t *)db.meta.p;
+    p.nans = (uint32_t *)db.nans.p;
+    p.nadd = (uint32_t *)db.nadd.p;
+    p.ans_bytes = (uint32_t *)db.ans_bytes.p;
+    p.resp_off = (unsigned long long *)db.resp_off.p;
+    p.rr_base = (unsigned long long *)db.rr_base.p;
+    p.counters = (unsigned long long *)db.count.p;
+    unsigned long long *hc = (unsigned long long *)db.h_count.p;
+    uint32_t launches = 0;
+    float ms = 0, part = 0;
+    CK(cudaMemsetAsync(db.count.p, 0, DNS_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(db.count.p, 0xFF, 8, s));            /* no bad message */
+    CK(cudaMemsetAsync(db.qtotals.p, 0, 2 * (tiles + nsup) * 8, s));
+    CK(cudaMemsetAsync(db.resp_off.p, 0, 8, s));
+    CK(cudaMemsetAsync(db.rr_base.p, 0, 8, s));
+    CK(cudaEventRecord(db.ev[0], s));
+    /* 1. once per resolve: addresses and the per-child wire sizes */
+    if (db.prep_gen != rb.gen) {
+        CK(cudaMemsetAsync(db.ptotals.p, 0, 3 * (ptiles + pnsup) * 8, s));
+        CK(cudaMemsetAsync(db.cum[0].p, 0, 8, s));
+        CK(cudaMemsetAsync(db.cum[1].p, 0, 8, s));
+        CK(cudaMemsetAsync(db.cum[2].p, 0, 8, s));
+        if (m) {
+            regk_dns_prep_kernel<<<(unsigned)ptiles, RV_TILE, 0, s>>>(p);
+            regk_dns_prep_scan_kernel<<<(unsigned)ptiles, RV_TILE, 0, s>>>(p);
+            CK(cudaGetLastError());
+            launches += 2;
+        }
+    }
+    /* 2. device offsets, before any message byte is read */
+    if (k && in_dev) {
+        regk_dns_check_kernel<<<(unsigned)((k + 255) / 256), 256, 0, s>>>(p);
+        CK(cudaGetLastError());
+        launches++;
+        CK(cudaEventRecord(db.ev[1], s));
+        CK(cudaMemcpyAsync(hc, db.count.p, 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        if (hc[DNS_C_BAD] != ~0ull)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: message %llu: offsets not monotone, past total or longer than 65535 bytes",
+                who, hc[DNS_C_BAD]);
+        cudaEventElapsedTime(&ms, db.ev[0], db.ev[1]);
+        CK(cudaEventRecord(db.ev[0], s));
+    }
+    db.prep_gen = rb.gen;
+    /* 3. parse, look up and cut; 4. place */
+    if (k) {
+        regk_dns_parse_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p);
+        regk_dns_place_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p);
+        CK(cudaGetLastError());
+        launches += 2;
+    }
+    CK(cudaEventRecord(db.ev[1], s));
+    CK(cudaMemcpyAsync(hc, db.count.p, DNS_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    cudaEventElapsedTime(&part, db.ev[0], db.ev[1]);
+    ms += part;
+    const uint64_t resp_total = k ? hc[DNS_C_RESP] : 0, n_rr = k ? hc[DNS_C_RR] : 0;
+    /* 5. emit */
+    if ((rc = ensure_dev(ctx, db.resp, resp_total + 16)))
+        return rc;
+    p.resp = (uint8_t *)db.resp.p;
+    CK(cudaEventRecord(db.ev[2], s));
+    if (resp_total) {
+        regk_dns_emit_head_kernel<<<(unsigned)((k + 255) / 256), 256, 0, s>>>(p);
+        launches++;
+        if (n_rr) {
+            regk_dns_emit_rr_kernel<<<(unsigned)((n_rr + 255) / 256), 256, 0, s>>>(p, n_rr);
+            launches++;
+        }
+        CK(cudaGetLastError());
+    }
+    CK(cudaEventRecord(db.ev[3], s));
+    const void *dsrc[5] = {db.resp_off.p, db.resp.p, db.status.p, db.tc.p, db.node.p};
+    if (!dev_out) {
+        HostBuf *hb[5] = {&db.h_resp_off, &db.h_resp, &db.h_status, &db.h_tc, &db.h_node};
+        const size_t sz[5] = {(size_t)(k + 1) * 8, (size_t)resp_total, (size_t)k, (size_t)k, (size_t)k * 8};
+        for (int j = 0; j < 5; j++) {
+            if ((rc = to_host(ctx, *hb[j], dsrc[j], sz[j], s)))
+                return rc;
+            dsrc[j] = hb[j]->p;
+        }
+    }
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    cudaEventElapsedTime(&part, db.ev[2], db.ev[3]);
+    ms += part;
+    out->k = k;
+    out->resp_total = resp_total;
+    for (int j = 0; j < 8; j++)
+        out->n_status[j] = k ? hc[DNS_C_STATUS + j] : 0;
+    out->n_truncated = k ? hc[DNS_C_TC] : 0;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->resp_off = (const uint64_t *)dsrc[0];
+    out->resp = (const uint8_t *)dsrc[1];
+    out->status = (const uint8_t *)dsrc[2];
+    out->tc = (const uint8_t *)dsrc[3];
+    out->node = (const uint64_t *)dsrc[4];
     out->kernel_ms = ms;
     return REGK_OK;
 }
