@@ -1252,6 +1252,71 @@ typedef struct regk_dns_out {
 
 int         regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *opts, regk_dns_out *out);
 
+/*
+ * ---- walk a registry subtree: getData and getChildren level by level, into the snapshot regk_resolve answers from
+ * (Binder's access pattern, README.md:502-536: fetch the node, list its children, fetch every child) -----------------
+ * The walk lives on the context, apart from every batch: finishing a batch does not touch it, and no walk call touches
+ * another call's results (regk_read_replies, regk_read_children, regk_resolve, ... stay valid across walk calls).
+ * regk_walk_start: the roots (host memory; root i = roots[root_off[i], root_off[i+1]), root_off monotone) are level 0's
+ *   frontier, in the order given; any earlier walk is dropped (a refused start leaves it as it was).  REGK_ERR_INVALID_ARG,
+ *   naming the smallest bad root:
+ *   flags != 0; n_roots == 0; a root ZooKeeper rejects (regk_mkdirp_dirs' INVALID rule, or empty); "/" (its listing would give
+ *   "//name", and /zookeeper is not registry data); a root equal to an earlier root; a root that another root is a
+ *   proper ancestor of.
+ * regk_walk_requests: the current frontier of f nodes as one buffer of 2 f frames - frame i < f is GetDataRequest{path
+ *   i, watch = false} = len | xid_base + i | 4 | P | path | 0, frame f + i is GetChildrenRequest{path i, watch = false},
+ *   the same layout with op word 8 and xid xid_base + f + i (xids wrap).  The replies can so be read as a getData
+ *   section followed, at its end, by a getChildren section.  Framing again (e.g. with a new xid base after a reconnect)
+ *   is allowed; the last framing counts.  REGK_ERR_STATE: no walk, or a complete walk (an empty frontier).
+ *   REGK_ERR_INVALID_ARG: [xid_base, xid_base + 2 f) covers -1 or -2; f >= 2^30.  flags: REGK_OUT_DEVICE returns
+ *   device pointers, else pinned host arrays; valid until the next regk_walk_requests or regk_walk_start.
+ * regk_read_walk: bytes[0, len) = what the caller read after sending that framing: the f getData replies, then the f
+ *   getChildren replies (host memory, or device memory with REGK_IN_DEVICE, 16-byte aligned).  Notifications (xid -1)
+ *   and pings (xid -2) before the last reply are skipped and counted; the stream may go on past the last reply.
+ *     found node   frontier node i becomes the next snapshot node iff its getData reply has err 0: its path, the
+ *                  reply's data (D = -1 reads as empty), Stat.version and Stat.ephemeralOwner
+ *     order        breadth first: level by level, frontier order within a level; level_off holds the boundaries
+ *     next level   for each node whose getChildren reply has err 0 (whether or not its getData found it: the two reads
+ *                  are separate, and a race between them is not an error), its children in the reply's order, as
+ *                  path + '/' + name
+ *     errors       NONODE (-101) on either read means the node is gone; any other code is counted in n_error /
+ *                  n_list_error: do not trust a snapshot built while either count is nonzero
+ *     duplicates   two equal names in one listing are not looked for (a server cannot hold them); regk_resolve would
+ *                  refuse the duplicate path, naming the later node
+ *   Refusals (REGK_ERR_INVALID_ARG; the message names the byte position and the expected xid): exactly regk_read_replies'
+ *   refusals on the getData section and regk_read_children's on the getChildren section, which starts at the getData
+ *   section's consumed.  A refused read changes nothing: the frontier, the framing and the snapshot stay as they were,
+ *   so the stream can be fixed and read again.  REGK_ERR_STATE: no framing of the current frontier.
+ *   The snapshot, version and ephemeral_owner are ALWAYS device arrays, in the layout regk_reconcile takes; level_off is
+ *   a host array.  REGK_OUT_DEVICE is accepted and changes nothing.  They stay valid until the next regk_read_walk or
+ *   regk_walk_start: a read appends and may reallocate.  A regk_resolve given an earlier walk snapshot must therefore
+ *   be redone before regk_dns_answer is used again: a device snapshot passed to that resolve must stay allocated and
+ *   unchanged until the last regk_dns_answer on it.
+ * PARITY UNPINNED: the layouts are restated from zookeeper.jute and tested against an independent restatement, not
+ * against a server.  A directory whose listing exceeds the server's jute.maxbuffer cannot be listed by any client, and
+ * this call does not handle it.
+ */
+typedef struct regk_walk {
+    uint64_t level;                 /* levels read so far */
+    uint64_t m;                     /* snapshot nodes so far */
+    uint64_t n_frontier;            /* nodes of the next level; 0: the walk is complete */
+    uint64_t n_found, n_missing, n_error;               /* this level's getData replies: err 0 / NONODE / other */
+    uint64_t n_listed, n_list_missing, n_list_error;    /* this level's getChildren replies, same split */
+    uint64_t n_children;            /* listing entries this level read (= the next level's size) */
+    uint64_t n_skipped;             /* notifications and pings met before the last reply */
+    uint64_t consumed;              /* stream bytes up to the end of the last reply */
+    uint32_t flags, launches;
+    const uint64_t *level_off;      /* [level + 1], host: level l's nodes are [level_off[l], level_off[l+1]) */
+    regk_decode_in  snapshot;       /* ALWAYS device (REGK_IN_DEVICE), aligned as regk_reconcile requires */
+    const int32_t  *version;        /* [m] device: Stat.version */
+    const int64_t  *ephemeral_owner;/* [m] device: Stat.ephemeralOwner */
+    float kernel_ms;
+} regk_walk;
+
+int         regk_walk_start(regk_ctx *ctx, const uint8_t *roots, const uint64_t *root_off, uint64_t n_roots, uint32_t flags);
+int         regk_walk_requests(regk_ctx *ctx, int32_t xid_base, uint32_t flags, regk_frames *out);
+int         regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t flags, regk_walk *out);
+
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);
 int64_t     regk_get_option(const regk_ctx *ctx, const char *name);

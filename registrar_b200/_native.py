@@ -548,6 +548,47 @@ class DnsResponses:
         return self.resp[int(self.resp_off[i]):int(self.resp_off[i + 1])].tobytes()
 
 
+class CWalk(C.Structure):            # regk_walk
+    _fields_ = [("level", C.c_uint64), ("m", C.c_uint64), ("n_frontier", C.c_uint64), ("n_found", C.c_uint64),
+                ("n_missing", C.c_uint64), ("n_error", C.c_uint64), ("n_listed", C.c_uint64),
+                ("n_list_missing", C.c_uint64), ("n_list_error", C.c_uint64), ("n_children", C.c_uint64),
+                ("n_skipped", C.c_uint64), ("consumed", C.c_uint64), ("flags", C.c_uint32), ("launches", C.c_uint32),
+                ("level_off", C.c_void_p), ("snapshot", CDecodeIn), ("version", C.c_void_p),
+                ("ephemeral_owner", C.c_void_p), ("kernel_ms", C.c_float)]
+
+
+class Walk:
+    """What read_walk() made of one level's replies: the counts of that level (n_found / n_missing / n_error of its
+    getData replies, n_listed / n_list_missing / n_list_error of its getChildren replies, n_children, n_skipped,
+    `consumed`), and the walk so far: `level` levels, m snapshot nodes in breadth-first order, level l being nodes
+    level_off[l]:level_off[l+1], and n_frontier nodes in the next level (0: the walk is complete).  The snapshot stays
+    on the device: pass this object to Context.resolve(walk, ...) as it is, or copy it out with snapshot().  Do not trust
+    a snapshot built while n_error or n_list_error was nonzero.  Valid until the next read_walk() or walk_start()."""
+
+    def __init__(self, ctx, out):
+        self._ctx, self._out = ctx, out
+        self.level, self.m, self.n_frontier = int(out.level), int(out.m), int(out.n_frontier)
+        self.n_found, self.n_missing, self.n_error = int(out.n_found), int(out.n_missing), int(out.n_error)
+        self.n_listed, self.n_list_missing = int(out.n_listed), int(out.n_list_missing)
+        self.n_list_error, self.n_children = int(out.n_list_error), int(out.n_children)
+        self.n_skipped, self.consumed = int(out.n_skipped), int(out.consumed)
+        self.launches, self.kernel_ms = int(out.launches), float(out.kernel_ms)
+        self.level_off = _as_np(out.level_off, self.level + 1, np.uint64).copy()
+
+    def cdecode_in(self):
+        """the device regk_decode_in of the snapshot.  Returns (struct, keepalive)."""
+        return self._out.snapshot, None
+
+    def cnode_stat(self, session: int, zk_flags: int):
+        """regk_node_stat over the snapshot's device version / owner arrays.  Returns (struct, keepalive)."""
+        return CNodeStat(version=self._out.version, ephemeral_owner=self._out.ephemeral_owner, session=session,
+                         zk_flags=zk_flags), None
+
+    def snapshot(self):
+        """host batch.Snapshot copy of the snapshot, with version and owner"""
+        return Replies.snapshot(self)
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -562,7 +603,8 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_mkdirp_requests", "regk_reconcile", "regk_reconcile_requests", "regk_reconcile_owned",
            "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results", "regk_read_stats",
            "regk_reconcile_stats", "regk_read_events", "regk_events_requests",
-           "regk_setwatches_requests", "regk_resolve", "regk_dns_answer"]
+           "regk_setwatches_requests", "regk_resolve", "regk_dns_answer", "regk_walk_start", "regk_walk_requests",
+           "regk_read_walk"]
 
 _lib = None
 
@@ -630,6 +672,9 @@ def load_library():
     lib.regk_setwatches_requests.argtypes = [vp, C.POINTER(CSetWatchesOpts), C.POINTER(CSetWatches)]
     lib.regk_resolve.argtypes = [vp, C.POINTER(CDecodeIn), C.POINTER(CResolveOpts), C.POINTER(CAnswers)]
     lib.regk_dns_answer.argtypes = [vp, C.POINTER(CDnsIn), C.POINTER(CDnsOpts), C.POINTER(CDnsOut)]
+    lib.regk_walk_start.argtypes = [vp, vp, vp, u64, u32]
+    lib.regk_walk_requests.argtypes = [vp, C.c_int32, u32, C.POINTER(CFrames)]
+    lib.regk_read_walk.argtypes = [vp, vp, u64, u32, C.POINTER(CWalk)]
     _lib = lib
     return lib
 
@@ -1206,7 +1251,7 @@ class Context:
     # -- what DNS answers for a snapshot --
     def resolve(self, snapshot, default_host_ttl: int, default_srv_ttl: int, device: bool = False):
         """regk_resolve: the A and SRV answers the host and service records of `snapshot` define (a batch.Snapshot,
-        host or CUDA, or anything with cdecode_in(), such as a Replies).  Returns an Answers, or the raw CAnswers
+        host or CUDA, or anything with cdecode_in(), such as a Replies or a Walk).  Returns an Answers, or the raw CAnswers
         (device pointers) with device=True."""
         cin, keep = snapshot.cdecode_in()
         o = CResolveOpts(FLAG_OUT_DEVICE if device else 0, int(default_host_ttl), int(default_srv_ttl), 0)
@@ -1241,6 +1286,68 @@ class Context:
         del keep
         self._check(rc)
         return out if device else DnsResponses(out)
+
+    # -- a registry subtree walked level by level: getData and getChildren per node, one breadth-first snapshot --
+    def walk_start(self, roots):
+        """regk_walk_start: `roots` (a list of bytes paths) are the walk's first level, in that order; any earlier walk
+        is dropped."""
+        roots = [bytes(r) for r in roots]
+        b = np.frombuffer(b"".join(roots), np.uint8) if any(roots) else np.zeros(1, np.uint8)
+        off = np.zeros(len(roots) + 1, np.uint64)
+        np.cumsum([len(r) for r in roots], out=off[1:])
+        self._check(self._lib.regk_walk_start(self._h, _np_ptr(b), _np_ptr(off), len(roots), 0))
+
+    def walk_requests(self, xid_base: int = 1, device: bool = False):
+        """regk_walk_requests: a getData frame per node of the walk's current frontier, then a getChildren frame per
+        node, xids from xid_base on.  Returns (frame_bytes, frame_off uint64[2f+1], kernel_ms), or the raw CFrames with
+        device=True."""
+        out = CFrames()
+        rc = self._lib.regk_walk_requests(self._h, (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31,
+                                          FLAG_OUT_DEVICE if device else 0, C.byref(out))
+        self._check(rc)
+        if device:
+            return out
+        return (_as_np(out.frame_bytes, int(out.total), np.uint8).copy(),
+                _as_np(out.frame_off, int(out.n) + 1, np.uint64).copy(), float(out.kernel_ms))
+
+    def read_walk(self, stream, device: bool = False):
+        """regk_read_walk: `stream` (a NumPy uint8 array, or a contiguous CUDA uint8 tensor) holds the replies to the last
+        walk_requests() framing: the getData replies, then the getChildren replies.  Appends the level's found nodes to
+        the walk's snapshot and makes the listed children the next frontier.  Returns a Walk, or the raw CWalk with
+        device=True."""
+        flags = FLAG_OUT_DEVICE if device else 0
+        if hasattr(stream, "data_ptr"):
+            import torch
+            if not stream.is_cuda or stream.dtype != torch.uint8 or not stream.is_contiguous():
+                raise ValueError("a device stream is a contiguous CUDA uint8 tensor")
+            keep, ptr, n = stream, stream.data_ptr() or None, stream.numel()
+            flags |= FLAG_IN_DEVICE
+        else:
+            keep = np.ascontiguousarray(stream)
+            if keep.dtype != np.uint8 or keep.ndim != 1:
+                raise ValueError("a host stream is a one-dimensional uint8 array")
+            ptr, n = _np_ptr(keep), keep.size
+        out = CWalk()
+        rc = self._lib.regk_read_walk(self._h, ptr, n, flags, C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else Walk(self, out)
+
+    def walk(self, roots, exchange, xid_base: int = 1):
+        """The whole walk from `roots`: each level's frames go to exchange(frame_bytes) -> reply stream (the caller's
+        session), and the replies are read, until no level is left.  Each level's xids follow the last level's, skipping
+        to 0 where a range would cover -1 or -2.  Returns the last level's Walk (the whole snapshot)."""
+        self.walk_start(roots)
+        xid, f = int(xid_base) % 2 ** 32, len(roots)
+        while True:
+            if any((r - xid) % 2 ** 32 < 2 * f for r in (2 ** 32 - 1, 2 ** 32 - 2)):
+                xid = 0
+            fb, _, _ = self.walk_requests(xid)
+            s = exchange(fb)
+            w = self.read_walk(np.frombuffer(s, np.uint8) if isinstance(s, (bytes, bytearray)) else s)
+            xid, f = (xid + 2 * f) % 2 ** 32, w.n_frontier
+            if f == 0:
+                return w
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

@@ -41,6 +41,7 @@
 #include "regk_setwatches.cuh"
 #include "regk_resolve.cuh"
 #include "regk_dns.cuh"
+#include "regk_walk.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -354,6 +355,26 @@ struct regk_ctx {
         HostBuf h_count, h_resp_off, h_resp, h_status, h_tc, h_node;
         Event ev[4];
     } dns;
+    /* regk_walk_start / regk_walk_requests / regk_read_walk (regk_walk.cuh): the frontier (packed paths from 0, their
+       lengths; two sets, the next level is read into the other), the framing, the snapshot so far (grown
+       geometrically, [0, cap) of each stream allocated), and the read's own chains, per-node arrays and level streams */
+    struct Walk {
+        bool active = false, framed = false;
+        int cur = 0;
+        uint64_t f = 0, fpt = 0;                /* nodes of the current frontier, their path bytes */
+        DevBuf fbytes[2], foff[2], flen[2];
+        int32_t xid = 0;
+        FrameBufs frames;
+        uint64_t m = 0, path_total = 0, data_total = 0;
+        DevBuf snap_bytes[2], snap_off[2], ver, own;
+        std::vector<uint64_t> level_off;
+        DevBuf stream, word, totals, totals2, tile_base, cand, mark, jump, err, data_pos, dlen, dver, down, count;
+        DevBuf cword, ctotals, ctile_base, ccand, cmark, cjump, ctotals2, fpos, fend, cerr, cnt, seed_g, last_g1, name_bad,
+            end_pos, fault_pos, child_off, eword, etotals, etile_base, ecand, emark, ejump, etotals2, ent_pos, ent_nlen, ent_k;
+        DevBuf ftotals, node_rec, node_ver, node_own, node_plen, node_dlen, wcount, gtotals, lvl_bytes[2], lvl_off[2];
+        HostBuf h_count, h_wcount;
+        Event ev[2];
+    } wk;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     struct Skip {
@@ -6083,6 +6104,616 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
     out->status = (const uint8_t *)dsrc[2];
     out->tc = (const uint8_t *)dsrc[3];
     out->node = (const uint64_t *)dsrc[4];
+    out->kernel_ms = ms;
+    return REGK_OK;
+}
+
+/* `b` grown to hold `need` bytes with its first `used` kept: at least doubled, so that the levels of a walk are copied
+   O(log levels) times in all */
+static int walk_grow(regk_ctx *ctx, DevBuf &b, size_t used, size_t need)
+{
+    if (need <= b.cap)
+        return REGK_OK;
+    DevBuf nb;
+    size_t want = (std::max(need, 2 * b.cap) + 255) & ~(size_t)255;
+    cudaError_t e = cudaMalloc(&nb.p, want);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        want = (need + 255) & ~(size_t)255;
+        e = cudaMalloc(&nb.p, want);
+    }
+    if (e != cudaSuccess)
+        return fail(ctx, REGK_ERR_NOMEM, "cudaMalloc(%zu) failed: %s", want, cudaGetErrorString(e));
+    nb.cap = want;
+    if (used)
+        CK(cudaMemcpyAsync(nb.p, b.p, used, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    std::swap(b, nb);                           /* nb now holds the old buffer and frees it */
+    return REGK_OK;
+}
+
+int regk_walk_start(regk_ctx *ctx, const uint8_t *roots, const uint64_t *root_off, uint64_t n_roots, uint32_t flags)
+{
+    if (!ctx || !root_off || (!roots && n_roots))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_start: NULL argument");
+    if (flags)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_start: flags must be 0 (the roots are host memory)");
+    if (!n_roots)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_start: no roots");
+    for (uint64_t i = 0; i < n_roots; i++)
+        if (root_off[i + 1] < root_off[i] || root_off[i + 1] - root_off[i] >= (1ull << 31))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_start: root %llu: offsets not monotone, or a root of 2^31 bytes "
+                                                   "or more", (unsigned long long)i);
+    std::vector<std::string> r(n_roots);
+    std::map<std::string, uint64_t> first;
+    for (uint64_t i = 0; i < n_roots; i++) {
+        r[i].assign((const char *)roots + root_off[i], root_off[i + 1] - root_off[i]);
+        first.emplace(r[i], i);
+    }
+    for (uint64_t i = 0; i < n_roots; i++) {
+        const std::string &s = r[i];
+        const uint32_t c = mkdir_components((const uint8_t *)s.data(), (uint32_t)s.size());
+        if (s.empty() || c == MKDIR_INVALID)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_start: root %llu is a path ZooKeeper rejects",
+                (unsigned long long)i);
+        if (c == 0)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_start: root %llu is \"/\": its listing holds /zookeeper, and "
+                                                   "'/' + name would give \"//name\"", (unsigned long long)i);
+        const uint64_t j = first[s];
+        if (j != i)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_start: root %llu equals root %llu", (unsigned long long)i,
+                (unsigned long long)j);
+        for (size_t t = 1; t < s.size(); t++) {
+            auto a = s[t] == '/' ? first.find(s.substr(0, t)) : first.end();
+            if (a != first.end())
+                return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_start: root %llu lies under root %llu", (unsigned long long)i,
+                    (unsigned long long)a->second);
+        }
+    }
+    CK(cudaSetDevice(ctx->device));
+    regk_ctx::Walk &wk = ctx->wk;
+    wk.active = wk.framed = false;              /* the earlier walk is gone even if staging fails */
+    std::vector<uint8_t> pb;
+    std::vector<unsigned long long> po(n_roots + 1, 0);
+    std::vector<uint32_t> pl(n_roots);
+    for (uint64_t i = 0; i < n_roots; i++) {
+        pb.insert(pb.end(), r[i].begin(), r[i].end());
+        po[i + 1] = pb.size();
+        pl[i] = (uint32_t)r[i].size();
+    }
+    cudaStream_t s = ctx->stream;
+    int rc;
+    if ((rc = stage_in(ctx, wk.fbytes[0], pb.data(), pb.size(), s)) || (rc = stage_in(ctx, wk.foff[0], po.data(), po.size() * 8, s)) ||
+        (rc = stage_in(ctx, wk.flen[0], pl.data(), pl.size() * 4, s)) || (rc = sync_or_fail(ctx, s, "regk_walk_start")))
+        return rc;
+    wk.cur = 0;
+    wk.f = n_roots;
+    wk.fpt = pb.size();
+    wk.m = wk.path_total = wk.data_total = 0;
+    wk.level_off.assign(1, 0);
+    wk.active = true;
+    return REGK_OK;
+}
+
+int regk_walk_requests(regk_ctx *ctx, int32_t xid_base, uint32_t flags, regk_frames *out)
+{
+    if (!ctx || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_requests: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Walk &wk = ctx->wk;
+    if (flags & ~REGK_OUT_DEVICE)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_requests: unknown flags 0x%x", flags);
+    if (!wk.active)
+        return fail(ctx, REGK_ERR_STATE, "regk_walk_requests: no walk on this context; call regk_walk_start first");
+    if (!wk.f)
+        return fail(ctx, REGK_ERR_STATE, "regk_walk_requests: the walk is complete (its frontier is empty)");
+    const uint64_t f = wk.f;
+    if (f >= (1ull << 30))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_requests: a frontier of %llu nodes: must be below 2^30",
+            (unsigned long long)f);
+    for (int32_t reserved : {-1, -2})
+        if ((uint64_t)((uint32_t)reserved - (uint32_t)xid_base) < 2 * f)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_requests: the xids [%d, %d + %llu) cover %d, which ZooKeeper uses "
+                                                   "for %s", xid_base, xid_base, (unsigned long long)(2 * f), reserved,
+                        reserved == -1 ? "watch notifications" : "pings");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    for (Event &ev : wk.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
+    const unsigned long long sec1 = 17ull * f + wk.fpt, total = 2 * sec1;
+    FrameBufs &fb = wk.frames;
+    if ((rc = ensure_dev(ctx, fb.bytes, total + 16)) || (rc = ensure_dev(ctx, fb.off, (2 * f + 1) * 8)))
+        return rc;
+    WalkFrameParams p{};
+    p.f = f;
+    p.path_bytes = (const uint8_t *)wk.fbytes[wk.cur].p;
+    p.path_off = (const unsigned long long *)wk.foff[wk.cur].p;
+    p.xid_base = xid_base;
+    p.sec1 = sec1;
+    p.out = (uint8_t *)fb.bytes.p;
+    p.out_off = (unsigned long long *)fb.off.p;
+    CK(cudaEventRecord(wk.ev[0], s));
+    regk_walk_frame_kernel<<<(unsigned)(2 * ((f + MK_TILE - 1) / MK_TILE)), MK_TILE, 0, s>>>(p);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(wk.ev[1], s));
+    const void *bytes = fb.bytes.p, *off = fb.off.p;
+    if (!(flags & REGK_OUT_DEVICE)) {
+        if ((rc = to_host(ctx, fb.h_bytes, fb.bytes.p, total, s)) || (rc = to_host(ctx, fb.h_off, fb.off.p, (2 * f + 1) * 8, s)))
+            return rc;
+        bytes = fb.h_bytes.p;
+        off = fb.h_off.p;
+    }
+    if ((rc = sync_or_fail(ctx, s, "regk_walk_requests")))
+        return rc;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, wk.ev[0], wk.ev[1]);
+    wk.framed = true;
+    wk.xid = xid_base;
+    out->n = 2 * f;
+    out->total = total;
+    out->flags = flags & REGK_OUT_DEVICE;
+    out->launches = 1;
+    out->frame_bytes = (const uint8_t *)bytes;
+    out->frame_off = (const uint64_t *)off;
+    out->kernel_ms = ms;
+    return REGK_OK;
+}
+
+int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t flags, regk_walk *out)
+{
+    const char *who = "regk_read_walk";
+    if (!ctx || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Walk &wk = ctx->wk;
+    if (flags & ~(REGK_IN_DEVICE | REGK_OUT_DEVICE))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: unknown flags 0x%x", flags);
+    if (!wk.active || !wk.framed)
+        return fail(ctx, REGK_ERR_STATE, "regk_read_walk: no framing of the walk's current frontier (regk_walk_requests)");
+    if (!bytes && len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: NULL stream of %llu bytes", (unsigned long long)len);
+    const bool in_dev = flags & REGK_IN_DEVICE;
+    if (in_dev && ((uintptr_t)bytes & 15u))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: misaligned device stream (16-byte alignment needed)");
+    const uint64_t f = wk.f;
+    const int32_t xb = wk.xid, xc = (int32_t)((uint32_t)xb + (uint32_t)f);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    for (Event &ev : wk.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
+    const uint8_t *ds = bytes;
+    if (!in_dev) {
+        if ((rc = stage_in(ctx, wk.stream, bytes, len, s)))
+            return rc;
+        ds = (const uint8_t *)wk.stream.p;
+    }
+    const int cur = wk.cur, nx = 1 - cur;
+    const uint8_t *fbytes = (const uint8_t *)wk.fbytes[cur].p;
+    const unsigned long long *foff = (const unsigned long long *)wk.foff[cur].p;
+    const uint64_t nblk = (len + 15) / 16, tiles_s = (nblk + RP_TILE - 1) / RP_TILE;
+    const size_t totals_bytes = align16(tiles_s * 4) + (tiles_s / SUPER + 1) * 8;
+    const size_t f8 = f * 8 + 16, f4 = f * 4 + 16;
+    if ((rc = ensure_dev(ctx, wk.word, nblk * 4 + 16)) || (rc = ensure_dev(ctx, wk.totals, totals_bytes)) ||
+        (rc = ensure_dev(ctx, wk.tile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, wk.err, f4)) ||
+        (rc = ensure_dev(ctx, wk.data_pos, f8)) || (rc = ensure_dev(ctx, wk.dlen, f4)) || (rc = ensure_dev(ctx, wk.dver, f4)) ||
+        (rc = ensure_dev(ctx, wk.down, f8)) || (rc = ensure_dev(ctx, wk.count, CQ_NCOUNTERS * 8)) ||
+        (rc = ensure_host(ctx, wk.h_count, CQ_NCOUNTERS * 8)))
+        return rc;
+    unsigned long long *hc = (unsigned long long *)wk.h_count.p;
+    /* 1. the getData section: the frame chain from 0, the replies of the f nodes (regk_replies.cuh) */
+    RepParams p{};
+    p.s = ds;
+    p.len = len;
+    p.xid_base = xb;
+    p.n = f;
+    p.word = (uint32_t *)wk.word.p;
+    p.tile_total = (uint32_t *)wk.totals.p;
+    p.super_total = (unsigned long long *)((uint8_t *)wk.totals.p + align16(tiles_s * 4));
+    p.tile_base = (unsigned long long *)wk.tile_base.p;
+    p.err = (int32_t *)wk.err.p;
+    p.data_pos = (unsigned long long *)wk.data_pos.p;
+    p.dlen = (uint32_t *)wk.dlen.p;
+    p.ver = (int32_t *)wk.dver.p;
+    p.own = (long long *)wk.down.p;
+    p.counters = (unsigned long long *)wk.count.p;
+    CK(cudaMemsetAsync(p.counters, 0, CQ_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(p.counters + RQ_ERR, 0xFF, 8, s));
+    CK(cudaMemsetAsync(p.tile_total, 0, totals_bytes, s));
+    CK(cudaEventRecord(wk.ev[0], s));
+    uint32_t launches = 0;
+    if (len) {
+        regk_replies_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(p);
+        CK(cudaGetLastError());
+        launches++;
+    }
+    RepParams pg = p;
+    uint32_t *J = nullptr;
+    if ((rc = chain_pass(ctx, &pg, tiles_s, ~0ull, wk.cand, wk.mark, wk.jump, [&](const RepParams &q) {
+            regk_children_seed_kernel<<<1, 256, 0, s>>>(q, nullptr, nullptr, 1, 0ull);
+        }, &J, &launches, who)))
+        return rc;
+    if (pg.C) {
+        const uint64_t tiles_c = (pg.C + RP_TILE - 1) / RP_TILE;
+        const size_t t2 = align16(tiles_c * 4) + (tiles_c / SUPER + 1) * 8;
+        if ((rc = ensure_dev(ctx, wk.totals2, t2)))
+            return rc;
+        RepParams p2 = pg;
+        p2.tile_total = (uint32_t *)wk.totals2.p;
+        p2.super_total = (unsigned long long *)((uint8_t *)wk.totals2.p + align16(tiles_c * 4));
+        CK(cudaMemsetAsync(wk.totals2.p, 0, t2, s));
+        regk_replies_chain_count_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(p2);
+        regk_replies_chain_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(p2);
+        CK(cudaGetLastError());
+        launches += 2;
+    }
+    CK(cudaMemcpyAsync(hc, p.counters, CQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    if (hc[RQ_ERR] != ~0ull) {
+        const uint64_t k = hc[RQ_ERR] >> 8;
+        const uint32_t code = (uint32_t)(hc[RQ_ERR] & 0xFF);
+        unsigned long long dpos = 0;
+        CK(cudaMemcpyAsync(&dpos, p.data_pos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: byte %llu: %s; expected the getData reply to node %llu (xid %d)",
+            dpos - 24, reply_reason(code), (unsigned long long)k, (int32_t)((uint32_t)xb + (uint32_t)k));
+    }
+    if (hc[RQ_NREP] < f) {
+        uint64_t stop = 0;
+        if (pg.C) {
+            regk_replies_stop_kernel<<<(unsigned)((pg.C + 255) / 256), 256, 0, s>>>(pg);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(hc + RQ_STOP, p.counters + RQ_STOP, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            stop = hc[RQ_STOP];
+        }
+        const uint64_t done = hc[RQ_NREP];
+        uint8_t head[24] = {0};
+        const uint64_t avail = len - stop, take = std::min<uint64_t>(avail, sizeof head);
+        if (take) {
+            CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+        }
+        ReplyHead h;
+        const uint32_t code = reply_head(head, avail, xb, f, &h);
+        const int32_t want = (int32_t)((uint32_t)xb + (uint32_t)done);
+        if (code == RP_TRUNC)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: byte %llu: the stream ends before the getData reply to node "
+                                                   "%llu (xid %d) is complete; %llu of %llu replies complete",
+                        (unsigned long long)stop, (unsigned long long)done, want, (unsigned long long)done, (unsigned long long)f);
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: byte %llu: %s (len %d, xid %d); expected the getData reply to "
+                                               "node %llu (xid %d)", (unsigned long long)stop,
+                    code ? reply_reason(code) : "internal error", h.len, h.xid, (unsigned long long)done, want);
+    }
+    const uint64_t start = hc[RQ_CONSUMED], gd_skipped = hc[RQ_SKIP];
+    /* 2. the getChildren section from the getData section's end (regk_children.cuh), the listing's entries */
+    if ((rc = ensure_dev(ctx, wk.cword, nblk * 4 + 16)) || (rc = ensure_dev(ctx, wk.ctotals, totals_bytes)) ||
+        (rc = ensure_dev(ctx, wk.ctile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, wk.fpos, f8)) ||
+        (rc = ensure_dev(ctx, wk.fend, f8)) || (rc = ensure_dev(ctx, wk.cerr, f4)) || (rc = ensure_dev(ctx, wk.cnt, f4)) ||
+        (rc = ensure_dev(ctx, wk.seed_g, f4)) || (rc = ensure_dev(ctx, wk.last_g1, f4)) ||
+        (rc = ensure_dev(ctx, wk.name_bad, f4)) || (rc = ensure_dev(ctx, wk.end_pos, f8)) ||
+        (rc = ensure_dev(ctx, wk.fault_pos, f8)) || (rc = ensure_dev(ctx, wk.child_off, f8)))
+        return rc;
+    ChParams cp{};
+    RepParams &pc = cp.r;
+    pc.s = ds;
+    pc.len = len;
+    pc.xid_base = xc;
+    pc.n = f;
+    pc.word = (uint32_t *)wk.cword.p;
+    pc.tile_total = (uint32_t *)wk.ctotals.p;
+    pc.super_total = (unsigned long long *)((uint8_t *)wk.ctotals.p + align16(tiles_s * 4));
+    pc.tile_base = (unsigned long long *)wk.ctile_base.p;
+    pc.counters = p.counters;
+    cp.start = start;
+    cp.d = f;
+    cp.fpos = (unsigned long long *)wk.fpos.p;
+    cp.fend = (unsigned long long *)wk.fend.p;
+    cp.err = (int32_t *)wk.cerr.p;
+    cp.cnt = (uint32_t *)wk.cnt.p;
+    cp.seed_g = (uint32_t *)wk.seed_g.p;
+    cp.last_g1 = (uint32_t *)wk.last_g1.p;
+    cp.name_bad = (uint32_t *)wk.name_bad.p;
+    cp.end_pos = (unsigned long long *)wk.end_pos.p;
+    cp.fault_pos = (unsigned long long *)wk.fault_pos.p;
+    cp.child_off = (unsigned long long *)wk.child_off.p;
+    cp.dir_len = (const uint32_t *)wk.flen[cur].p;
+    const RepParams pc0 = pc;
+    CK(cudaMemsetAsync(p.counters, 0, CQ_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(p.counters + RQ_ERR, 0xFF, 8, s));
+    CK(cudaMemsetAsync(p.counters + CQ_ENT_ERR, 0xFF, 8, s));
+    CK(cudaMemsetAsync(pc.tile_total, 0, totals_bytes, s));
+    RepParams pf = pc;
+    if (len) {
+        regk_children_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(cp);
+        CK(cudaGetLastError());
+        launches++;
+        if ((rc = chain_pass(ctx, &pf, tiles_s, ~0ull, wk.ccand, wk.cmark, wk.cjump, [&](const RepParams &q) {
+                regk_children_seed_kernel<<<1, 256, 0, s>>>(q, nullptr, nullptr, 1, start);
+            }, &J, &launches, who)))
+            return rc;
+        if (pf.C) {
+            const uint64_t tiles_c = (pf.C + RP_TILE - 1) / RP_TILE;
+            const size_t t2 = align16(tiles_c * 4) + (tiles_c / SUPER + 1) * 8;
+            if ((rc = ensure_dev(ctx, wk.ctotals2, t2)))
+                return rc;
+            cp.r = pf;
+            cp.r.tile_total = (uint32_t *)wk.ctotals2.p;
+            cp.r.super_total = (unsigned long long *)((uint8_t *)wk.ctotals2.p + align16(tiles_c * 4));
+            CK(cudaMemsetAsync(wk.ctotals2.p, 0, t2, s));
+            regk_replies_chain_count_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(cp.r);
+            regk_children_chain_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(cp);
+            CK(cudaGetLastError());
+            launches += 2;
+        }
+    }
+    CK(cudaMemcpyAsync(hc, p.counters, CQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    const uint64_t frame_err_k = hc[RQ_ERR] != ~0ull ? hc[RQ_ERR] >> 8 : f;
+    const uint64_t d_eff = std::min<uint64_t>(std::min<uint64_t>(frame_err_k, hc[RQ_NREP]), f);
+    const uint64_t ch_skipped = hc[RQ_SKIP], n_listed = hc[RQ_FOUND], n_list_missing = hc[RQ_MISSING];
+    const uint64_t n_list_error = hc[RQ_ERROR], consumed = hc[RQ_CONSUMED];
+    uint64_t ne = 0, Ce = 0;
+    if (d_eff) {
+        cp.d_eff = d_eff;
+        if ((rc = ensure_dev(ctx, wk.eword, nblk * 4 + 16)) || (rc = ensure_dev(ctx, wk.etotals, totals_bytes)) ||
+            (rc = ensure_dev(ctx, wk.etile_base, tiles_s * 8 + 16)))
+            return rc;
+        RepParams pe = pc0;
+        pe.word = (uint32_t *)wk.eword.p;
+        pe.tile_total = (uint32_t *)wk.etotals.p;
+        pe.super_total = (unsigned long long *)((uint8_t *)wk.etotals.p + align16(tiles_s * 4));
+        pe.tile_base = (unsigned long long *)wk.etile_base.p;
+        CK(cudaMemsetAsync(pe.tile_total, 0, totals_bytes, s));
+        CK(cudaMemsetAsync(cp.seed_g, 0xFF, d_eff * 4, s));
+        CK(cudaMemsetAsync(cp.name_bad, 0xFF, d_eff * 4, s));
+        CK(cudaMemsetAsync(cp.last_g1, 0, d_eff * 4, s));
+        cp.r = pe;
+        regk_children_ent_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(cp);
+        CK(cudaGetLastError());
+        launches++;
+        const unsigned gd = (unsigned)((d_eff + 255) / 256);
+        if ((rc = chain_pass(ctx, &pe, tiles_s, hc[CQ_MAXC] + 1, wk.ecand, wk.emark, wk.ejump, [&](const RepParams &q) {
+                regk_children_seed_kernel<<<gd, 256, 0, s>>>(q, cp.fpos, cp.cnt, d_eff, 24ull);
+            }, &J, &launches, who)))
+            return rc;
+        Ce = pe.C;
+        /* the entries' listing path lengths go straight to the next frontier's lengths */
+        if ((rc = ensure_dev(ctx, wk.ent_pos, Ce * 8 + 16)) || (rc = ensure_dev(ctx, wk.ent_nlen, Ce * 4 + 16)) ||
+            (rc = ensure_dev(ctx, wk.ent_k, Ce * 4 + 16)) || (rc = ensure_dev(ctx, wk.flen[nx], Ce * 4 + 16)))
+            return rc;
+        cp.j0 = J;
+        cp.ent_pos = (unsigned long long *)wk.ent_pos.p;
+        cp.ent_nlen = (uint32_t *)wk.ent_nlen.p;
+        cp.ent_k = (uint32_t *)wk.ent_k.p;
+        cp.ent_plen = (uint32_t *)wk.flen[nx].p;
+        cp.r = pe;
+        if (Ce) {
+            const uint64_t tiles_e = (Ce + RP_TILE - 1) / RP_TILE;
+            const size_t t2 = align16(tiles_e * 4) + (tiles_e / SUPER + 1) * 8;
+            if ((rc = ensure_dev(ctx, wk.etotals2, t2)))
+                return rc;
+            cp.r.tile_total = (uint32_t *)wk.etotals2.p;
+            cp.r.super_total = (unsigned long long *)((uint8_t *)wk.etotals2.p + align16(tiles_e * 4));
+            CK(cudaMemsetAsync(wk.etotals2.p, 0, t2, s));
+            regk_children_ent_count_kernel<<<(unsigned)tiles_e, RP_TILE, 0, s>>>(cp.r);
+            regk_children_ent_kernel<<<(unsigned)tiles_e, RP_TILE, 0, s>>>(cp);
+            launches += 2;
+        }
+        regk_children_ent_frame_kernel<<<gd, 256, 0, s>>>(cp);
+        CK(cudaGetLastError());
+        launches++;
+        CK(cudaMemcpyAsync(hc, p.counters, CQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        ne = hc[CQ_NENT];
+    }
+    if (hc[CQ_ENT_ERR] != ~0ull) {
+        const uint64_t k = hc[CQ_ENT_ERR] >> 8;
+        const uint32_t code = (uint32_t)(hc[CQ_ENT_ERR] & 0xFF);
+        unsigned long long at[2] = {0, 0};
+        CK(cudaMemcpyAsync(&at[0], cp.fault_pos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&at[1], cp.fpos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: byte %llu: %s (entry of the reply frame at byte %llu); expected "
+                                               "the getChildren reply to node %llu (xid %d)", at[0], children_reason(code), at[1],
+                    (unsigned long long)k, (int32_t)((uint32_t)xc + (uint32_t)k));
+    }
+    if (hc[RQ_ERR] != ~0ull) {
+        const uint64_t k = hc[RQ_ERR] >> 8;
+        const uint32_t code = (uint32_t)(hc[RQ_ERR] & 0xFF);
+        unsigned long long pos = 0;
+        CK(cudaMemcpyAsync(&pos, cp.fpos + k, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: byte %llu: %s; expected the getChildren reply to node %llu "
+                                               "(xid %d)", pos, children_reason(code), (unsigned long long)k,
+                    (int32_t)((uint32_t)xc + (uint32_t)k));
+    }
+    if (hc[RQ_NREP] < f) {
+        uint64_t stop = start;
+        if (pf.C) {
+            regk_replies_stop_kernel<<<(unsigned)((pf.C + 255) / 256), 256, 0, s>>>(pf);
+            CK(cudaGetLastError());
+            CK(cudaMemcpyAsync(hc + RQ_STOP, p.counters + RQ_STOP, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            stop = std::max<uint64_t>(stop, hc[RQ_STOP]);
+        }
+        const uint64_t done = hc[RQ_NREP];
+        uint8_t head[24] = {0};
+        const uint64_t avail = len - stop, take = std::min<uint64_t>(avail, sizeof head);
+        if (take) {
+            CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+        }
+        ChildHead h;
+        const uint32_t code = children_head(head, avail, xc, f, &h);
+        const int32_t want = (int32_t)((uint32_t)xc + (uint32_t)done);
+        if (code == CH_TRUNC)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: byte %llu: the stream ends before the getChildren reply to "
+                                                   "node %llu (xid %d) is complete; %llu of %llu replies complete",
+                        (unsigned long long)stop, (unsigned long long)done, want, (unsigned long long)done, (unsigned long long)f);
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: byte %llu: %s (len %d, xid %d); expected the getChildren reply "
+                                               "to node %llu (xid %d)", (unsigned long long)stop,
+                    code ? children_reason(code) : "internal error", h.len, h.xid, (unsigned long long)done, want);
+    }
+    if (ne >= 0xFFFFFFFFull)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_read_walk: %llu children: must be below 2^32 - 1", (unsigned long long)ne);
+    /* 3. the next frontier: listing path e = frontier path + '/' + name, packed from 0 */
+    uint64_t lst_total = 0;
+    {
+        const uint64_t gt = (ne + MK_TILE - 1) / MK_TILE;
+        if ((rc = ensure_dev(ctx, wk.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)) ||
+            (rc = ensure_dev(ctx, wk.foff[nx], (ne + 1) * 8)) || (rc = ensure_dev(ctx, wk.flen[nx], ne * 4 + 16)))
+            return rc;
+        if (ne) {
+            MkGatherParams gp{};
+            gp.n_dirs = ne;
+            gp.dir_len = cp.ent_plen;
+            gp.tile_total = (unsigned long long *)wk.gtotals.p;
+            gp.super_total = gp.tile_total + gt;
+            CK(cudaMemsetAsync(gp.super_total, 0, (gt / SUPER + 1) * 8, s));
+            regk_mkdirp_len_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(gp);
+            std::vector<unsigned long long> gs(gt / SUPER + 1);
+            CK(cudaMemcpyAsync(gs.data(), gp.super_total, gs.size() * 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            for (unsigned long long v : gs)
+                lst_total += v;
+            if ((rc = ensure_dev(ctx, wk.fbytes[nx], lst_total + 16)))
+                return rc;
+            ChGatherParams g{};
+            g.n = ne;
+            g.tile_total = gp.tile_total;
+            g.super_total = gp.super_total;
+            g.ent_k = cp.ent_k;
+            g.ent_nlen = cp.ent_nlen;
+            g.ent_plen = cp.ent_plen;
+            g.ent_pos = cp.ent_pos;
+            g.dir_bytes = fbytes;
+            g.dir_off = foff;
+            g.s = ds;
+            g.out_bytes = (uint8_t *)wk.fbytes[nx].p;
+            g.out_off = (unsigned long long *)wk.foff[nx].p;
+            regk_children_gather_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(g);
+            CK(cudaGetLastError());
+            launches += 2;
+        } else {
+            if ((rc = ensure_dev(ctx, wk.fbytes[nx], 16)))
+                return rc;
+            CK(cudaMemsetAsync(wk.foff[nx].p, 0, 8, s));
+        }
+    }
+    /* 4. the level's nodes: the found getData replies in frontier order, with their stats */
+    const uint64_t tiles_r = (f + RP_TILE - 1) / RP_TILE;
+    const size_t ft_bytes = align16(tiles_r * 4) + (tiles_r / SUPER + 1) * 8;
+    if ((rc = ensure_dev(ctx, wk.ftotals, ft_bytes)) || (rc = ensure_dev(ctx, wk.node_rec, f8)) ||
+        (rc = ensure_dev(ctx, wk.node_ver, f4)) || (rc = ensure_dev(ctx, wk.node_own, f8)) ||
+        (rc = ensure_dev(ctx, wk.node_plen, f4)) || (rc = ensure_dev(ctx, wk.node_dlen, f4)) ||
+        (rc = ensure_dev(ctx, wk.wcount, WK_NCOUNTERS * 8)) || (rc = ensure_host(ctx, wk.h_wcount, WK_NCOUNTERS * 8)))
+        return rc;
+    WalkFoundParams fp{};
+    fp.f = f;
+    fp.err = p.err;
+    fp.dlen = p.dlen;
+    fp.ver = p.ver;
+    fp.own = p.own;
+    fp.path_off = foff;
+    fp.tile_total = (uint32_t *)wk.ftotals.p;
+    fp.super_total = (unsigned long long *)((uint8_t *)wk.ftotals.p + align16(tiles_r * 4));
+    fp.node_rec = (unsigned long long *)wk.node_rec.p;
+    fp.node_ver = (int32_t *)wk.node_ver.p;
+    fp.node_own = (long long *)wk.node_own.p;
+    fp.node_plen = (uint32_t *)wk.node_plen.p;
+    fp.node_dlen = (uint32_t *)wk.node_dlen.p;
+    fp.counters = (unsigned long long *)wk.wcount.p;
+    CK(cudaMemsetAsync(wk.ftotals.p, 0, ft_bytes, s));
+    CK(cudaMemsetAsync(fp.counters, 0, WK_NCOUNTERS * 8, s));
+    regk_walk_found_count_kernel<<<(unsigned)tiles_r, RP_TILE, 0, s>>>(fp);
+    regk_walk_found_kernel<<<(unsigned)tiles_r, RP_TILE, 0, s>>>(fp);
+    CK(cudaGetLastError());
+    launches += 2;
+    unsigned long long *hw = (unsigned long long *)wk.h_wcount.p;
+    CK(cudaMemcpyAsync(hw, fp.counters, WK_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    const uint64_t mf = hw[WK_FOUND], m0 = wk.m;
+    /* 5. the level's paths (from the frontier) and data (from the stream) packed, then appended to the snapshot */
+    uint64_t tot[2] = {0, 0};
+    for (int g = 0; g < 2; g++) {
+        uint32_t l = 0;
+        if ((rc = pack_strings(ctx, mf, g ? ds : fbytes, g ? p.data_pos : foff, fp.node_rec, g ? fp.node_dlen : fp.node_plen,
+                 wk.gtotals, wk.lvl_bytes[g], wk.lvl_off[g], &tot[g], &l)))
+            return rc;
+        launches += l;
+    }
+    const uint64_t at[2] = {wk.path_total, wk.data_total};
+    for (int g = 0; g < 2; g++)
+        if ((rc = walk_grow(ctx, wk.snap_bytes[g], at[g], at[g] + tot[g] + 16)) ||
+            (rc = walk_grow(ctx, wk.snap_off[g], m0 * 8, (m0 + mf + 1) * 8)))
+            return rc;
+    if ((rc = walk_grow(ctx, wk.ver, m0 * 4, (m0 + mf) * 4 + 16)) || (rc = walk_grow(ctx, wk.own, m0 * 8, (m0 + mf) * 8 + 16)))
+        return rc;
+    for (int g = 0; g < 2; g++) {
+        WalkAppendParams ap{};
+        ap.src = (const uint8_t *)wk.lvl_bytes[g].p;
+        ap.len = tot[g];
+        ap.dst = (uint8_t *)wk.snap_bytes[g].p;
+        ap.at = at[g];
+        ap.src_off = (const unsigned long long *)wk.lvl_off[g].p;
+        ap.n = mf;
+        ap.dst_off = (unsigned long long *)wk.snap_off[g].p + m0;
+        const uint64_t nb = (at[g] + tot[g] - (at[g] & ~15ull) + 15) / 16, th = std::max<uint64_t>(nb, mf + 1);
+        regk_walk_append_kernel<<<(unsigned)((th + 255) / 256), 256, 0, s>>>(ap);
+        CK(cudaGetLastError());
+        launches++;
+    }
+    if (mf) {
+        CK(cudaMemcpyAsync((int32_t *)wk.ver.p + m0, fp.node_ver, mf * 4, cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemcpyAsync((long long *)wk.own.p + m0, fp.node_own, mf * 8, cudaMemcpyDeviceToDevice, s));
+    }
+    CK(cudaEventRecord(wk.ev[1], s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, wk.ev[0], wk.ev[1]);
+    /* the level is in: the listing is the next frontier, unframed */
+    wk.m = m0 + mf;
+    wk.path_total += tot[0];
+    wk.data_total += tot[1];
+    wk.level_off.push_back(wk.m);
+    wk.cur = nx;
+    wk.f = ne;
+    wk.fpt = lst_total;
+    wk.framed = false;
+    out->level = wk.level_off.size() - 1;
+    out->m = wk.m;
+    out->n_frontier = ne;
+    out->n_found = hw[WK_FOUND];
+    out->n_missing = hw[WK_MISSING];
+    out->n_error = hw[WK_ERROR];
+    out->n_listed = n_listed;
+    out->n_list_missing = n_list_missing;
+    out->n_list_error = n_list_error;
+    out->n_children = ne;
+    out->n_skipped = gd_skipped + ch_skipped;
+    out->consumed = consumed;
+    out->flags = flags & REGK_OUT_DEVICE;
+    out->launches = launches;
+    out->level_off = wk.level_off.data();
+    out->snapshot.n = wk.m;
+    out->snapshot.flags = REGK_IN_DEVICE;
+    out->snapshot.path_total = wk.path_total;
+    out->snapshot.json_total = wk.data_total;
+    out->snapshot.path_bytes = (const uint8_t *)wk.snap_bytes[0].p;
+    out->snapshot.path_off = (const uint64_t *)wk.snap_off[0].p;
+    out->snapshot.json_bytes = (const uint8_t *)wk.snap_bytes[1].p;
+    out->snapshot.json_off = (const uint64_t *)wk.snap_off[1].p;
+    out->version = (const int32_t *)wk.ver.p;
+    out->ephemeral_owner = (const int64_t *)wk.own.p;
     out->kernel_ms = ms;
     return REGK_OK;
 }
