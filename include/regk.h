@@ -1295,6 +1295,57 @@ int         regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns
  * PARITY UNPINNED: the layouts are restated from zookeeper.jute and tested against an independent restatement, not
  * against a server.  A directory whose listing exceeds the server's jute.maxbuffer cannot be listed by any client, and
  * this call does not handle it.
+ *
+ * ---- a watched walk: keep the snapshot current with ZooKeeper watches, as Binder keeps its cache ---------------------
+ * regk_walk_requests(..., flags | REGK_ZK_WATCH, ...) writes the trailing watch byte of every frame of both sections as
+ *   1; nothing else changes, and without the flag every frame is what it was.  A walk is WATCHED while every level it
+ *   has read was framed with the flag (the last framing before each read counts); the two calls below refuse an
+ *   unwatched walk with REGK_ERR_STATE.  regk_walk_start drops the marks, the table and the refresh state.
+ * Each snapshot node carries two marks: PENDING (re-read it) and REMOVED (drop it).  n_pending counts the nodes that are
+ *   pending and not removed, n_removed the removed ones.
+ * regk_walk_events: the notifications in bytes[start, len), by exactly regk_read_events' frame rules (opts the same;
+ *   notifications, pings, replies in [xid_base, xid_base + n_xids) skipped and counted, a trailing partial frame,
+ *   the same refusals, nothing marked on a refusal).  Each event's path is looked up byte for byte among the snapshot's
+ *   nodes not marked REMOVED, as the call found them (an event never sees another event of the same call):
+ *     NodeDataChanged (3), NodeChildrenChanged (4)   node j becomes PENDING
+ *     NodeDeleted (2)                                 j is marked REMOVED (and leaves the pending set); the node at
+ *                                                     dirname(path), if it is a node not marked REMOVED, becomes PENDING
+ *     any other type, or no such node                 unmatched (node UINT64_MAX); types -1 and 5 .. 7 also count in
+ *                                                     n_other
+ *   REMOVED wins over PENDING whatever the events' order.  pos, type, state, zxid, node per event are pinned host
+ *   arrays, or device arrays with REGK_OUT_DEVICE, valid until the next call.  The path table is brought up to date on the first call
+ *   after the snapshot changed: the nodes a level appended are inserted, and after a rebuild (which renumbers the
+ *   nodes) or once the table would be over half full it is built anew.  table_nodes / table_ms report the nodes
+ *   inserted and that time (0 when the table was current), kernel_ms the rest.
+ * regk_walk_refresh (flags 0): on a watched walk with an empty frontier (else REGK_ERR_STATE), (1) drops every REMOVED
+ *   node, the survivors keeping their order, data, version, owner and marks; (2) makes the PENDING nodes, ascending, the
+ *   frontier of a REFRESH LEVEL and clears the marks; (3) reports n_removed, n_kept, n_frontier, and out->walk: the
+ *   walk as it now stands (level 0, level_off = {n_kept}).  No pending node: the walk stays complete.
+ * A refresh level is framed by regk_walk_requests as any level (getData and getChildren per node), and regk_read_walk
+ *   reads it with these differences:
+ *     getData err 0      the node's data, version and owner are replaced in place
+ *     getData NONODE     the node is REMOVED; any other err keeps it unchanged (n_error)
+ *     getChildren err 0  only the listed children whose path is not a node of the snapshot after this read's
+ *                        removals become the next frontier (frontier order, then listing order)
+ *     the snapshot       rebuilt once, without every REMOVED node; node ids may change, marks move with their nodes
+ *     level_off          {m}: level 0 is the nodes kept from before the refresh, and `level` counts the levels
+ *                        appended since (a walk that is never refreshed reports what it always did)
+ *   The plain levels after a refresh append as before, but drop every listed child whose path is a node of the snapshot
+ *   (REMOVED or not), so the snapshot never holds one path twice and regk_resolve accepts it.
+ * ORDERING RULE: every byte the session delivers goes through regk_walk_events exactly once, and bytes that also hold
+ *   replies to a walk framing go through regk_read_walk first.  A watch exists only after its read was processed, so a
+ *   notification always follows the reply that armed it, and reading replies first maps every event to a present node.
+ * WHY NodeDeleted MAKES THE PARENT PENDING: a refresh reads its replies before the events of the same stream.  If node p
+ *   is deleted and recreated and its parent g (its child watch already spent) is re-listed after both, g's listing shows
+ *   p while the old p is still present, so the new p reads as known; p's NodeDeleted then removes it, and g's child
+ *   watch will not fire again.  Making g pending re-lists g once p is gone, so the new p is walked.  A deleted ROOT has
+ *   no watched parent: it stays gone until a new walk.
+ * CONVERGENCE: once the tree stops changing and every byte has been fed, refreshing until nothing is pending or removed
+ *   leaves a snapshot equal, as a set of (path, data, version, owner), to a fresh walk of the same roots (deleted roots
+ *   aside); node order differs.  Re-resolve it (regk_resolve is not incremental).  After a reconnect, start a new
+ *   watched walk: the walk has no SetWatches.
+ * PARITY UNPINNED: restated from zookeeper.jute (WatcherEvent) and the server's watch rules (one-shot, per session; a
+ *   getData on a missing node arms nothing; a watch still armed is not duplicated), not tested against a server.
  */
 typedef struct regk_walk {
     uint64_t level;                 /* levels read so far */
@@ -1316,6 +1367,35 @@ typedef struct regk_walk {
 int         regk_walk_start(regk_ctx *ctx, const uint8_t *roots, const uint64_t *root_off, uint64_t n_roots, uint32_t flags);
 int         regk_walk_requests(regk_ctx *ctx, int32_t xid_base, uint32_t flags, regk_frames *out);
 int         regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t flags, regk_walk *out);
+
+typedef struct regk_walk_events_out {
+    uint64_t n_events, n_pings, n_replies;
+    uint64_t n_unmatched, n_other;
+    uint64_t consumed;              /* end of the last complete frame (start when none) */
+    uint64_t n_pending, n_removed;  /* after the call */
+    uint64_t table_nodes;           /* nodes this call inserted into the path table; 0: it was current */
+    uint32_t partial;               /* 1: a frame starts at consumed and the stream ends inside it */
+    uint32_t flags, launches;       /* REGK_OUT_DEVICE */
+    uint32_t reserved;
+    const uint64_t *pos;            /* [n_events] the frame's first byte */
+    const int32_t  *type;           /* WatcherEvent.type */
+    const int32_t  *state;          /* WatcherEvent.state */
+    const int64_t  *zxid;           /* ReplyHeader.zxid */
+    const uint64_t *node;           /* the snapshot node, or UINT64_MAX */
+    float kernel_ms;                /* the events, without the table build */
+    float table_ms;                 /* the table build */
+} regk_walk_events_out;
+
+typedef struct regk_walk_refresh_out {
+    uint64_t n_removed, n_kept, n_frontier;
+    uint32_t flags, launches;
+    regk_walk walk;                 /* the walk after the refresh: level 0, level_off {n_kept}, the compacted snapshot */
+    float kernel_ms;
+} regk_walk_refresh_out;
+
+int         regk_walk_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, const regk_events_opts *opts,
+                             regk_walk_events_out *out);
+int         regk_walk_refresh(regk_ctx *ctx, uint32_t flags, regk_walk_refresh_out *out);
 
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);

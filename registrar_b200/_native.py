@@ -589,6 +589,51 @@ class Walk:
         return Replies.snapshot(self)
 
 
+class CWalkEvents(C.Structure):      # regk_walk_events_out
+    _fields_ = [("n_events", C.c_uint64), ("n_pings", C.c_uint64), ("n_replies", C.c_uint64),
+                ("n_unmatched", C.c_uint64), ("n_other", C.c_uint64), ("consumed", C.c_uint64),
+                ("n_pending", C.c_uint64), ("n_removed", C.c_uint64), ("table_nodes", C.c_uint64),
+                ("partial", C.c_uint32), ("flags", C.c_uint32), ("launches", C.c_uint32), ("reserved", C.c_uint32),
+                ("pos", C.c_void_p), ("type", C.c_void_p), ("state", C.c_void_p), ("zxid", C.c_void_p),
+                ("node", C.c_void_p), ("kernel_ms", C.c_float), ("table_ms", C.c_float)]
+
+
+class WalkEvents:
+    """What walk_events() made of one piece of the session stream: event e (stream order) has pos[e], type, state, zxid
+    and node[e], the snapshot node its path names (UINT64_MAX: unmatched).  Counts n_events, n_pings, n_replies,
+    n_unmatched, n_other; `consumed` and `partial`; n_pending / n_removed after the call; table_nodes / table_ms the path
+    table build this call made (0 when it was current), kernel_ms the rest."""
+
+    def __init__(self, out):
+        n = int(out.n_events)
+        self.n_events, self.n_pings, self.n_replies = n, int(out.n_pings), int(out.n_replies)
+        self.n_unmatched, self.n_other = int(out.n_unmatched), int(out.n_other)
+        self.consumed, self.partial = int(out.consumed), bool(out.partial)
+        self.n_pending, self.n_removed = int(out.n_pending), int(out.n_removed)
+        self.table_nodes, self.table_ms = int(out.table_nodes), float(out.table_ms)
+        self.launches, self.kernel_ms = int(out.launches), float(out.kernel_ms)
+        self.pos = _as_np(out.pos, n, np.uint64).copy()
+        self.type = _as_np(out.type, n, np.int32).copy()
+        self.state = _as_np(out.state, n, np.int32).copy()
+        self.zxid = _as_np(out.zxid, n, np.int64).copy()
+        self.node = _as_np(out.node, n, np.uint64).copy()
+
+
+class CWalkRefresh(C.Structure):     # regk_walk_refresh_out
+    _fields_ = [("n_removed", C.c_uint64), ("n_kept", C.c_uint64), ("n_frontier", C.c_uint64), ("flags", C.c_uint32),
+                ("launches", C.c_uint32), ("walk", CWalk), ("kernel_ms", C.c_float)]
+
+
+class WalkRefresh:
+    """What walk_refresh() did: n_removed nodes dropped, n_kept kept, n_frontier pending nodes made the refresh level's
+    frontier; `walk` is the walk as it now stands (a Walk at level 0)."""
+
+    def __init__(self, ctx, out):
+        self.n_removed, self.n_kept, self.n_frontier = int(out.n_removed), int(out.n_kept), int(out.n_frontier)
+        self.launches, self.kernel_ms = int(out.launches), float(out.kernel_ms)
+        self.walk = Walk(ctx, out.walk)
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -604,7 +649,7 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results", "regk_read_stats",
            "regk_reconcile_stats", "regk_read_events", "regk_events_requests",
            "regk_setwatches_requests", "regk_resolve", "regk_dns_answer", "regk_walk_start", "regk_walk_requests",
-           "regk_read_walk"]
+           "regk_read_walk", "regk_walk_events", "regk_walk_refresh"]
 
 _lib = None
 
@@ -675,6 +720,8 @@ def load_library():
     lib.regk_walk_start.argtypes = [vp, vp, vp, u64, u32]
     lib.regk_walk_requests.argtypes = [vp, C.c_int32, u32, C.POINTER(CFrames)]
     lib.regk_read_walk.argtypes = [vp, vp, u64, u32, C.POINTER(CWalk)]
+    lib.regk_walk_events.argtypes = [vp, vp, u64, u64, C.POINTER(CEventsOpts), C.POINTER(CWalkEvents)]
+    lib.regk_walk_refresh.argtypes = [vp, u32, C.POINTER(CWalkRefresh)]
     _lib = lib
     return lib
 
@@ -1297,13 +1344,13 @@ class Context:
         np.cumsum([len(r) for r in roots], out=off[1:])
         self._check(self._lib.regk_walk_start(self._h, _np_ptr(b), _np_ptr(off), len(roots), 0))
 
-    def walk_requests(self, xid_base: int = 1, device: bool = False):
+    def walk_requests(self, xid_base: int = 1, device: bool = False, watch: bool = False):
         """regk_walk_requests: a getData frame per node of the walk's current frontier, then a getChildren frame per
-        node, xids from xid_base on.  Returns (frame_bytes, frame_off uint64[2f+1], kernel_ms), or the raw CFrames with
-        device=True."""
+        node, xids from xid_base on; watch=True arms a watch with every read.  Returns (frame_bytes, frame_off
+        uint64[2f+1], kernel_ms), or the raw CFrames with device=True."""
         out = CFrames()
-        rc = self._lib.regk_walk_requests(self._h, (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31,
-                                          FLAG_OUT_DEVICE if device else 0, C.byref(out))
+        flags = (FLAG_OUT_DEVICE if device else 0) | (FLAG_ZK_WATCH if watch else 0)
+        rc = self._lib.regk_walk_requests(self._h, (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31, flags, C.byref(out))
         self._check(rc)
         if device:
             return out
@@ -1333,21 +1380,69 @@ class Context:
         self._check(rc)
         return out if device else Walk(self, out)
 
-    def walk(self, roots, exchange, xid_base: int = 1):
+    def walk(self, roots, exchange, xid_base: int = 1, watch: bool = False):
         """The whole walk from `roots`: each level's frames go to exchange(frame_bytes) -> reply stream (the caller's
         session), and the replies are read, until no level is left.  Each level's xids follow the last level's, skipping
-        to 0 where a range would cover -1 or -2.  Returns the last level's Walk (the whole snapshot)."""
+        to 0 where a range would cover -1 or -2.  With watch=True every read arms a watch and each level's stream also
+        goes through walk_events() (after read_walk(), with that level's xids as the reply range), so refresh_walk() can
+        keep the snapshot current; exchange must then return whole frames (a stream that ends inside a notification is
+        a ValueError, after the level was read).  Returns the last level's Walk (the whole snapshot)."""
         self.walk_start(roots)
-        xid, f = int(xid_base) % 2 ** 32, len(roots)
-        while True:
+        return self._walk_levels(exchange, int(xid_base) % 2 ** 32, len(roots), watch)[0]
+
+    def _walk_levels(self, exchange, xid, f, watch, w=None):
+        while f:
             if any((r - xid) % 2 ** 32 < 2 * f for r in (2 ** 32 - 1, 2 ** 32 - 2)):
                 xid = 0
-            fb, _, _ = self.walk_requests(xid)
+            fb, _, _ = self.walk_requests(xid, watch=watch)
             s = exchange(fb)
-            w = self.read_walk(np.frombuffer(s, np.uint8) if isinstance(s, (bytes, bytearray)) else s)
+            s = np.frombuffer(s, np.uint8) if isinstance(s, (bytes, bytearray)) else s
+            w = self.read_walk(s)
+            if watch and self.walk_events(s, xid_base=xid, n_xids=2 * f).partial:
+                raise ValueError("exchange returned bytes that end inside a frame: return whole frames, so that every "
+                                 "notification goes through walk_events exactly once")
             xid, f = (xid + 2 * f) % 2 ** 32, w.n_frontier
-            if f == 0:
-                return w
+        return w, xid
+
+    def walk_events(self, stream, start: int = 0, xid_base: int = 0, n_xids: int = 0, device: bool = False):
+        """regk_walk_events: the watch notifications in `stream` (a NumPy uint8 array, or a contiguous CUDA uint8 tensor)
+        from byte `start` on, mapped to the nodes of the watched walk's snapshot: NodeDataChanged and NodeChildrenChanged
+        make a node pending, NodeDeleted marks it removed and makes its parent pending.  Pings and replies to the
+        [xid_base, xid_base + n_xids) requests are skipped.  Returns a WalkEvents, or the raw CWalkEvents (arrays on the
+        device) with device=True."""
+        flags = FLAG_OUT_DEVICE if device else 0
+        if hasattr(stream, "data_ptr"):
+            import torch
+            if not stream.is_cuda or stream.dtype != torch.uint8 or not stream.is_contiguous():
+                raise ValueError("a device stream is a contiguous CUDA uint8 tensor")
+            keep, ptr, n = stream, stream.data_ptr() or None, stream.numel()
+            flags |= FLAG_IN_DEVICE
+        else:
+            keep = np.ascontiguousarray(stream)
+            if keep.dtype != np.uint8 or keep.ndim != 1:
+                raise ValueError("a host stream is a one-dimensional uint8 array")
+            ptr, n = _np_ptr(keep), keep.size
+        xid = (int(xid_base) + 2 ** 31) % 2 ** 32 - 2 ** 31
+        o = CEventsOpts(xid, int(n_xids), flags, 0)
+        out = CWalkEvents()
+        rc = self._lib.regk_walk_events(self._h, ptr, n, int(start), C.byref(o), C.byref(out))
+        del keep
+        self._check(rc)
+        return out if device else WalkEvents(out)
+
+    def walk_refresh(self):
+        """regk_walk_refresh: on a complete watched walk, drop the removed nodes and make the pending ones the frontier
+        of a refresh level (read it with walk_requests() / read_walk() as any level).  Returns a WalkRefresh."""
+        out = CWalkRefresh()
+        self._check(self._lib.regk_walk_refresh(self._h, 0, C.byref(out)))
+        return WalkRefresh(self, out)
+
+    def refresh_walk(self, exchange, xid_base: int = 1):
+        """walk_refresh(), then the refresh level and the levels under it as walk(..., watch=True) runs them.  Returns
+        (WalkRefresh, the Walk as it stands after the last level)."""
+        r = self.walk_refresh()
+        w, _ = self._walk_levels(exchange, int(xid_base) % 2 ** 32, r.n_frontier, True, r.walk)
+        return r, w
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

@@ -42,6 +42,7 @@
 #include "regk_resolve.cuh"
 #include "regk_dns.cuh"
 #include "regk_walk.cuh"
+#include "regk_walk_watch.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -374,6 +375,21 @@ struct regk_ctx {
         DevBuf ftotals, node_rec, node_ver, node_own, node_plen, node_dlen, wcount, gtotals, lvl_bytes[2], lvl_off[2];
         HostBuf h_count, h_wcount;
         Event ev[2];
+        /* watches (regk_walk_watch.cuh).  watched: every level read was framed with REGK_ZK_WATCH (framed_watch: the
+           current framing was); refreshed: a regk_walk_refresh ran since the start (listings are then filtered);
+           rlevel: the frontier is a refresh level, frontier node i being snapshot node fnode[i].  The marks and their
+           counts (mcount: pending, removed) per node; the path table holds nodes [0, tab_m) and is valid while
+           tab_rgen == rgen (rgen counts the rebuilds, which renumber the nodes).  The rebuild writes the other set of
+           snapshot arrays and swaps. */
+        bool watched = true, framed_watch = false, refreshed = false, rlevel = false, tab_valid = false;
+        uint64_t rgen = 0, tab_rgen = 0, tab_m = 0, n_pending = 0, n_removed = 0;
+        uint32_t tab_mask = 0;
+        DevBuf wmark, mcount, table, fnode, rpos, rlen, snap2_bytes[2], snap2_off[2], ver2, own2, wmark2;
+        DevBuf ktotals, kcount, psrc, dsrc, kplen, kdlen, dsel, xkeep, xtotals, xrec, xlen, xcount, xbytes, xoff;
+        DevBuf vstream, vword, vtotals, vtile_base, vcand, vmark, vjump, vcount, vntotals, e_pos, e_type, e_state, e_zxid,
+            e_node, e_parent;
+        HostBuf h_epos, h_etype, h_estate, h_ezxid, h_enode, h_vcount;
+        Event eev[4];
     } wk;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
@@ -6132,6 +6148,259 @@ static int walk_grow(regk_ctx *ctx, DevBuf &b, size_t used, size_t need)
     return REGK_OK;
 }
 
+/* The walk's path table over its current snapshot (regk_walk_insert_kernel: node + 1 under the hash of its path).  A
+   table stays valid while the snapshot only grows (rgen counts the rebuilds, which renumber nodes): the nodes appended
+   since it was built are inserted while the table still has twice as many slots as nodes, else it is built anew.
+   *built = the nodes inserted this call (0: it was current). */
+static int walk_table(regk_ctx *ctx, uint64_t *built, uint32_t *launches, const char *who)
+{
+    regk_ctx::Walk &wk = ctx->wk;
+    cudaStream_t s = ctx->stream;
+    const uint64_t m = wk.m;
+    int rc;
+    *built = 0;
+    const bool valid = wk.tab_valid && wk.tab_rgen == wk.rgen;
+    if (valid && wk.tab_m == m)
+        return REGK_OK;
+    uint64_t j0 = 0;
+    if (valid && 2 * m <= (uint64_t)wk.tab_mask + 1) {
+        j0 = wk.tab_m;
+    } else {
+        uint64_t sr = 1024;
+        while (sr < 2 * m)
+            sr <<= 1;
+        if (sr > (1ull << 32))
+            return fail(ctx, REGK_ERR_INVALID_ARG, "%s: a snapshot of %llu nodes is too large for one table", who,
+                (unsigned long long)m);
+        if ((rc = ensure_dev(ctx, wk.table, sr * 4)))
+            return rc;
+        CK(cudaMemsetAsync(wk.table.p, 0, sr * 4, s));
+        wk.tab_mask = (uint32_t)(sr - 1);
+    }
+    if (m > j0) {
+        regk_walk_insert_kernel<<<(unsigned)((m - j0 + 255) / 256), 256, 0, s>>>((uint32_t *)wk.table.p, wk.tab_mask,
+            (const uint8_t *)wk.snap_bytes[0].p, (const unsigned long long *)wk.snap_off[0].p, j0, m);
+        CK(cudaGetLastError());
+        (*launches)++;
+    }
+    wk.tab_m = m;
+    wk.tab_rgen = wk.rgen;
+    wk.tab_valid = true;
+    *built = m - j0;
+    return REGK_OK;
+}
+
+/* Every buffer walk_filter needs for n listed paths of `total` bytes, so that it cannot fail on an allocation once a
+   refresh level's replies have been applied (pack_strings then finds its buffers large enough). */
+static int walk_filter_reserve(regk_ctx *ctx, uint64_t n, uint64_t total)
+{
+    regk_ctx::Walk &wk = ctx->wk;
+    const uint64_t tiles = (n + RP_TILE - 1) / RP_TILE, gt = (n + MK_TILE - 1) / MK_TILE;
+    const size_t tb = align16(tiles * 4) + (tiles / SUPER + 1) * 8;
+    int rc;
+    if ((rc = ensure_dev(ctx, wk.xtotals, tb)) || (rc = ensure_dev(ctx, wk.xkeep, n + 16)) ||
+        (rc = ensure_dev(ctx, wk.xrec, n * 8 + 16)) || (rc = ensure_dev(ctx, wk.xlen, n * 4 + 16)) ||
+        (rc = ensure_dev(ctx, wk.xcount, 16)) || (rc = ensure_dev(ctx, wk.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)) ||
+        (rc = ensure_dev(ctx, wk.xoff, (n + 1) * 8)) || (rc = ensure_dev(ctx, wk.xbytes, total + 16)))
+        return rc;
+    return REGK_OK;
+}
+
+/* Every buffer walk_rebuild needs for the current snapshot, whose data may take up to `extra` more bytes from a reply
+   stream. */
+static int walk_rebuild_reserve(regk_ctx *ctx, uint64_t extra)
+{
+    regk_ctx::Walk &wk = ctx->wk;
+    const uint64_t m = wk.m, tiles = (m + RP_TILE - 1) / RP_TILE, gt = (m + MK_TILE - 1) / MK_TILE;
+    const size_t tb = align16(tiles * 4) + (tiles / SUPER + 1) * 8;
+    const size_t m8 = m * 8 + 16, m4 = m * 4 + 16;
+    int rc;
+    if ((rc = ensure_dev(ctx, wk.ktotals, tb)) || (rc = ensure_dev(ctx, wk.kcount, 16)) || (rc = ensure_dev(ctx, wk.psrc, m8)) ||
+        (rc = ensure_dev(ctx, wk.dsrc, m8)) || (rc = ensure_dev(ctx, wk.kplen, m4)) || (rc = ensure_dev(ctx, wk.kdlen, m4)) ||
+        (rc = ensure_dev(ctx, wk.dsel, m + 16)) || (rc = ensure_dev(ctx, wk.wmark2, m4)) || (rc = ensure_dev(ctx, wk.ver2, m4)) ||
+        (rc = ensure_dev(ctx, wk.own2, m8)) || (rc = ensure_dev(ctx, wk.rpos, m8)) || (rc = ensure_dev(ctx, wk.rlen, m4)) ||
+        (rc = ensure_dev(ctx, wk.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)))
+        return rc;
+    const uint64_t bytes[2] = {wk.path_total, wk.data_total + extra};
+    for (int g = 0; g < 2; g++)
+        if ((rc = ensure_dev(ctx, wk.snap2_off[g], (m + 1) * 8 + 16)) || (rc = ensure_dev(ctx, wk.snap2_bytes[g], bytes[g] + 16)))
+            return rc;
+    return REGK_OK;
+}
+
+/* The n listed paths of frontier set nx without those the snapshot holds (skip_removed: holds unmarked), repacked in
+   listing order as that frontier; *kept / *total = the entries and bytes left. */
+static int walk_filter(regk_ctx *ctx, int nx, uint64_t n, bool skip_removed, uint64_t *kept, uint64_t *total,
+    uint32_t *launches, const char *who)
+{
+    regk_ctx::Walk &wk = ctx->wk;
+    cudaStream_t s = ctx->stream;
+    uint64_t built;
+    int rc;
+    if ((rc = walk_table(ctx, &built, launches, who)) || (rc = walk_filter_reserve(ctx, n, *total)))
+        return rc;
+    const uint64_t tiles = (n + RP_TILE - 1) / RP_TILE;
+    const size_t tb = align16(tiles * 4) + (tiles / SUPER + 1) * 8;
+    WalkFilterParams fp{};
+    fp.n = n;
+    fp.lbytes = (const uint8_t *)wk.fbytes[nx].p;
+    fp.loff = (const unsigned long long *)wk.foff[nx].p;
+    fp.ltotal = *total;
+    fp.spath = (const uint8_t *)wk.snap_bytes[0].p;
+    fp.soff = (const unsigned long long *)wk.snap_off[0].p;
+    fp.table = (const uint32_t *)wk.table.p;
+    fp.mask = wk.tab_mask;
+    fp.mark = (const uint32_t *)wk.wmark.p;
+    fp.skip_removed = skip_removed ? 1u : 0u;
+    fp.tile_total = (uint32_t *)wk.xtotals.p;
+    fp.super_total = (unsigned long long *)((uint8_t *)wk.xtotals.p + align16(tiles * 4));
+    fp.keep = (uint8_t *)wk.xkeep.p;
+    fp.rec = (unsigned long long *)wk.xrec.p;
+    fp.len = (uint32_t *)wk.xlen.p;
+    fp.count = (unsigned long long *)wk.xcount.p;
+    CK(cudaMemsetAsync(wk.xtotals.p, 0, tb, s));
+    regk_walk_filter_count_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(fp);
+    regk_walk_filter_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(fp);
+    CK(cudaGetLastError());
+    *launches += 2;
+    unsigned long long k = 0;
+    CK(cudaMemcpyAsync(&k, fp.count, 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    if ((rc = pack_strings(ctx, k, fp.lbytes, fp.loff, fp.rec, fp.len, wk.gtotals, wk.xbytes, wk.xoff, total, launches)))
+        return rc;
+    if (k)
+        CK(cudaMemcpyAsync(wk.flen[nx].p, fp.len, k * 4, cudaMemcpyDeviceToDevice, s));
+    std::swap(wk.fbytes[nx], wk.xbytes);
+    std::swap(wk.foff[nx], wk.xoff);
+    *kept = k;
+    return REGK_OK;
+}
+
+/* n items (item k: len[k] bytes at src_off[k] of src1 where sel[k], else of src0) packed into bytes / off by
+   regk_mkdirp_len_kernel's totals and the rebuild gather; *total = their bytes. */
+static int walk_pack(regk_ctx *ctx, uint64_t n, const uint8_t *src0, const uint8_t *src1, const unsigned long long *src_off,
+    const uint8_t *sel, const uint32_t *len, DevBuf &bytes, DevBuf &off, uint64_t *total, uint32_t *launches)
+{
+    regk_ctx::Walk &wk = ctx->wk;
+    cudaStream_t s = ctx->stream;
+    const uint64_t gt = (n + MK_TILE - 1) / MK_TILE;
+    int rc;
+    *total = 0;
+    if ((rc = ensure_dev(ctx, wk.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)) || (rc = ensure_dev(ctx, off, (n + 1) * 8 + 16)))
+        return rc;
+    if (!n) {
+        if ((rc = ensure_dev(ctx, bytes, 16)))
+            return rc;
+        CK(cudaMemsetAsync(off.p, 0, 8, s));
+        return REGK_OK;
+    }
+    MkGatherParams gp{};
+    gp.n_dirs = n;
+    gp.dir_len = len;
+    gp.tile_total = (unsigned long long *)wk.gtotals.p;
+    gp.super_total = gp.tile_total + gt;
+    CK(cudaMemsetAsync(gp.super_total, 0, (gt / SUPER + 1) * 8, s));
+    regk_mkdirp_len_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(gp);
+    std::vector<unsigned long long> gs(gt / SUPER + 1);
+    CK(cudaMemcpyAsync(gs.data(), gp.super_total, gs.size() * 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    for (unsigned long long v : gs)
+        *total += v;
+    if ((rc = ensure_dev(ctx, bytes, *total + 16)))
+        return rc;
+    WalkRebuildParams rp{};
+    rp.n = n;
+    rp.src0 = src0;
+    rp.src1 = src1;
+    rp.src_off = src_off;
+    rp.sel = sel;
+    rp.len = len;
+    rp.tile_total = gp.tile_total;
+    rp.super_total = gp.super_total;
+    rp.out = (uint8_t *)bytes.p;
+    rp.out_off = (unsigned long long *)off.p;
+    regk_walk_rebuild_kernel<<<(unsigned)gt, MK_TILE, 0, s>>>(rp);
+    CK(cudaGetLastError());
+    *launches += 2;
+    return REGK_OK;
+}
+
+/* The snapshot without its removed nodes, in order, their marks, versions and owners moving with them; a node marked
+   replaced takes its data from `ds` (a refresh level's reply stream).  The pending count is recounted, the removed count
+   is 0, and the path table is stale. */
+static int walk_rebuild(regk_ctx *ctx, const uint8_t *ds, uint32_t *launches, const char *who)
+{
+    regk_ctx::Walk &wk = ctx->wk;
+    cudaStream_t s = ctx->stream;
+    const uint64_t m = wk.m;
+    const uint64_t tiles = (m + RP_TILE - 1) / RP_TILE;
+    const size_t tb = align16(tiles * 4) + (tiles / SUPER + 1) * 8;
+    int rc;
+    if ((rc = walk_rebuild_reserve(ctx, 0)))
+        return rc;
+    unsigned long long kc[2] = {0, 0};
+    CK(cudaMemsetAsync(wk.kcount.p, 0, 16, s));
+    WalkKeepParams kp{};
+    kp.m = m;
+    kp.mark = (const uint32_t *)wk.wmark.p;
+    kp.path_off = (const unsigned long long *)wk.snap_off[0].p;
+    kp.json_off = (const unsigned long long *)wk.snap_off[1].p;
+    kp.ver = (const int32_t *)wk.ver.p;
+    kp.own = (const long long *)wk.own.p;
+    kp.rpos = (const unsigned long long *)wk.rpos.p;
+    kp.rlen = (const uint32_t *)wk.rlen.p;
+    kp.tile_total = (uint32_t *)wk.ktotals.p;
+    kp.super_total = (unsigned long long *)((uint8_t *)wk.ktotals.p + align16(tiles * 4));
+    kp.counters = (unsigned long long *)wk.kcount.p;
+    kp.psrc = (unsigned long long *)wk.psrc.p;
+    kp.dsrc = (unsigned long long *)wk.dsrc.p;
+    kp.plen = (uint32_t *)wk.kplen.p;
+    kp.dlen = (uint32_t *)wk.kdlen.p;
+    kp.dsel = (uint8_t *)wk.dsel.p;
+    kp.nmark = (uint32_t *)wk.wmark2.p;
+    kp.nver = (int32_t *)wk.ver2.p;
+    kp.nown = (long long *)wk.own2.p;
+    if (m) {
+        CK(cudaMemsetAsync(wk.ktotals.p, 0, tb, s));
+        regk_walk_keep_count_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(kp);
+        regk_walk_keep_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(kp);
+        CK(cudaGetLastError());
+        *launches += 2;
+        CK(cudaMemcpyAsync(kc, kp.counters, 16, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+    }
+    const uint64_t k = kc[0];
+    uint64_t tot[2] = {0, 0};
+    for (int g = 0; g < 2; g++)
+        if ((rc = walk_pack(ctx, k, (const uint8_t *)wk.snap_bytes[g].p, g ? ds : nullptr, g ? kp.dsrc : kp.psrc,
+                 g ? kp.dsel : nullptr, g ? kp.dlen : kp.plen, wk.snap2_bytes[g], wk.snap2_off[g], &tot[g], launches)))
+            return rc;
+    for (int g = 0; g < 2; g++) {
+        std::swap(wk.snap_bytes[g], wk.snap2_bytes[g]);
+        std::swap(wk.snap_off[g], wk.snap2_off[g]);
+    }
+    std::swap(wk.wmark, wk.wmark2);
+    std::swap(wk.ver, wk.ver2);
+    std::swap(wk.own, wk.own2);
+    const unsigned long long mc[WM_NCOUNTERS] = {kc[1], 0ull};
+    CK(cudaMemcpyAsync(wk.mcount.p, mc, sizeof mc, cudaMemcpyHostToDevice, s));
+    CK(cudaStreamSynchronize(s));
+    wk.m = k;
+    wk.path_total = tot[0];
+    wk.data_total = tot[1];
+    wk.n_pending = kc[1];
+    wk.n_removed = 0;
+    wk.rgen++;
+    return REGK_OK;
+}
+
+static int walk_append(regk_ctx *ctx, const uint8_t *ds, const uint8_t *fbytes, const unsigned long long *foff,
+    const unsigned long long *data_pos, const WalkFoundParams &fp, uint64_t mf, uint32_t *launches);
+static int walk_out(regk_ctx *ctx, const unsigned long long *hw, uint64_t ne, uint64_t n_listed, uint64_t n_list_missing,
+    uint64_t n_list_error, uint64_t n_skipped, uint64_t consumed, uint32_t flags, uint32_t launches, float ms, regk_walk *out);
+
 int regk_walk_start(regk_ctx *ctx, const uint8_t *roots, const uint64_t *root_off, uint64_t n_roots, uint32_t flags)
 {
     if (!ctx || !root_off || (!roots && n_roots))
@@ -6184,13 +6453,21 @@ int regk_walk_start(regk_ctx *ctx, const uint8_t *roots, const uint64_t *root_of
     cudaStream_t s = ctx->stream;
     int rc;
     if ((rc = stage_in(ctx, wk.fbytes[0], pb.data(), pb.size(), s)) || (rc = stage_in(ctx, wk.foff[0], po.data(), po.size() * 8, s)) ||
-        (rc = stage_in(ctx, wk.flen[0], pl.data(), pl.size() * 4, s)) || (rc = sync_or_fail(ctx, s, "regk_walk_start")))
+        (rc = stage_in(ctx, wk.flen[0], pl.data(), pl.size() * 4, s)) || (rc = ensure_dev(ctx, wk.mcount, WM_NCOUNTERS * 8)))
+        return rc;
+    CK(cudaMemsetAsync(wk.mcount.p, 0, WM_NCOUNTERS * 8, s));
+    if ((rc = sync_or_fail(ctx, s, "regk_walk_start")))
         return rc;
     wk.cur = 0;
     wk.f = n_roots;
     wk.fpt = pb.size();
     wk.m = wk.path_total = wk.data_total = 0;
     wk.level_off.assign(1, 0);
+    /* the marks, the table and the refresh state go with the earlier walk */
+    wk.watched = true;
+    wk.framed_watch = wk.refreshed = wk.rlevel = wk.tab_valid = false;
+    wk.n_pending = wk.n_removed = 0;
+    wk.rgen++;
     wk.active = true;
     return REGK_OK;
 }
@@ -6201,7 +6478,7 @@ int regk_walk_requests(regk_ctx *ctx, int32_t xid_base, uint32_t flags, regk_fra
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_requests: NULL argument");
     memset(out, 0, sizeof *out);
     regk_ctx::Walk &wk = ctx->wk;
-    if (flags & ~REGK_OUT_DEVICE)
+    if (flags & ~(REGK_OUT_DEVICE | REGK_ZK_WATCH))
         return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_requests: unknown flags 0x%x", flags);
     if (!wk.active)
         return fail(ctx, REGK_ERR_STATE, "regk_walk_requests: no walk on this context; call regk_walk_start first");
@@ -6236,6 +6513,9 @@ int regk_walk_requests(regk_ctx *ctx, int32_t xid_base, uint32_t flags, regk_fra
     p.out_off = (unsigned long long *)fb.off.p;
     CK(cudaEventRecord(wk.ev[0], s));
     regk_walk_frame_kernel<<<(unsigned)(2 * ((f + MK_TILE - 1) / MK_TILE)), MK_TILE, 0, s>>>(p);
+    const bool watch = flags & REGK_ZK_WATCH;
+    if (watch)
+        regk_walk_watch_byte_kernel<<<(unsigned)((2 * f + 255) / 256), 256, 0, s>>>(p.out, p.out_off, 2 * f);
     CK(cudaGetLastError());
     CK(cudaEventRecord(wk.ev[1], s));
     const void *bytes = fb.bytes.p, *off = fb.off.p;
@@ -6250,11 +6530,12 @@ int regk_walk_requests(regk_ctx *ctx, int32_t xid_base, uint32_t flags, regk_fra
     float ms = 0;
     cudaEventElapsedTime(&ms, wk.ev[0], wk.ev[1]);
     wk.framed = true;
+    wk.framed_watch = watch;
     wk.xid = xid_base;
     out->n = 2 * f;
     out->total = total;
     out->flags = flags & REGK_OUT_DEVICE;
-    out->launches = 1;
+    out->launches = watch ? 2 : 1;
     out->frame_bytes = (const uint8_t *)bytes;
     out->frame_off = (const uint64_t *)off;
     out->kernel_ms = ms;
@@ -6607,6 +6888,35 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
             CK(cudaMemsetAsync(wk.foff[nx].p, 0, 8, s));
         }
     }
+    /* 3b. watches: a refresh level's getData replies land on their nodes (regk_walk_refresh), and once a walk has been
+       refreshed every listing drops the paths the snapshot already holds */
+    uint64_t nf = ne;
+    if (wk.rlevel) {
+        /* the table and every buffer the filter and the rebuild need come first: once the replies are applied, nothing
+           that follows can fail on an allocation */
+        uint64_t built;
+        if ((rc = walk_table(ctx, &built, &launches, who)) || (rc = walk_filter_reserve(ctx, ne, lst_total)) ||
+            (rc = walk_rebuild_reserve(ctx, len)))
+            return rc;
+        WalkApplyParams ap{};
+        ap.f = f;
+        ap.fnode = (const unsigned long long *)wk.fnode.p;
+        ap.err = p.err;
+        ap.ver = p.ver;
+        ap.own = p.own;
+        ap.data_pos = p.data_pos;
+        ap.dlen = p.dlen;
+        ap.mark = (uint32_t *)wk.wmark.p;
+        ap.snap_ver = (int32_t *)wk.ver.p;
+        ap.snap_own = (long long *)wk.own.p;
+        ap.rpos = (unsigned long long *)wk.rpos.p;
+        ap.rlen = (uint32_t *)wk.rlen.p;
+        regk_walk_apply_kernel<<<(unsigned)((f + 255) / 256), 256, 0, s>>>(ap);
+        CK(cudaGetLastError());
+        launches++;
+    }
+    if (wk.refreshed && ne && (rc = walk_filter(ctx, nx, ne, wk.rlevel, &nf, &lst_total, &launches, who)))
+        return rc;
     /* 4. the level's nodes: the found getData replies in frontier order, with their stats */
     const uint64_t tiles_r = (f + RP_TILE - 1) / RP_TILE;
     const size_t ft_bytes = align16(tiles_r * 4) + (tiles_r / SUPER + 1) * 8;
@@ -6640,22 +6950,60 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
     CK(cudaMemcpyAsync(hw, fp.counters, WK_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
     if ((rc = sync_or_fail(ctx, s, who)))
         return rc;
-    const uint64_t mf = hw[WK_FOUND], m0 = wk.m;
-    /* 5. the level's paths (from the frontier) and data (from the stream) packed, then appended to the snapshot */
+    const uint64_t mf = hw[WK_FOUND];
+    if (wk.rlevel) {
+        /* 5'. a refresh level appends nothing: the snapshot is rebuilt without its removed nodes, with the replaced data */
+        if ((rc = walk_rebuild(ctx, ds, &launches, who)))
+            return rc;
+    } else if ((rc = walk_append(ctx, ds, fbytes, foff, p.data_pos, fp, mf, &launches)))
+        return rc;
+    CK(cudaEventRecord(wk.ev[1], s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, wk.ev[0], wk.ev[1]);
+    /* the level is in: the listing is the next frontier, unframed */
+    if (wk.rlevel)
+        wk.level_off.assign(1, wk.m);
+    else
+        wk.level_off.push_back(wk.m);
+    wk.watched = wk.watched && wk.framed_watch;
+    wk.rlevel = false;
+    wk.cur = nx;
+    wk.f = nf;
+    wk.fpt = lst_total;
+    wk.framed = false;
+    out->level = wk.level_off.size() - 1;
+    out->m = wk.m;
+    out->n_frontier = nf;
+    return walk_out(ctx, hw, ne, n_listed, n_list_missing, n_list_error, gd_skipped + ch_skipped, consumed, flags, launches,
+                    ms, out);
+}
+
+/* One plain level's found nodes appended to the snapshot: their paths (from the frontier) and data (from the stream)
+   packed, then written at the snapshot streams' ends; version, owner and a clear mark per node. */
+static int walk_append(regk_ctx *ctx, const uint8_t *ds, const uint8_t *fbytes, const unsigned long long *foff,
+    const unsigned long long *data_pos, const WalkFoundParams &fp, uint64_t mf, uint32_t *launches)
+{
+    regk_ctx::Walk &wk = ctx->wk;
+    cudaStream_t s = ctx->stream;
+    const uint64_t m0 = wk.m;
+    int rc;
     uint64_t tot[2] = {0, 0};
     for (int g = 0; g < 2; g++) {
         uint32_t l = 0;
-        if ((rc = pack_strings(ctx, mf, g ? ds : fbytes, g ? p.data_pos : foff, fp.node_rec, g ? fp.node_dlen : fp.node_plen,
+        if ((rc = pack_strings(ctx, mf, g ? ds : fbytes, g ? data_pos : foff, fp.node_rec, g ? fp.node_dlen : fp.node_plen,
                  wk.gtotals, wk.lvl_bytes[g], wk.lvl_off[g], &tot[g], &l)))
             return rc;
-        launches += l;
+        *launches += l;
     }
     const uint64_t at[2] = {wk.path_total, wk.data_total};
     for (int g = 0; g < 2; g++)
         if ((rc = walk_grow(ctx, wk.snap_bytes[g], at[g], at[g] + tot[g] + 16)) ||
             (rc = walk_grow(ctx, wk.snap_off[g], m0 * 8, (m0 + mf + 1) * 8)))
             return rc;
-    if ((rc = walk_grow(ctx, wk.ver, m0 * 4, (m0 + mf) * 4 + 16)) || (rc = walk_grow(ctx, wk.own, m0 * 8, (m0 + mf) * 8 + 16)))
+    if ((rc = walk_grow(ctx, wk.ver, m0 * 4, (m0 + mf) * 4 + 16)) || (rc = walk_grow(ctx, wk.own, m0 * 8, (m0 + mf) * 8 + 16)) ||
+        (rc = walk_grow(ctx, wk.wmark, m0 * 4, (m0 + mf) * 4 + 16)))
         return rc;
     for (int g = 0; g < 2; g++) {
         WalkAppendParams ap{};
@@ -6669,29 +7017,24 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
         const uint64_t nb = (at[g] + tot[g] - (at[g] & ~15ull) + 15) / 16, th = std::max<uint64_t>(nb, mf + 1);
         regk_walk_append_kernel<<<(unsigned)((th + 255) / 256), 256, 0, s>>>(ap);
         CK(cudaGetLastError());
-        launches++;
+        (*launches)++;
     }
     if (mf) {
         CK(cudaMemcpyAsync((int32_t *)wk.ver.p + m0, fp.node_ver, mf * 4, cudaMemcpyDeviceToDevice, s));
         CK(cudaMemcpyAsync((long long *)wk.own.p + m0, fp.node_own, mf * 8, cudaMemcpyDeviceToDevice, s));
+        CK(cudaMemsetAsync((uint32_t *)wk.wmark.p + m0, 0, mf * 4, s));
     }
-    CK(cudaEventRecord(wk.ev[1], s));
-    if ((rc = sync_or_fail(ctx, s, who)))
-        return rc;
-    float ms = 0;
-    cudaEventElapsedTime(&ms, wk.ev[0], wk.ev[1]);
-    /* the level is in: the listing is the next frontier, unframed */
     wk.m = m0 + mf;
     wk.path_total += tot[0];
     wk.data_total += tot[1];
-    wk.level_off.push_back(wk.m);
-    wk.cur = nx;
-    wk.f = ne;
-    wk.fpt = lst_total;
-    wk.framed = false;
-    out->level = wk.level_off.size() - 1;
-    out->m = wk.m;
-    out->n_frontier = ne;
+    return REGK_OK;
+}
+
+/* regk_read_walk's result: the level's counts and the walk's state */
+static int walk_out(regk_ctx *ctx, const unsigned long long *hw, uint64_t ne, uint64_t n_listed, uint64_t n_list_missing,
+    uint64_t n_list_error, uint64_t n_skipped, uint64_t consumed, uint32_t flags, uint32_t launches, float ms, regk_walk *out)
+{
+    regk_ctx::Walk &wk = ctx->wk;
     out->n_found = hw[WK_FOUND];
     out->n_missing = hw[WK_MISSING];
     out->n_error = hw[WK_ERROR];
@@ -6699,7 +7042,7 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
     out->n_list_missing = n_list_missing;
     out->n_list_error = n_list_error;
     out->n_children = ne;
-    out->n_skipped = gd_skipped + ch_skipped;
+    out->n_skipped = n_skipped;
     out->consumed = consumed;
     out->flags = flags & REGK_OUT_DEVICE;
     out->launches = launches;
@@ -6715,6 +7058,300 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
     out->version = (const int32_t *)wk.ver.p;
     out->ephemeral_owner = (const int64_t *)wk.own.p;
     out->kernel_ms = ms;
+    return REGK_OK;
+}
+
+int regk_walk_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, const regk_events_opts *o,
+    regk_walk_events_out *out)
+{
+    const char *who = "regk_walk_events";
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_events: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Walk &wk = ctx->wk;
+    if (!wk.active)
+        return fail(ctx, REGK_ERR_STATE, "regk_walk_events: no walk on this context; call regk_walk_start first");
+    if (!wk.watched)
+        return fail(ctx, REGK_ERR_STATE, "regk_walk_events: the walk is unwatched (a level was framed without "
+                                         "REGK_ZK_WATCH); start a new walk with watches");
+    if (o->flags & ~(REGK_IN_DEVICE | REGK_OUT_DEVICE))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_events: unknown flags 0x%x", o->flags);
+    if (!bytes && len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_events: NULL stream of %llu bytes", (unsigned long long)len);
+    if (start > len)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_events: start %llu is past the stream's %llu bytes",
+            (unsigned long long)start, (unsigned long long)len);
+    const bool in_dev = o->flags & REGK_IN_DEVICE, dev_out = o->flags & REGK_OUT_DEVICE;
+    if (in_dev && ((uintptr_t)bytes & 15u))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_events: misaligned device stream (16-byte alignment needed)");
+    const int32_t xb = o->xid_base;
+    const uint64_t nx = o->n_xids;
+    for (int32_t reserved : {-1, -2})
+        if ((uint64_t)((uint32_t)reserved - (uint32_t)xb) < nx)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_events: the reply xids [%d, %d + %llu) cover %d, which ZooKeeper "
+                                                   "uses for %s", xb, xb, (unsigned long long)nx, reserved,
+                        reserved == -1 ? "watch notifications" : "pings");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    for (Event &e : wk.eev)
+        if ((rc = ensure_event(ctx, e)))
+            return rc;
+    uint32_t launches = 0;
+    /* 0. the path table, when the snapshot changed since it was built: timed on its own */
+    uint64_t built = 0;
+    CK(cudaEventRecord(wk.eev[2], s));
+    if ((rc = walk_table(ctx, &built, &launches, who)))
+        return rc;
+    CK(cudaEventRecord(wk.eev[3], s));
+    const uint8_t *ds = bytes;
+    if (!in_dev && len) {
+        if ((rc = stage_in(ctx, wk.vstream, bytes, len, s)))
+            return rc;
+        ds = (const uint8_t *)wk.vstream.p;
+    }
+    const uint64_t nblk = (len + 15) / 16, tiles_s = (nblk + RP_TILE - 1) / RP_TILE;
+    const size_t totals_bytes = align16(tiles_s * 4) + (tiles_s / SUPER + 1) * 8;
+    if ((rc = ensure_dev(ctx, wk.vword, nblk * 4 + 16)) || (rc = ensure_dev(ctx, wk.vtotals, totals_bytes)) ||
+        (rc = ensure_dev(ctx, wk.vtile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, wk.vcount, EQ_NCOUNTERS * 8)) ||
+        (rc = ensure_host(ctx, wk.h_vcount, EQ_NCOUNTERS * 8 + WM_NCOUNTERS * 8)))
+        return rc;
+    WalkEvParams wp{};
+    EvParams &ep = wp.e;
+    RepParams &p = ep.r;
+    p.s = ds;
+    p.len = len;
+    p.xid_base = xb;
+    p.n = nx;
+    p.word = (uint32_t *)wk.vword.p;
+    p.tile_total = (uint32_t *)wk.vtotals.p;
+    p.super_total = (unsigned long long *)((uint8_t *)wk.vtotals.p + align16(tiles_s * 4));
+    p.tile_base = (unsigned long long *)wk.vtile_base.p;
+    p.counters = (unsigned long long *)wk.vcount.p;
+    ep.start = start;
+    unsigned long long *hc = (unsigned long long *)wk.h_vcount.p;
+    CK(cudaMemsetAsync(p.counters, 0, EQ_NCOUNTERS * 8, s));
+    CK(cudaMemsetAsync(p.tile_total, 0, totals_bytes, s));
+    CK(cudaEventRecord(wk.eev[0], s));
+    /* 1. the frame chain from `start` (regk_read_events' passes) and where it stops */
+    RepParams pf = p;
+    if (len > start) {
+        regk_events_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(ep);
+        CK(cudaGetLastError());
+        launches++;
+        uint32_t *J = nullptr;
+        if ((rc = chain_pass(ctx, &pf, tiles_s, ~0ull, wk.vcand, wk.vmark, wk.vjump, [&](const RepParams &q) {
+                regk_children_seed_kernel<<<1, 256, 0, s>>>(q, nullptr, nullptr, 1, start);
+            }, &J, &launches, who)))
+            return rc;
+        if (pf.C) {
+            regk_replies_stop_kernel<<<(unsigned)((pf.C + 255) / 256), 256, 0, s>>>(pf);
+            CK(cudaGetLastError());
+            launches++;
+        }
+    }
+    CK(cudaMemcpyAsync(hc, p.counters, EQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    const uint64_t stop = std::max<uint64_t>(start, hc[RQ_STOP]);
+    bool partial = false;
+    if (stop < len) {
+        /* the first position the chain does not pass: a frame still arriving, or a fault.  Nothing has been marked. */
+        uint8_t head[32] = {0};
+        const uint64_t avail = len - stop, take = std::min<uint64_t>(avail, sizeof head);
+        CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        EvHead h;
+        const uint32_t code = ev_head(head, avail, xb, nx, &h);
+        if (code != EV_TRUNC)
+            return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_events: byte %llu: %s (len %d, xid %d)", (unsigned long long)stop,
+                code ? events_reason(code) : "internal error", h.len, h.xid);
+        partial = true;
+    }
+    /* 2. the events of the chain mapped against the snapshot as the call found it, then marked */
+    const uint64_t C = pf.C;
+    if ((rc = ensure_dev(ctx, wk.e_pos, C * 8 + 16)) || (rc = ensure_dev(ctx, wk.e_node, C * 8 + 16)) ||
+        (rc = ensure_dev(ctx, wk.e_parent, C * 8 + 16)) || (rc = ensure_dev(ctx, wk.e_zxid, C * 8 + 16)) ||
+        (rc = ensure_dev(ctx, wk.e_type, C * 4 + 16)) || (rc = ensure_dev(ctx, wk.e_state, C * 4 + 16)))
+        return rc;
+    ep.r = pf;
+    ep.pos = (unsigned long long *)wk.e_pos.p;
+    ep.zxid = (long long *)wk.e_zxid.p;
+    ep.type = (int32_t *)wk.e_type.p;
+    ep.state = (int32_t *)wk.e_state.p;
+    wp.spath = (const uint8_t *)wk.snap_bytes[0].p;
+    wp.soff = (const unsigned long long *)wk.snap_off[0].p;
+    wp.table = (const uint32_t *)wk.table.p;
+    wp.mask = wk.tab_mask;
+    wp.mark = (uint32_t *)wk.wmark.p;
+    wp.node = (unsigned long long *)wk.e_node.p;
+    wp.parent = (unsigned long long *)wk.e_parent.p;
+    wp.mcount = (unsigned long long *)wk.mcount.p;
+    uint64_t ne = 0;
+    if (C) {
+        const uint64_t tiles_c = (C + RP_TILE - 1) / RP_TILE;
+        const size_t t2 = align16(tiles_c * 4) + (tiles_c / SUPER + 1) * 8;
+        if ((rc = ensure_dev(ctx, wk.vntotals, t2)))
+            return rc;
+        ep.tile_total = (uint32_t *)wk.vntotals.p;
+        ep.super_total = (unsigned long long *)((uint8_t *)wk.vntotals.p + align16(tiles_c * 4));
+        CK(cudaMemsetAsync(wk.vntotals.p, 0, t2, s));
+        regk_events_count_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(ep);
+        regk_walk_events_kernel<<<(unsigned)tiles_c, RP_TILE, 0, s>>>(wp);
+        CK(cudaGetLastError());
+        launches += 2;
+        CK(cudaMemcpyAsync(hc, p.counters, EQ_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        ne = hc[EQ_NEV];
+        if (ne) {
+            wp.n_ev = ne;
+            regk_walk_mark_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, s>>>(wp);
+            CK(cudaGetLastError());
+            launches++;
+        }
+    }
+    CK(cudaEventRecord(wk.eev[1], s));
+    CK(cudaMemcpyAsync(hc + EQ_NCOUNTERS, wk.mcount.p, WM_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    float ms = 0, tms = 0;
+    cudaEventElapsedTime(&ms, wk.eev[0], wk.eev[1]);
+    cudaEventElapsedTime(&tms, wk.eev[2], wk.eev[3]);
+    const void *src[5] = {wk.e_pos.p, wk.e_type.p, wk.e_state.p, wk.e_zxid.p, wk.e_node.p};
+    if (!dev_out) {
+        HostBuf *hb[5] = {&wk.h_epos, &wk.h_etype, &wk.h_estate, &wk.h_ezxid, &wk.h_enode};
+        const size_t sz[5] = {ne * 8, ne * 4, ne * 4, ne * 8, ne * 8};
+        for (int k = 0; k < 5; k++) {
+            if ((rc = to_host(ctx, *hb[k], src[k], sz[k], s)))
+                return rc;
+            src[k] = hb[k]->p;
+        }
+        CK(cudaStreamSynchronize(s));
+    }
+    wk.n_pending = hc[EQ_NCOUNTERS + WM_PENDING];
+    wk.n_removed = hc[EQ_NCOUNTERS + WM_REMOVED];
+    out->n_events = ne;
+    out->n_pings = hc[EQ_PING];
+    out->n_replies = hc[EQ_REPLY];
+    out->n_unmatched = hc[EQ_UNMATCHED];
+    out->n_other = hc[EQ_OTHER];
+    out->consumed = stop;
+    out->n_pending = wk.n_pending;
+    out->n_removed = wk.n_removed;
+    out->table_nodes = built;
+    out->partial = partial ? 1u : 0u;
+    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = launches;
+    out->pos = (const uint64_t *)src[0];
+    out->type = (const int32_t *)src[1];
+    out->state = (const int32_t *)src[2];
+    out->zxid = (const int64_t *)src[3];
+    out->node = (const uint64_t *)src[4];
+    out->kernel_ms = ms;
+    out->table_ms = built ? tms : 0.0f;
+    return REGK_OK;
+}
+
+int regk_walk_refresh(regk_ctx *ctx, uint32_t flags, regk_walk_refresh_out *out)
+{
+    const char *who = "regk_walk_refresh";
+    if (!ctx || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_refresh: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Walk &wk = ctx->wk;
+    if (flags)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_refresh: flags must be 0");
+    if (!wk.active)
+        return fail(ctx, REGK_ERR_STATE, "regk_walk_refresh: no walk on this context; call regk_walk_start first");
+    if (!wk.watched)
+        return fail(ctx, REGK_ERR_STATE, "regk_walk_refresh: the walk is unwatched (a level was framed without "
+                                         "REGK_ZK_WATCH); start a new walk with watches");
+    if (wk.f)
+        return fail(ctx, REGK_ERR_STATE, "regk_walk_refresh: a level is outstanding (the frontier holds %llu nodes); read "
+                                         "the walk to its end first", (unsigned long long)wk.f);
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    for (Event &e : wk.ev)
+        if ((rc = ensure_event(ctx, e)))
+            return rc;
+    uint32_t launches = 0;
+    const uint64_t m0 = wk.m;
+    CK(cudaEventRecord(wk.ev[0], s));
+    /* 1. the removed nodes dropped (nothing to do when none is marked) */
+    if (wk.n_removed && (rc = walk_rebuild(ctx, nullptr, &launches, who)))
+        return rc;
+    /* 2. the pending nodes, ascending, as a refresh level's frontier (paths packed from the snapshot); marks cleared */
+    const uint64_t m = wk.m, tiles = (m + RP_TILE - 1) / RP_TILE;
+    const size_t tb = align16(tiles * 4) + (tiles / SUPER + 1) * 8;
+    const int cur = wk.cur;
+    if ((rc = ensure_dev(ctx, wk.ktotals, tb)) || (rc = ensure_dev(ctx, wk.kcount, 16)) ||
+        (rc = ensure_dev(ctx, wk.xrec, m * 8 + 16)) || (rc = ensure_dev(ctx, wk.fnode, m * 8 + 16)) ||
+        (rc = ensure_dev(ctx, wk.flen[cur], m * 4 + 16)))
+        return rc;
+    uint64_t f = 0, fpt = 0;
+    if (m) {
+        EvPendParams pp{};
+        pp.n = m;
+        pp.mark = (const uint32_t *)wk.wmark.p;
+        pp.shift = 0;
+        pp.epoch = WK_PENDING;
+        pp.path_off = (const unsigned long long *)wk.snap_off[0].p;
+        pp.tile_total = (uint32_t *)wk.ktotals.p;
+        pp.super_total = (unsigned long long *)((uint8_t *)wk.ktotals.p + align16(tiles * 4));
+        pp.item = (unsigned long long *)wk.fnode.p;
+        pp.rec = (unsigned long long *)wk.xrec.p;
+        pp.len = (uint32_t *)wk.flen[cur].p;
+        pp.count = (unsigned long long *)wk.kcount.p;
+        CK(cudaMemsetAsync(wk.ktotals.p, 0, tb, s));
+        regk_events_pending_count_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(pp);
+        regk_events_pending_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(pp);
+        CK(cudaGetLastError());
+        launches += 2;
+        unsigned long long cnt = 0;
+        CK(cudaMemcpyAsync(&cnt, pp.count, 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        f = cnt;
+        if ((rc = pack_strings(ctx, f, (const uint8_t *)wk.snap_bytes[0].p, pp.path_off, pp.rec, pp.len, wk.gtotals,
+                 wk.fbytes[cur], wk.foff[cur], &fpt, &launches)))
+            return rc;
+        CK(cudaMemsetAsync(wk.wmark.p, 0, m * 4, s));
+        CK(cudaMemsetAsync(wk.mcount.p, 0, WM_NCOUNTERS * 8, s));
+    }
+    CK(cudaEventRecord(wk.ev[1], s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, wk.ev[0], wk.ev[1]);
+    wk.n_pending = wk.n_removed = 0;
+    wk.f = f;
+    wk.fpt = fpt;
+    wk.framed = false;
+    wk.refreshed = true;
+    wk.rlevel = f != 0;
+    wk.level_off.assign(1, m);
+    out->n_removed = m0 - m;
+    out->n_kept = m;
+    out->n_frontier = f;
+    out->launches = launches;
+    out->kernel_ms = ms;
+    regk_walk &w = out->walk;
+    w.level = 0;
+    w.m = m;
+    w.n_frontier = f;
+    w.level_off = wk.level_off.data();
+    w.snapshot.n = m;
+    w.snapshot.flags = REGK_IN_DEVICE;
+    w.snapshot.path_total = wk.path_total;
+    w.snapshot.json_total = wk.data_total;
+    w.snapshot.path_bytes = (const uint8_t *)wk.snap_bytes[0].p;
+    w.snapshot.path_off = (const uint64_t *)wk.snap_off[0].p;
+    w.snapshot.json_bytes = (const uint8_t *)wk.snap_bytes[1].p;
+    w.snapshot.json_off = (const uint64_t *)wk.snap_off[1].p;
+    w.version = (const int32_t *)wk.ver.p;
+    w.ephemeral_owner = (const int64_t *)wk.own.p;
     return REGK_OK;
 }
 
