@@ -1342,8 +1342,8 @@ int         regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns
  *   no watched parent: it stays gone until a new walk.
  * CONVERGENCE: once the tree stops changing and every byte has been fed, refreshing until nothing is pending or removed
  *   leaves a snapshot equal, as a set of (path, data, version, owner), to a fresh walk of the same roots (deleted roots
- *   aside); node order differs.  Re-resolve it (regk_resolve is not incremental).  After a reconnect, start a new
- *   watched walk: the walk has no SetWatches.
+ *   aside); node order differs.  Re-resolve it (regk_resolve is not incremental).  After a reconnect, carry the walk
+ *   over with regk_walk_setwatches below; after a session expiry, start a new watched walk.
  * PARITY UNPINNED: restated from zookeeper.jute (WatcherEvent) and the server's watch rules (one-shot, per session; a
  *   getData on a missing node arms nothing; a watch still armed is not duplicated), not tested against a server.
  */
@@ -1396,6 +1396,69 @@ typedef struct regk_walk_refresh_out {
 int         regk_walk_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t start, const regk_events_opts *opts,
                              regk_walk_events_out *out);
 int         regk_walk_refresh(regk_ctx *ctx, uint32_t flags, regk_walk_refresh_out *out);
+
+/*
+ * ---- a watched walk across a reconnect: ZooKeeper drops a connection's watches with the connection, though the
+ * session survives.  regk_walk_setwatches frames SetWatches (op 101) for the watches the walk's session holds, so the
+ * server re-arms them on the new connection or fires what the walk missed, and re-pends every other node -------------
+ * ARMED: each snapshot node carries one more bit, set when the last read of the node (the plain level that appended it,
+ *   or a refresh level that re-read it) was framed with REGK_ZK_WATCH and both its getData and its getChildren reply had
+ *   err 0.  Any other outcome clears it: an unwatched framing, a refresh-level getData err other than NONODE (which
+ *   arms nothing), a getChildren err (no child watch).  The bit moves with its node through a rebuild, and
+ *   regk_walk_start clears everything.  This bookkeeping, and the mark's below, is not counted in any call's
+ *   `launches`.
+ * The walk's zxid high-water mark is the largest ReplyHeader.zxid of every reply frame a successful regk_read_walk read
+ *   (both sections' frame chains, not the listing entries) and of every reply and SetWatches reply a successful
+ *   regk_walk_events walked; never a notification or a ping.  A refused call does not move it, regk_walk_start resets it
+ *   to 0, and it is the walk's own, apart from the heartbeat's: an overestimate loses events, and only the bytes this
+ *   walk read vouch for it.  It is safe as relativeZxid for the reason the heartbeat's is: a reply with zxid R leaves the
+ *   server after every notification of a change at or below R, and TCP keeps that order.  The ORDERING RULE feeds every
+ *   delivered byte through regk_walk_events, so a change the walk missed was notified after the last reply it read,
+ *   and its zxid is above the mark: the server fires it again.  An underestimate only fires spurious events.
+ *
+ * regk_walk_setwatches (opts as regk_setwatches_requests takes them): on a watched walk (else REGK_ERR_STATE), complete
+ *   or with a level in flight.  Call it when the connection drops, before reconnecting; relative_zxid is also the
+ *   ConnectRequest's lastZxidSeen.
+ *     LISTED     every node that is ARMED and neither PENDING, REMOVED nor a node of the refresh frontier (a refresh
+ *                level framed or about to be), ascending, into D (data watches); the same nodes in the same order
+ *                into C (child watches); E is empty.
+ *     RE-PENDED  every other node that is neither PENDING, REMOVED nor of the refresh frontier becomes PENDING
+ *                (n_repend), so the next refresh re-reads and re-arms it.
+ *     LEFT ALONE pending and removed nodes, and the frontier: n_frontier (0: none) is the level to frame again after the
+ *                reconnect with regk_walk_requests, whose reads arm those nodes.
+ *   Frames: exactly regk_setwatches_requests' layout and split, with Lmax = 4 + the snapshot's longest path; max_frame's
+ *   default, bounds and refusal (naming the minimum) are the same.  Pinned host arrays, or device arrays with
+ *   REGK_OUT_DEVICE, valid until the next call.  A refused call changes nothing, and every buffer is reserved before any
+ *   node is re-pended.  After a successful call regk_walk_events also accepts a SetWatches reply (xid -8, len 16,
+ *   err 0: skipped, counted in n_replies, its zxid entering the mark); a -8 frame with a body or an err is refused.
+ *   Before any such call -8 is refused as any negative xid; regk_walk_start closes the gate.  regk_read_walk is unchanged.
+ * RECONNECT PROTOCOL:
+ *   1. Feed every delivered byte through regk_walk_events as usual.  The bytes of a level whose replies were cut off may
+ *      be fed with that level's reply range, or discarded: an event fed is a real change, and an event discarded was
+ *      notified after every reply the walk read, so its zxid is above the mark and SetWatches fires it again.
+ *   2. Call regk_walk_setwatches, and reconnect with lastZxidSeen = relative_zxid.
+ *   3. Send the SetWatches frames.
+ *   4. Feed the stream through regk_walk_events until every SetWatches reply has been seen (one per frame).  The
+ *      notifications the server fires from DataTree.setWatches arrive before each reply and mark the nodes that changed.
+ *      A deleted node, listed in D and in C, fires NodeDeleted twice; REMOVED is idempotent.
+ *   5. If n_frontier > 0, frame that level again (regk_walk_requests, a fresh xid base) and read it as usual.
+ *   6. Refresh as usual.
+ * CONVERGENCE: a walk carried over this way converges as a watched walk does: once the tree stops changing, refreshing
+ *   until nothing is pending or removed leaves the set of a fresh walk of the same roots, deleted roots aside.  A
+ *   session expiry still means a new walk.
+ * PARITY UNPINNED: the server's re-arming is restated from ZooKeeper 3.4's DataTree.setWatches, not tested against a
+ *   server.
+ */
+typedef struct regk_walk_setwatches_out {
+    uint64_t n_listed;              /* snapshot nodes listed (each once in D and once in C) */
+    uint64_t n_repend;              /* nodes this call made PENDING */
+    uint64_t n_pending, n_removed;  /* after the call, as regk_walk_events reports them */
+    uint64_t n_frontier;            /* the level in flight, to be framed again after the reconnect; 0: none */
+    int64_t  relative_zxid;
+    regk_frames frames;
+} regk_walk_setwatches_out;
+
+int         regk_walk_setwatches(regk_ctx *ctx, const regk_setwatches_opts *opts, regk_walk_setwatches_out *out);
 
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);

@@ -634,6 +634,30 @@ class WalkRefresh:
         self.walk = Walk(ctx, out.walk)
 
 
+class CWalkSetWatches(C.Structure):  # regk_walk_setwatches_out
+    _fields_ = [("n_listed", C.c_uint64), ("n_repend", C.c_uint64), ("n_pending", C.c_uint64),
+                ("n_removed", C.c_uint64), ("n_frontier", C.c_uint64), ("relative_zxid", C.c_int64),
+                ("frames", CFrames)]
+
+
+class WalkSetWatches:
+    """What walk_setwatches() framed: SetWatches frames (frames uint8[total], frame_off uint64[n_frames+1]) listing the
+    n_listed armed snapshot nodes in D and in C, relative_zxid (also the ConnectRequest's lastZxidSeen), n_repend nodes
+    made pending instead, n_pending / n_removed after the call, and n_frontier, the level to frame again after the
+    reconnect (0: none)."""
+
+    def __init__(self, out):
+        f = out.frames
+        self.n_frames, self.launches, self.kernel_ms = int(f.n), int(f.launches), float(f.kernel_ms)
+        self.frames = _as_np(f.frame_bytes, int(f.total), np.uint8).copy()
+        self.frame_off = _as_np(f.frame_off, self.n_frames + 1, np.uint64).copy()
+        self.n_listed, self.n_repend = int(out.n_listed), int(out.n_repend)
+        self.n_pending, self.n_removed = int(out.n_pending), int(out.n_removed)
+        self.n_frontier, self.relative_zxid = int(out.n_frontier), int(out.relative_zxid)
+
+    lists = SetWatches.lists
+
+
 class CSkipped(C.Structure):         # regk_skipped
     _fields_ = [("n", C.c_uint64), ("n_skipped", C.c_uint64), ("flags", C.c_uint32), ("bad_bits", C.c_uint32),
                 ("index", C.c_void_p), ("bits", C.c_void_p)]
@@ -649,7 +673,7 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results", "regk_read_stats",
            "regk_reconcile_stats", "regk_read_events", "regk_events_requests",
            "regk_setwatches_requests", "regk_resolve", "regk_dns_answer", "regk_walk_start", "regk_walk_requests",
-           "regk_read_walk", "regk_walk_events", "regk_walk_refresh"]
+           "regk_read_walk", "regk_walk_events", "regk_walk_refresh", "regk_walk_setwatches"]
 
 _lib = None
 
@@ -722,6 +746,7 @@ def load_library():
     lib.regk_read_walk.argtypes = [vp, vp, u64, u32, C.POINTER(CWalk)]
     lib.regk_walk_events.argtypes = [vp, vp, u64, u64, C.POINTER(CEventsOpts), C.POINTER(CWalkEvents)]
     lib.regk_walk_refresh.argtypes = [vp, u32, C.POINTER(CWalkRefresh)]
+    lib.regk_walk_setwatches.argtypes = [vp, C.POINTER(CSetWatchesOpts), C.POINTER(CWalkSetWatches)]
     _lib = lib
     return lib
 
@@ -804,6 +829,7 @@ class Context:
         if rc != REGK_OK:
             raise RegkError(rc, (self._lib.regk_last_error(None) or b"").decode())
         self._h = h
+        self._walk = None
         self.device = device
         self._types = None
         if types is not None:
@@ -1343,6 +1369,7 @@ class Context:
         off = np.zeros(len(roots) + 1, np.uint64)
         np.cumsum([len(r) for r in roots], out=off[1:])
         self._check(self._lib.regk_walk_start(self._h, _np_ptr(b), _np_ptr(off), len(roots), 0))
+        self._walk = None
 
     def walk_requests(self, xid_base: int = 1, device: bool = False, watch: bool = False):
         """regk_walk_requests: a getData frame per node of the walk's current frontier, then a getChildren frame per
@@ -1378,7 +1405,8 @@ class Context:
         rc = self._lib.regk_read_walk(self._h, ptr, n, flags, C.byref(out))
         del keep
         self._check(rc)
-        return out if device else Walk(self, out)
+        self._walk = Walk(self, out)
+        return out if device else self._walk
 
     def walk(self, roots, exchange, xid_base: int = 1, watch: bool = False):
         """The whole walk from `roots`: each level's frames go to exchange(frame_bytes) -> reply stream (the caller's
@@ -1435,13 +1463,42 @@ class Context:
         of a refresh level (read it with walk_requests() / read_walk() as any level).  Returns a WalkRefresh."""
         out = CWalkRefresh()
         self._check(self._lib.regk_walk_refresh(self._h, 0, C.byref(out)))
-        return WalkRefresh(self, out)
+        r = WalkRefresh(self, out)
+        self._walk = r.walk
+        return r
 
     def refresh_walk(self, exchange, xid_base: int = 1):
         """walk_refresh(), then the refresh level and the levels under it as walk(..., watch=True) runs them.  Returns
         (WalkRefresh, the Walk as it stands after the last level)."""
         r = self.walk_refresh()
         w, _ = self._walk_levels(exchange, int(xid_base) % 2 ** 32, r.n_frontier, True, r.walk)
+        return r, w
+
+    def walk_setwatches(self, max_frame: int = 0, device: bool = False):
+        """regk_walk_setwatches: after the connection dropped, SetWatches frames for the watches the watched walk's
+        session holds (frames of at most max_frame bytes; 0 = 131072), with every other node made pending for the next
+        refresh.  Returns a WalkSetWatches, or the raw CWalkSetWatches (frames on the device) with device=True."""
+        o = CSetWatchesOpts(int(max_frame), FLAG_OUT_DEVICE if device else 0)
+        out = CWalkSetWatches()
+        self._check(self._lib.regk_walk_setwatches(self._h, C.byref(o), C.byref(out)))
+        return out if device else WalkSetWatches(out)
+
+    def resume_walk(self, exchange, xid_base: int = 1, max_frame: int = 0):
+        """The watched walk carried over a reconnect: walk_setwatches(), then exchange(frames) -> the new connection's
+        stream, which must hold whole frames through the last SetWatches reply; that stream goes through walk_events(),
+        and a level that was in flight is framed again and read as walk(..., watch=True) reads it.  Returns
+        (WalkSetWatches, the Walk as it then stands); refresh_walk() then re-reads what changed.  Raises ValueError when
+        the stream ends inside a frame or holds fewer SetWatches replies than frames."""
+        r = self.walk_setwatches(max_frame)
+        s = exchange(r.frames.tobytes()) if r.n_frames else b""
+        s = np.frombuffer(s, np.uint8) if isinstance(s, (bytes, bytearray)) else s
+        e = self.walk_events(s)
+        if e.partial:
+            raise ValueError("exchange returned bytes that end inside a frame: return whole frames, so that every "
+                             "notification goes through walk_events exactly once")
+        if e.n_replies < r.n_frames:
+            raise ValueError("exchange returned %d SetWatches replies for %d frames" % (e.n_replies, r.n_frames))
+        w, _ = self._walk_levels(exchange, int(xid_base) % 2 ** 32, r.n_frontier, True, getattr(self, "_walk", None))
         return r, w
 
     def _d2h(self, ptr, count, dtype):

@@ -43,6 +43,7 @@
 #include "regk_dns.cuh"
 #include "regk_walk.cuh"
 #include "regk_walk_watch.cuh"
+#include "regk_walk_setwatches.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -390,6 +391,14 @@ struct regk_ctx {
             e_node, e_parent;
         HostBuf h_epos, h_etype, h_estate, h_ezxid, h_enode, h_vcount;
         Event eev[4];
+        /* across a reconnect (regk_walk_setwatches.cuh): the armed byte per node (armed2: the rebuild's copy), the
+           walk's zxid high-water mark (largest ReplyHeader.zxid of the replies its successful reads and event calls
+           walked), the SetWatches gate of regk_walk_events, and the framing's working arrays and frames */
+        DevBuf armed, armed2, zmax, sw_lmax, sw_cls, sw_totals, sw_count, sw_ent_src, sw_ent_s, sw_ent_len;
+        long long zxid = 0;
+        bool gate = false;
+        FrameBufs swframes;
+        Event swev[2];
     } wk;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
@@ -6219,7 +6228,7 @@ static int walk_rebuild_reserve(regk_ctx *ctx, uint64_t extra)
         (rc = ensure_dev(ctx, wk.dsrc, m8)) || (rc = ensure_dev(ctx, wk.kplen, m4)) || (rc = ensure_dev(ctx, wk.kdlen, m4)) ||
         (rc = ensure_dev(ctx, wk.dsel, m + 16)) || (rc = ensure_dev(ctx, wk.wmark2, m4)) || (rc = ensure_dev(ctx, wk.ver2, m4)) ||
         (rc = ensure_dev(ctx, wk.own2, m8)) || (rc = ensure_dev(ctx, wk.rpos, m8)) || (rc = ensure_dev(ctx, wk.rlen, m4)) ||
-        (rc = ensure_dev(ctx, wk.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)))
+        (rc = ensure_dev(ctx, wk.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)) || (rc = ensure_dev(ctx, wk.armed2, m + 16)))
         return rc;
     const uint64_t bytes[2] = {wk.path_total, wk.data_total + extra};
     for (int g = 0; g < 2; g++)
@@ -6365,6 +6374,8 @@ static int walk_rebuild(regk_ctx *ctx, const uint8_t *ds, uint32_t *launches, co
         CK(cudaMemsetAsync(wk.ktotals.p, 0, tb, s));
         regk_walk_keep_count_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(kp);
         regk_walk_keep_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(kp);
+        /* the armed bytes move with their nodes; not counted in `launches` (bookkeeping for regk_walk_setwatches) */
+        regk_walk_keep_armed_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(kp, (const uint8_t *)wk.armed.p, (uint8_t *)wk.armed2.p);
         CK(cudaGetLastError());
         *launches += 2;
         CK(cudaMemcpyAsync(kc, kp.counters, 16, cudaMemcpyDeviceToHost, s));
@@ -6382,6 +6393,7 @@ static int walk_rebuild(regk_ctx *ctx, const uint8_t *ds, uint32_t *launches, co
         std::swap(wk.snap_off[g], wk.snap2_off[g]);
     }
     std::swap(wk.wmark, wk.wmark2);
+    std::swap(wk.armed, wk.armed2);
     std::swap(wk.ver, wk.ver2);
     std::swap(wk.own, wk.own2);
     const unsigned long long mc[WM_NCOUNTERS] = {kc[1], 0ull};
@@ -6467,6 +6479,8 @@ int regk_walk_start(regk_ctx *ctx, const uint8_t *roots, const uint64_t *root_of
     wk.watched = true;
     wk.framed_watch = wk.refreshed = wk.rlevel = wk.tab_valid = false;
     wk.n_pending = wk.n_removed = 0;
+    wk.zxid = 0;
+    wk.gate = false;
     wk.rgen++;
     wk.active = true;
     return REGK_OK;
@@ -6582,7 +6596,7 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
         (rc = ensure_dev(ctx, wk.tile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, wk.err, f4)) ||
         (rc = ensure_dev(ctx, wk.data_pos, f8)) || (rc = ensure_dev(ctx, wk.dlen, f4)) || (rc = ensure_dev(ctx, wk.dver, f4)) ||
         (rc = ensure_dev(ctx, wk.down, f8)) || (rc = ensure_dev(ctx, wk.count, CQ_NCOUNTERS * 8)) ||
-        (rc = ensure_host(ctx, wk.h_count, CQ_NCOUNTERS * 8)))
+        (rc = ensure_host(ctx, wk.h_count, CQ_NCOUNTERS * 8)) || (rc = ensure_dev(ctx, wk.zmax, 16)))
         return rc;
     unsigned long long *hc = (unsigned long long *)wk.h_count.p;
     /* 1. the getData section: the frame chain from 0, the replies of the f nodes (regk_replies.cuh) */
@@ -6912,6 +6926,15 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
         ap.rpos = (unsigned long long *)wk.rpos.p;
         ap.rlen = (uint32_t *)wk.rlen.p;
         regk_walk_apply_kernel<<<(unsigned)((f + 255) / 256), 256, 0, s>>>(ap);
+        /* the frontier nodes' armed bytes, before the rebuild renumbers them (not counted in `launches`) */
+        WalkArmParams am{};
+        am.n = f;
+        am.fnode = ap.fnode;
+        am.err = p.err;
+        am.cerr = (const int32_t *)wk.cerr.p;
+        am.watch = wk.framed_watch ? 1u : 0u;
+        am.armed = (uint8_t *)wk.armed.p;
+        regk_walk_arm_kernel<<<(unsigned)((f + 255) / 256), 256, 0, s>>>(am);
         CK(cudaGetLastError());
         launches++;
     }
@@ -6950,7 +6973,7 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
     CK(cudaMemcpyAsync(hw, fp.counters, WK_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
     if ((rc = sync_or_fail(ctx, s, who)))
         return rc;
-    const uint64_t mf = hw[WK_FOUND];
+    const uint64_t mf = hw[WK_FOUND], m0 = wk.m;
     if (wk.rlevel) {
         /* 5'. a refresh level appends nothing: the snapshot is rebuilt without its removed nodes, with the replaced data */
         if ((rc = walk_rebuild(ctx, ds, &launches, who)))
@@ -6958,8 +6981,29 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
     } else if ((rc = walk_append(ctx, ds, fbytes, foff, p.data_pos, fp, mf, &launches)))
         return rc;
     CK(cudaEventRecord(wk.ev[1], s));
+    /* regk_walk_setwatches' bookkeeping, outside the read's launches and kernel_ms: the appended nodes' armed bytes,
+       and the largest zxid of both sections' reply frames */
+    if (!wk.rlevel && mf) {
+        WalkArmParams am{};
+        am.n = mf;
+        am.node_rec = fp.node_rec;
+        am.base = m0;
+        am.err = p.err;
+        am.cerr = (const int32_t *)wk.cerr.p;
+        am.watch = wk.framed_watch ? 1u : 0u;
+        am.armed = (uint8_t *)wk.armed.p;
+        regk_walk_arm_kernel<<<(unsigned)((mf + 255) / 256), 256, 0, s>>>(am);
+    }
+    CK(cudaMemsetAsync(wk.zmax.p, 0, 8, s));
+    for (const RepParams *q : {&pg, &pf})
+        if (q->C)
+            regk_events_zxid_kernel<<<(unsigned)((q->C + 255) / 256), 256, 0, s>>>(*q, (long long *)wk.zmax.p);
+    CK(cudaGetLastError());
+    long long zmax = 0;
+    CK(cudaMemcpyAsync(&zmax, wk.zmax.p, 8, cudaMemcpyDeviceToHost, s));
     if ((rc = sync_or_fail(ctx, s, who)))
         return rc;
+    wk.zxid = std::max(wk.zxid, zmax);
     float ms = 0;
     cudaEventElapsedTime(&ms, wk.ev[0], wk.ev[1]);
     /* the level is in: the listing is the next frontier, unframed */
@@ -7003,7 +7047,7 @@ static int walk_append(regk_ctx *ctx, const uint8_t *ds, const uint8_t *fbytes, 
             (rc = walk_grow(ctx, wk.snap_off[g], m0 * 8, (m0 + mf + 1) * 8)))
             return rc;
     if ((rc = walk_grow(ctx, wk.ver, m0 * 4, (m0 + mf) * 4 + 16)) || (rc = walk_grow(ctx, wk.own, m0 * 8, (m0 + mf) * 8 + 16)) ||
-        (rc = walk_grow(ctx, wk.wmark, m0 * 4, (m0 + mf) * 4 + 16)))
+        (rc = walk_grow(ctx, wk.wmark, m0 * 4, (m0 + mf) * 4 + 16)) || (rc = walk_grow(ctx, wk.armed, m0, m0 + mf + 16)))
         return rc;
     for (int g = 0; g < 2; g++) {
         WalkAppendParams ap{};
@@ -7114,7 +7158,7 @@ int regk_walk_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
     const size_t totals_bytes = align16(tiles_s * 4) + (tiles_s / SUPER + 1) * 8;
     if ((rc = ensure_dev(ctx, wk.vword, nblk * 4 + 16)) || (rc = ensure_dev(ctx, wk.vtotals, totals_bytes)) ||
         (rc = ensure_dev(ctx, wk.vtile_base, tiles_s * 8 + 16)) || (rc = ensure_dev(ctx, wk.vcount, EQ_NCOUNTERS * 8)) ||
-        (rc = ensure_host(ctx, wk.h_vcount, EQ_NCOUNTERS * 8 + WM_NCOUNTERS * 8)))
+        (rc = ensure_host(ctx, wk.h_vcount, EQ_NCOUNTERS * 8 + WM_NCOUNTERS * 8)) || (rc = ensure_dev(ctx, wk.zmax, 16)))
         return rc;
     WalkEvParams wp{};
     EvParams &ep = wp.e;
@@ -7135,8 +7179,12 @@ int regk_walk_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
     CK(cudaEventRecord(wk.eev[0], s));
     /* 1. the frame chain from `start` (regk_read_events' passes) and where it stops */
     RepParams pf = p;
+    const bool sw = wk.gate;                    /* after regk_walk_setwatches: SetWatches replies are frames too */
     if (len > start) {
-        regk_events_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(ep);
+        if (sw)
+            regk_events_sw_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(ep);
+        else
+            regk_events_cand_kernel<<<(unsigned)tiles_s, RP_TILE, 0, s>>>(ep);
         CK(cudaGetLastError());
         launches++;
         uint32_t *J = nullptr;
@@ -7162,7 +7210,7 @@ int regk_walk_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
         CK(cudaMemcpyAsync(head, ds + stop, take, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         EvHead h;
-        const uint32_t code = ev_head(head, avail, xb, nx, &h);
+        const uint32_t code = sw ? ev_sw_head(head, avail, xb, nx, &h) : ev_head(head, avail, xb, nx, &h);
         if (code != EV_TRUNC)
             return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_events: byte %llu: %s (len %d, xid %d)", (unsigned long long)stop,
                 code ? events_reason(code) : "internal error", h.len, h.xid);
@@ -7213,6 +7261,14 @@ int regk_walk_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
     }
     CK(cudaEventRecord(wk.eev[1], s));
     CK(cudaMemcpyAsync(hc + EQ_NCOUNTERS, wk.mcount.p, WM_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+    /* the zxid high-water mark: the chain's replies and SetWatches replies (outside launches and kernel_ms) */
+    long long zmax = 0;
+    if (C) {
+        CK(cudaMemsetAsync(wk.zmax.p, 0, 8, s));
+        regk_events_zxid_kernel<<<(unsigned)((C + 255) / 256), 256, 0, s>>>(pf, (long long *)wk.zmax.p);
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(&zmax, wk.zmax.p, 8, cudaMemcpyDeviceToHost, s));
+    }
     if ((rc = sync_or_fail(ctx, s, who)))
         return rc;
     float ms = 0, tms = 0;
@@ -7231,6 +7287,7 @@ int regk_walk_events(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint64_t
     }
     wk.n_pending = hc[EQ_NCOUNTERS + WM_PENDING];
     wk.n_removed = hc[EQ_NCOUNTERS + WM_REMOVED];
+    wk.zxid = std::max(wk.zxid, zmax);
     out->n_events = ne;
     out->n_pings = hc[EQ_PING];
     out->n_replies = hc[EQ_REPLY];
@@ -7352,6 +7409,177 @@ int regk_walk_refresh(regk_ctx *ctx, uint32_t flags, regk_walk_refresh_out *out)
     w.snapshot.json_off = (const uint64_t *)wk.snap_off[1].p;
     w.version = (const int32_t *)wk.ver.p;
     w.ephemeral_owner = (const int64_t *)wk.own.p;
+    return REGK_OK;
+}
+
+int regk_walk_setwatches(regk_ctx *ctx, const regk_setwatches_opts *o, regk_walk_setwatches_out *out)
+{
+    const char *who = "regk_walk_setwatches";
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_setwatches: NULL argument");
+    memset(out, 0, sizeof *out);
+    regk_ctx::Walk &wk = ctx->wk;
+    if (o->flags & ~(uint32_t)REGK_OUT_DEVICE)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_setwatches: unknown flag bits 0x%x (only REGK_OUT_DEVICE)",
+            o->flags & ~(uint32_t)REGK_OUT_DEVICE);
+    if (o->max_frame >= 0x80000000u)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_setwatches: max_frame %u is 2^31 or more; a frame's length is a "
+                                               "signed 32-bit int", o->max_frame);
+    if (!wk.active)
+        return fail(ctx, REGK_ERR_STATE, "regk_walk_setwatches: no walk on this context; call regk_walk_start first");
+    if (!wk.watched)
+        return fail(ctx, REGK_ERR_STATE, "regk_walk_setwatches: the walk is unwatched (a level was framed without "
+                                         "REGK_ZK_WATCH); it holds no watches to carry over");
+    const uint64_t m = wk.m;
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->stream;
+    int rc;
+    for (Event &e : wk.swev)
+        if ((rc = ensure_event(ctx, e)))
+            return rc;
+    const unsigned long long *soff = (const unsigned long long *)wk.snap_off[0].p;
+    const uint64_t tiles = (m + RP_TILE - 1) / RP_TILE;
+    const size_t reg = align16(tiles * 4) + (tiles / SUPER + 1) * 8;
+    if ((rc = ensure_dev(ctx, wk.sw_lmax, 16)) || (rc = ensure_dev(ctx, wk.sw_totals, 2 * reg)) ||
+        (rc = ensure_dev(ctx, wk.sw_count, 16)) || (rc = ensure_dev(ctx, wk.sw_cls, m + 16)))
+        return rc;
+    uint32_t launches = 0;
+    CK(cudaEventRecord(wk.swev[0], s));
+    /* 1. the split's bound: the snapshot's longest path */
+    CK(cudaMemsetAsync(wk.sw_lmax.p, 0, 4, s));
+    if (m) {
+        regk_sw_lmax_kernel<<<(unsigned)((m + 255) / 256), 256, 0, s>>>(soff, m, (uint32_t *)wk.sw_lmax.p);
+        CK(cudaGetLastError());
+        launches++;
+    }
+    /* 2. classify: listed or re-pend per node, and the listed nodes' per-tile counts and bytes; nothing is marked yet */
+    WalkSwParams wp{};
+    wp.m = m;
+    wp.path_off = soff;
+    wp.armed = (const uint8_t *)wk.armed.p;
+    wp.mark = (uint32_t *)wk.wmark.p;
+    wp.fnode = (const unsigned long long *)wk.fnode.p;
+    wp.f = wk.rlevel ? wk.f : 0;
+    wp.cls = (uint8_t *)wk.sw_cls.p;
+    for (int k = 0; k < 2; k++) {
+        uint8_t *t = (uint8_t *)wk.sw_totals.p + k * reg;
+        wp.tt[k] = (uint32_t *)t;
+        wp.st[k] = (unsigned long long *)(t + align16(tiles * 4));
+    }
+    wp.counters = (unsigned long long *)wk.sw_count.p;
+    CK(cudaMemsetAsync(wk.sw_totals.p, 0, 2 * reg, s));
+    CK(cudaMemsetAsync(wk.sw_count.p, 0, 8, s));
+    if (m) {
+        regk_walk_sw_classify_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(wp);
+        CK(cudaGetLastError());
+        launches++;
+    }
+    std::vector<unsigned long long> sup(2 * (tiles / SUPER + 1));
+    for (int k = 0; k < 2; k++)
+        CK(cudaMemcpyAsync(sup.data() + k * (tiles / SUPER + 1), wp.st[k], (tiles / SUPER + 1) * 8, cudaMemcpyDeviceToHost, s));
+    unsigned long long hq[2] = {0, 0};
+    uint32_t lmax = 0;
+    CK(cudaMemcpyAsync(hq, wk.sw_count.p, 8, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&lmax, wk.sw_lmax.p, 4, cudaMemcpyDeviceToHost, s));
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    const uint64_t Lmax = 4ull + lmax, mf = o->max_frame ? o->max_frame : 131072u;
+    if (mf < SW_OVERHEAD + 2 * Lmax)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_setwatches: max_frame %llu is below this snapshot's minimum of %llu "
+                                               "(32 + 2 x (4 + its longest path, %u bytes))", (unsigned long long)mf,
+                    (unsigned long long)(SW_OVERHEAD + 2 * Lmax), lmax);
+    const uint64_t B = mf - SW_OVERHEAD - Lmax;
+    uint64_t nL = 0, bL = 0;
+    for (uint64_t q = 0; q <= tiles / SUPER; q++) {
+        nL += sup[q];
+        bL += sup[tiles / SUPER + 1 + q];
+    }
+    const uint64_t n_repend = hq[0], ne = 2 * nL, total_s = 2 * bL;
+    /* 3. every buffer the rest needs, before any node is re-pended: the last entry starts below total_s, so
+       F <= total_s / B + 1 */
+    const uint64_t F_max = ne ? total_s / B + 1 : 0, total_max = SW_OVERHEAD * F_max + total_s;
+    const bool dev_out = o->flags & REGK_OUT_DEVICE;
+    FrameBufs &fb = wk.swframes;
+    if ((rc = ensure_dev(ctx, wk.sw_ent_src, ne * 8 + 16)) || (rc = ensure_dev(ctx, wk.sw_ent_s, ne * 8 + 16)) ||
+        (rc = ensure_dev(ctx, wk.sw_ent_len, ne * 4 + 16)) || (rc = ensure_dev(ctx, fb.bytes, total_max + 16)) ||
+        (rc = ensure_dev(ctx, fb.off, (F_max + 1) * 8)))
+        return rc;
+    if (!dev_out && ((rc = ensure_host(ctx, fb.h_bytes, total_max + 16)) || (rc = ensure_host(ctx, fb.h_off, (F_max + 1) * 8 + 16))))
+        return rc;
+    /* 4. place: the entries of D and C, and the re-pend marks */
+    wp.nD = nL;
+    wp.bD = bL;
+    wp.ent_src = (unsigned long long *)wk.sw_ent_src.p;
+    wp.ent_s = (unsigned long long *)wk.sw_ent_s.p;
+    wp.ent_len = (uint32_t *)wk.sw_ent_len.p;
+    if (m) {
+        regk_walk_sw_place_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(wp);
+        CK(cudaGetLastError());
+        launches++;
+    }
+    const unsigned long long mc[WM_NCOUNTERS] = {wk.n_pending + n_repend, wk.n_removed};
+    CK(cudaMemcpyAsync(wk.mcount.p, mc, sizeof mc, cudaMemcpyHostToDevice, s));
+    uint64_t F = 0;
+    if (ne) {
+        unsigned long long last_s = 0;
+        CK(cudaMemcpyAsync(&last_s, wp.ent_s + (ne - 1), 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        F = last_s / B + 1;
+    }
+    /* 5. the frames: regk_setwatches_requests' entry writer and frame heads, with E empty */
+    const uint64_t total = SW_OVERHEAD * F + total_s;
+    SwParams sp{};
+    sp.nD = nL;
+    sp.nE = 0;
+    sp.m = ne;
+    sp.bD = bL;
+    sp.bE = 0;
+    sp.total_s = total_s;
+    sp.B = B;
+    sp.zxid = wk.zxid;
+    sp.ent_src = wp.ent_src;
+    sp.ent_s = wp.ent_s;
+    sp.ent_len = wp.ent_len;
+    sp.path_bytes = (const uint8_t *)wk.snap_bytes[0].p;
+    sp.out = (uint8_t *)fb.bytes.p;
+    sp.frame_off = (unsigned long long *)fb.off.p;
+    sp.F = F;
+    if (ne) {
+        regk_sw_write_kernel<<<(unsigned)((ne + RP_TILE - 1) / RP_TILE), RP_TILE, 0, s>>>(sp);
+        regk_sw_head_kernel<<<(unsigned)((F + 255) / 256), 256, 0, s>>>(sp);
+        CK(cudaGetLastError());
+        launches += 2;
+    } else {
+        CK(cudaMemsetAsync(fb.off.p, 0, 8, s));
+    }
+    CK(cudaEventRecord(wk.swev[1], s));
+    const void *src[2] = {fb.bytes.p, fb.off.p};
+    if (!dev_out) {
+        if ((rc = to_host(ctx, fb.h_bytes, fb.bytes.p, total, s)) || (rc = to_host(ctx, fb.h_off, fb.off.p, (F + 1) * 8, s)))
+            return rc;
+        src[0] = fb.h_bytes.p;
+        src[1] = fb.h_off.p;
+    }
+    if ((rc = sync_or_fail(ctx, s, who)))
+        return rc;
+    float ms = 0;
+    cudaEventElapsedTime(&ms, wk.swev[0], wk.swev[1]);
+    wk.n_pending += n_repend;
+    wk.gate = true;
+    out->n_listed = nL;
+    out->n_repend = n_repend;
+    out->n_pending = wk.n_pending;
+    out->n_removed = wk.n_removed;
+    out->n_frontier = wk.f;
+    out->relative_zxid = wk.zxid;
+    out->frames.n = F;
+    out->frames.total = total;
+    out->frames.flags = dev_out ? REGK_OUT_DEVICE : 0;
+    out->frames.launches = launches;
+    out->frames.frame_bytes = (const uint8_t *)src[0];
+    out->frames.frame_off = (const uint64_t *)src[1];
+    out->frames.kernel_ms = ms;
     return REGK_OK;
 }
 
