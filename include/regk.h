@@ -1167,7 +1167,8 @@ int         regk_resolve(regk_ctx *ctx, const regk_decode_in *snapshot, const re
 
 /*
  * ---- DNS responses from the last regk_resolve: RFC 1035 query messages in, wire-format A and SRV responses out ------
- * Answers against the last regk_resolve on the context; REGK_ERR_STATE when there was none or it failed.  A device
+ * Answers against the last regk_resolve (or regk_walk_resolve, below) on the context; REGK_ERR_STATE when there was
+ * none or it failed, or when the walk's snapshot changed since that regk_walk_resolve.  A device
  * snapshot passed to that resolve must stay allocated and unchanged until the last regk_dns_answer on it (a host
  * snapshot was staged by the resolve).  Results stay valid until the next regk_dns_answer or regk_resolve.
  * Input: k messages back to back, no TCP length prefix; message i = msgs[off[i], off[i+1]).  Host memory, or device
@@ -1291,7 +1292,8 @@ int         regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns
  *   a host array.  REGK_OUT_DEVICE is accepted and changes nothing.  They stay valid until the next regk_read_walk or
  *   regk_walk_start: a read appends and may reallocate.  A regk_resolve given an earlier walk snapshot must therefore
  *   be redone before regk_dns_answer is used again: a device snapshot passed to that resolve must stay allocated and
- *   unchanged until the last regk_dns_answer on it.
+ *   unchanged until the last regk_dns_answer on it.  regk_walk_resolve (below) resolves the walk's own snapshot, and
+ *   regk_dns_answer refuses to answer from it once the snapshot has changed.
  * PARITY UNPINNED: the layouts are restated from zookeeper.jute and tested against an independent restatement, not
  * against a server.  A directory whose listing exceeds the server's jute.maxbuffer cannot be listed by any client, and
  * this call does not handle it.
@@ -1342,8 +1344,8 @@ int         regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns
  *   no watched parent: it stays gone until a new walk.
  * CONVERGENCE: once the tree stops changing and every byte has been fed, refreshing until nothing is pending or removed
  *   leaves a snapshot equal, as a set of (path, data, version, owner), to a fresh walk of the same roots (deleted roots
- *   aside); node order differs.  Re-resolve it (regk_resolve is not incremental).  After a reconnect, carry the walk
- *   over with regk_walk_setwatches below; after a session expiry, start a new watched walk.
+ *   aside); node order differs.  Resolve it with regk_walk_resolve (below), which formats only what changed.  After a
+ *   reconnect, carry the walk over with regk_walk_setwatches below; after a session expiry, start a new watched walk.
  * PARITY UNPINNED: restated from zookeeper.jute (WatcherEvent) and the server's watch rules (one-shot, per session; a
  *   getData on a missing node arms nothing; a watch still armed is not duplicated), not tested against a server.
  */
@@ -1444,7 +1446,8 @@ int         regk_walk_refresh(regk_ctx *ctx, uint32_t flags, regk_walk_refresh_o
  *   5. If n_frontier > 0, frame that level again (regk_walk_requests, a fresh xid base) and read it as usual.
  *   6. Refresh as usual.
  * CONVERGENCE: a walk carried over this way converges as a watched walk does: once the tree stops changing, refreshing
- *   until nothing is pending or removed leaves the set of a fresh walk of the same roots, deleted roots aside.  A
+ *   until nothing is pending or removed leaves the set of a fresh walk of the same roots, deleted roots aside; then
+ *   regk_walk_resolve brings the answers up to date, re-read nodes whose data did not change keeping their text.  A
  *   session expiry still means a new walk.
  * PARITY UNPINNED: the server's re-arming is restated from ZooKeeper 3.4's DataTree.setWatches, not tested against a
  *   server.
@@ -1459,6 +1462,51 @@ typedef struct regk_walk_setwatches_out {
 } regk_walk_setwatches_out;
 
 int         regk_walk_setwatches(regk_ctx *ctx, const regk_setwatches_opts *opts, regk_walk_setwatches_out *out);
+
+/*
+ * ---- a walk's answers kept current: re-resolve the walk's snapshot as it stands, reusing the last call's text for
+ * every answer whose inputs did not change -----------------------------------------------------------------------------
+ * regk_walk_resolve: REGK_ERR_STATE when there is no walk; batches in flight are refused as regk_resolve refuses them.
+ *   A walk in any phase is accepted (a level in flight, REMOVED nodes not yet refreshed, complete): what is resolved is
+ *   the walk's snapshot as it stands, which is what regk_resolve(ctx, &walk.snapshot, opts, ...) sees.
+ * RESULT: out->answers has every count (m, n_queries, n_answers, n_additional, n_unresolved, text_total) and every
+ *   array (q_kind, q_node, sec_off, text, node_cls, unresolved) byte-identical to what that regk_resolve would return;
+ *   launches and kernel_ms are this call's own.  opts is validated as regk_resolve validates it (the same refusals,
+ *   and the same refusal of a duplicate path naming the later node), the message naming this call.  Pinned host arrays,
+ *   or device arrays with REGK_OUT_DEVICE, valid until the next regk_walk_resolve, regk_resolve or regk_walk_start.
+ * regk_dns_answer then answers from this call as it answers after regk_resolve, byte for byte.  Once the walk's
+ *   snapshot has changed since the call (a regk_read_walk that appended or rebuilt, a regk_walk_refresh that rebuilt,
+ *   a regk_walk_start), regk_dns_answer returns REGK_ERR_STATE: resolve again.  After a plain regk_resolve it behaves as
+ *   it always did.
+ * IDENTITY: each walk snapshot node has an identity (its index at the last successful regk_walk_resolve) or none.
+ *   After a successful call every node has one.  A node a plain level appends has none.  A refresh-level getData with
+ *   err 0 takes a node's identity only when the new data bytes differ from its old ones (length or any byte); version
+ *   and owner enter no answer, so a re-read of unchanged data (e.g. of a node regk_walk_setwatches re-pended) keeps it.
+ *   The identity moves with its node through every rebuild, a node dropped as REMOVED takes it along, and
+ *   regk_walk_start clears everything, the kept text included.  This bookkeeping is not counted in any walk call's
+ *   launches or kernel_ms, and no walk call's outputs change.
+ * REUSE: full = 1 when there was no successful regk_walk_resolve since the last regk_walk_start, or its
+ *   default_host_ttl / default_srv_ttl differ from this call's: n_fresh = m, copied_bytes = 0, every line formatted.
+ *   Otherwise a HOST_A section is copied from the last call's text when its node has an identity, and a service child's
+ *   A line, SRV lines and additional line when the child and its service both have one; everything else is formatted.
+ *   This is exact: a node's class, roles and TTL depend only on its own path, data and opts; whether a node is a child
+ *   of a service, and the child's lines, depend only on the two of them; a node's path never changes.  So a copied run
+ *   holds the bytes regk_resolve would write.
+ * A refused or failed call keeps the last successful call's text and every identity (and, as regk_resolve, leaves no
+ *   answers for regk_dns_answer).  A plain regk_resolve in between does not break reuse: the kept text is this call's.
+ * The option "walk_resolve_segments" (regk_get_option) reports the last successful call's segments: the runs its text
+ *   was assembled from (0 when full).
+ */
+typedef struct regk_walk_answers {
+    regk_answers answers;           /* exactly regk_resolve's outputs for the walk's snapshot as it stands */
+    uint64_t n_fresh;               /* snapshot nodes without an identity at the last regk_walk_resolve (all m when full) */
+    uint64_t copied_bytes;          /* text bytes taken from the last regk_walk_resolve's text */
+    uint64_t formatted_bytes;       /* text_total - copied_bytes */
+    uint32_t full;                  /* 1: nothing to reuse, every line formatted */
+    uint32_t reserved;
+} regk_walk_answers;
+
+int         regk_walk_resolve(regk_ctx *ctx, const regk_resolve_opts *opts, regk_walk_answers *out);
 
 /* Tuning knobs (kernel variant selection for A/B measurement); see DESIGN.md. */
 int         regk_set_option(regk_ctx *ctx, const char *name, int64_t value);

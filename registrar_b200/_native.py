@@ -510,6 +510,22 @@ class Answers:
         return self.text[int(self.sec_off[2 * q + 1]):int(self.sec_off[2 * q + 2])].tobytes()
 
 
+class CWalkAnswers(C.Structure):     # regk_walk_answers
+    _fields_ = [("answers", CAnswers), ("n_fresh", C.c_uint64), ("copied_bytes", C.c_uint64),
+                ("formatted_bytes", C.c_uint64), ("full", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class WalkAnswers(Answers):
+    """Host copy of a regk_walk_answers: the Answers of the walk's snapshot as it stands, and how they were made: full
+    (1: every line formatted), n_fresh snapshot nodes without an identity from the last walk_resolve(), copied_bytes of
+    text taken from that call's text, formatted_bytes formatted anew."""
+
+    def __init__(self, out):
+        super().__init__(out.answers)
+        self.full, self.n_fresh = int(out.full), int(out.n_fresh)
+        self.copied_bytes, self.formatted_bytes = int(out.copied_bytes), int(out.formatted_bytes)
+
+
 class CDnsIn(C.Structure):           # regk_dns_in
     _fields_ = [("msgs", C.c_void_p), ("off", C.c_void_p), ("k", C.c_uint64), ("total", C.c_uint64),
                 ("flags", C.c_uint32), ("reserved", C.c_uint32)]
@@ -673,7 +689,8 @@ EXPORTS = ["regk_abi_version", "regk_create", "regk_destroy", "regk_last_error",
            "regk_read_replies", "regk_children_requests", "regk_read_children", "regk_read_results", "regk_read_stats",
            "regk_reconcile_stats", "regk_read_events", "regk_events_requests",
            "regk_setwatches_requests", "regk_resolve", "regk_dns_answer", "regk_walk_start", "regk_walk_requests",
-           "regk_read_walk", "regk_walk_events", "regk_walk_refresh", "regk_walk_setwatches"]
+           "regk_read_walk", "regk_walk_events", "regk_walk_refresh", "regk_walk_setwatches",
+           "regk_walk_resolve"]
 
 _lib = None
 
@@ -747,6 +764,7 @@ def load_library():
     lib.regk_walk_events.argtypes = [vp, vp, u64, u64, C.POINTER(CEventsOpts), C.POINTER(CWalkEvents)]
     lib.regk_walk_refresh.argtypes = [vp, u32, C.POINTER(CWalkRefresh)]
     lib.regk_walk_setwatches.argtypes = [vp, C.POINTER(CSetWatchesOpts), C.POINTER(CWalkSetWatches)]
+    lib.regk_walk_resolve.argtypes = [vp, C.POINTER(CResolveOpts), C.POINTER(CWalkAnswers)]
     _lib = lib
     return lib
 
@@ -1500,6 +1518,16 @@ class Context:
             raise ValueError("exchange returned %d SetWatches replies for %d frames" % (e.n_replies, r.n_frames))
         w, _ = self._walk_levels(exchange, int(xid_base) % 2 ** 32, r.n_frontier, True, getattr(self, "_walk", None))
         return r, w
+
+    def walk_resolve(self, default_host_ttl: int, default_srv_ttl: int, device: bool = False):
+        """regk_walk_resolve: the answers of the walk's snapshot as it stands, exactly what resolve(walk, ...) returns,
+        with every line whose inputs did not change since the last walk_resolve() copied from that call's text.
+        answer_dns() then answers from it until the walk's snapshot changes.  Returns a WalkAnswers, or the raw
+        CWalkAnswers (device pointers) with device=True."""
+        o = CResolveOpts(FLAG_OUT_DEVICE if device else 0, int(default_host_ttl), int(default_srv_ttl), 0)
+        out = CWalkAnswers()
+        self._check(self._lib.regk_walk_resolve(self._h, C.byref(o), C.byref(out)))
+        return out if device else WalkAnswers(out)
 
     def _d2h(self, ptr, count, dtype):
         out = np.zeros(count, dtype)

@@ -44,6 +44,7 @@
 #include "regk_walk.cuh"
 #include "regk_walk_watch.cuh"
 #include "regk_walk_setwatches.cuh"
+#include "regk_walk_resolve.cuh"
 #include "regk_types.hpp"
 
 using namespace regk;
@@ -344,6 +345,8 @@ struct regk_ctx {
         Event ev[5];
         /* the last call succeeded: regk_dns_answer answers against it (the snapshot streams it read, its table size) */
         bool valid = false;
+        bool walk = false;                      /* it was a regk_walk_resolve, of walk snapshot generation walk_sgen */
+        uint64_t walk_sgen = 0;
         uint64_t gen = 0, m = 0, path_total = 0, slots = 0;
         const uint8_t *pb = nullptr, *jb = nullptr;
         const uint64_t *po = nullptr, *jo = nullptr;
@@ -399,7 +402,21 @@ struct regk_ctx {
         bool gate = false;
         FrameBufs swframes;
         Event swev[2];
+        /* regk_walk_resolve (regk_walk_resolve.cuh): the identity word per node (ident2: the rebuild's copy), and the
+           snapshot generation, bumped whenever the snapshot's nodes or buffers change (regk_dns_answer's gate) */
+        DevBuf ident, ident2;
+        uint64_t sgen = 0;
     } wk;
+    /* regk_walk_resolve: the last successful call (have; its default TTLs) and its text and run offsets (set cur; the
+       other set is written by the next call and becomes cur on success), the pieces and segments of one call */
+    struct WalkResolve {
+        bool have = false;
+        int cur = 0;
+        int32_t dflt_host = 0, dflt_srv = 0;
+        uint64_t segments = 0;
+        DevBuf text[2], run[2], kind, len, src, dest, totals, count, seg_src, seg_dest, seg_sel, seg_len, seg_off, scratch;
+        Event ev[4];
+    } wr;
     std::vector<Event> pipe_events;             /* run_pipelined */
     /* skip mode (regk_skip.cuh): fence workspace, the compacted batch, the expanded offsets, the skipped list */
     struct Skip {
@@ -1309,6 +1326,8 @@ int64_t regk_get_option(const regk_ctx *ctx, const char *name)
         return -1;
     if (!strcmp(name, "sm_count"))
         return ctx->sm_count;
+    if (!strcmp(name, "walk_resolve_segments"))
+        return (int64_t)ctx->wr.segments;
     return opt_get(ctx, name, 0);
 }
 
@@ -5652,13 +5671,21 @@ int regk_setwatches_requests(regk_ctx *ctx, const regk_setwatches_opts *o, regk_
     return REGK_OK;
 }
 
-int regk_resolve(regk_ctx *ctx, const regk_decode_in *in, const regk_resolve_opts *o, regk_answers *out)
+/* regk_resolve's passes up to the text (shared with regk_walk_resolve): the checks, the insert, decode, classify,
+   join, sort, child_len / child_scan and qlen / place passes, and the counters they leave */
+struct ResolveRun {
+    ResolveParams p;
+    uint64_t m = 0, nq = 0, text_total = 0, n_unres = 0, path_total = 0, slots = 0;
+    unsigned long long answers = 0, additional = 0;
+    bool dev_out = false;
+    uint32_t launches = 0;
+    float ms = 0;
+    const uint8_t *pb = nullptr, *jb = nullptr;
+    const uint64_t *po = nullptr, *jo = nullptr;
+};
+
+static int resolve_meta(regk_ctx *ctx, const regk_decode_in *in, const regk_resolve_opts *o, const char *who, ResolveRun *run)
 {
-    const char *who = "regk_resolve";
-    if (!ctx || !in || !o || !out)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_resolve: NULL argument");
-    memset(out, 0, sizeof *out);
-    ctx->rsv.valid = false;
     if (in->flags & REGK_DECODE_LAST)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams", who);
     if (o->flags & ~REGK_OUT_DEVICE)
@@ -5869,22 +5896,39 @@ int regk_resolve(regk_ctx *ctx, const regk_decode_in *in, const regk_resolve_opt
     cudaEventElapsedTime(&ms, rb.ev[0], rb.ev[1]);
     cudaEventElapsedTime(&part, rb.ev[2], rb.ev[3]);
     ms += part;
-    const uint64_t nq = m ? hc[RV_C_QUERIES] : 0, text_total = m ? hc[RV_C_TEXT] : 0, n_unres = m ? hc[RV_C_UNRESOLVED] : 0;
-    /* 7. emit */
-    if ((rc = ensure_dev(ctx, rb.text, text_total + 16)))
-        return rc;
-    p.text = (uint8_t *)rb.text.p;
-    CK(cudaEventRecord(rb.ev[3], s));
-    if (m && text_total) {
-        regk_resolve_emit_kernel<<<(unsigned)((2 * m + 255) / 256), 256, 0, s>>>(p);
-        CK(cudaGetLastError());
-        launches++;
-    }
-    CK(cudaEventRecord(rb.ev[4], s));
-    const void *dsrc[6] = {rb.q_kind.p, rb.q_node.p, rb.sec_off.p, rb.text.p, rb.cls.p, rb.unres.p};
-    if (!dev_out) {
+    run->p = p;
+    run->m = m;
+    run->nq = m ? hc[RV_C_QUERIES] : 0;
+    run->text_total = m ? hc[RV_C_TEXT] : 0;
+    run->n_unres = m ? hc[RV_C_UNRESOLVED] : 0;
+    run->answers = m ? hc[RV_C_ANSWERS] : 0;
+    run->additional = m ? hc[RV_C_ADDITIONAL] : 0;
+    run->path_total = path_total;
+    run->slots = slots;
+    run->dev_out = dev_out;
+    run->launches = launches;
+    run->ms = ms;
+    run->pb = pb;
+    run->po = po;
+    run->jb = jb;
+    run->jo = jo;
+    return REGK_OK;
+}
+
+/* The answers of a resolve whose text is `text` (device): copied out unless REGK_OUT_DEVICE, kernel_ms adding the
+   events [a, b), and the state regk_dns_answer answers from. */
+static int resolve_publish(regk_ctx *ctx, const ResolveRun &r, const void *text, cudaEvent_t a, cudaEvent_t b, regk_answers *out,
+    const char *who)
+{
+    regk_ctx::Resolve &rb = ctx->rsv;
+    cudaStream_t s = ctx->stream;
+    int rc;
+    const uint64_t m = r.m, nq = r.nq;
+    const void *dsrc[6] = {rb.q_kind.p, rb.q_node.p, rb.sec_off.p, text, rb.cls.p, rb.unres.p};
+    if (!r.dev_out) {
         HostBuf *hb[6] = {&rb.h_q_kind, &rb.h_q_node, &rb.h_sec_off, &rb.h_text, &rb.h_cls, &rb.h_unres};
-        const size_t sz[6] = {(size_t)nq, (size_t)nq * 8, (size_t)(2 * nq + 1) * 8, (size_t)text_total, (size_t)m, (size_t)n_unres * 8};
+        const size_t sz[6] = {(size_t)nq, (size_t)nq * 8, (size_t)(2 * nq + 1) * 8, (size_t)r.text_total, (size_t)m,
+                              (size_t)r.n_unres * 8};
         for (int k = 0; k < 6; k++) {
             if ((rc = to_host(ctx, *hb[k], dsrc[k], sz[k], s)))
                 return rc;
@@ -5893,33 +5937,61 @@ int regk_resolve(regk_ctx *ctx, const regk_decode_in *in, const regk_resolve_opt
     }
     if ((rc = sync_or_fail(ctx, s, who)))
         return rc;
-    cudaEventElapsedTime(&part, rb.ev[3], rb.ev[4]);
-    ms += part;
+    float part = 0;
+    cudaEventElapsedTime(&part, a, b);
     out->m = m;
     out->n_queries = nq;
-    out->n_answers = m ? hc[RV_C_ANSWERS] : 0;
-    out->n_additional = m ? hc[RV_C_ADDITIONAL] : 0;
-    out->n_unresolved = n_unres;
-    out->text_total = text_total;
-    out->flags = dev_out ? REGK_OUT_DEVICE : 0;
-    out->launches = launches;
+    out->n_answers = r.answers;
+    out->n_additional = r.additional;
+    out->n_unresolved = r.n_unres;
+    out->text_total = r.text_total;
+    out->flags = r.dev_out ? REGK_OUT_DEVICE : 0;
+    out->launches = r.launches;
     out->q_kind = (const uint8_t *)dsrc[0];
     out->q_node = (const uint64_t *)dsrc[1];
     out->sec_off = (const uint64_t *)dsrc[2];
     out->text = (const uint8_t *)dsrc[3];
     out->node_cls = (const uint8_t *)dsrc[4];
     out->unresolved = (const uint64_t *)dsrc[5];
-    out->kernel_ms = ms;
+    out->kernel_ms = r.ms + part;
     rb.valid = true;
+    rb.walk = false;
     rb.gen++;
     rb.m = m;
-    rb.path_total = path_total;
-    rb.slots = slots;
-    rb.pb = pb;
-    rb.po = po;
-    rb.jb = jb;
-    rb.jo = jo;
+    rb.path_total = r.path_total;
+    rb.slots = r.slots;
+    rb.pb = r.pb;
+    rb.po = r.po;
+    rb.jb = r.jb;
+    rb.jo = r.jo;
     return REGK_OK;
+}
+
+int regk_resolve(regk_ctx *ctx, const regk_decode_in *in, const regk_resolve_opts *o, regk_answers *out)
+{
+    const char *who = "regk_resolve";
+    if (!ctx || !in || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_resolve: NULL argument");
+    memset(out, 0, sizeof *out);
+    ctx->rsv.valid = false;
+    ResolveRun r;
+    int rc;
+    if ((rc = resolve_meta(ctx, in, o, who, &r)))
+        return rc;
+    regk_ctx::Resolve &rb = ctx->rsv;
+    cudaStream_t s = ctx->stream;
+    /* 7. emit */
+    if ((rc = ensure_dev(ctx, rb.text, r.text_total + 16)))
+        return rc;
+    r.p.text = (uint8_t *)rb.text.p;
+    CK(cudaEventRecord(rb.ev[3], s));
+    if (r.m && r.text_total) {
+        regk_resolve_emit_kernel<<<(unsigned)((2 * r.m + 255) / 256), 256, 0, s>>>(r.p);
+        CK(cudaGetLastError());
+        r.launches++;
+    }
+    CK(cudaEventRecord(rb.ev[4], s));
+    return resolve_publish(ctx, r, rb.text.p, rb.ev[3], rb.ev[4], out, who);
 }
 
 int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o, regk_dns_out *out)
@@ -5939,6 +6011,9 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
     const regk_ctx::Resolve &rb = ctx->rsv;
     if (!rb.valid)
         return fail(ctx, REGK_ERR_STATE, "%s: no successful regk_resolve on this context to answer from", who);
+    if (rb.walk && rb.walk_sgen != ctx->wk.sgen)
+        return fail(ctx, REGK_ERR_STATE, "%s: the walk's snapshot changed since regk_walk_resolve; resolve it again "
+                                         "(regk_walk_resolve) before answering", who);
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "%s: batches are still in flight; finish them first", who);
     const uint64_t k = in->k, m = rb.m;
@@ -6228,7 +6303,8 @@ static int walk_rebuild_reserve(regk_ctx *ctx, uint64_t extra)
         (rc = ensure_dev(ctx, wk.dsrc, m8)) || (rc = ensure_dev(ctx, wk.kplen, m4)) || (rc = ensure_dev(ctx, wk.kdlen, m4)) ||
         (rc = ensure_dev(ctx, wk.dsel, m + 16)) || (rc = ensure_dev(ctx, wk.wmark2, m4)) || (rc = ensure_dev(ctx, wk.ver2, m4)) ||
         (rc = ensure_dev(ctx, wk.own2, m8)) || (rc = ensure_dev(ctx, wk.rpos, m8)) || (rc = ensure_dev(ctx, wk.rlen, m4)) ||
-        (rc = ensure_dev(ctx, wk.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)) || (rc = ensure_dev(ctx, wk.armed2, m + 16)))
+        (rc = ensure_dev(ctx, wk.gtotals, gt * 8 + (gt / SUPER + 1) * 8 + 16)) || (rc = ensure_dev(ctx, wk.armed2, m + 16)) ||
+        (rc = ensure_dev(ctx, wk.ident2, m4)))
         return rc;
     const uint64_t bytes[2] = {wk.path_total, wk.data_total + extra};
     for (int g = 0; g < 2; g++)
@@ -6376,6 +6452,10 @@ static int walk_rebuild(regk_ctx *ctx, const uint8_t *ds, uint32_t *launches, co
         regk_walk_keep_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(kp);
         /* the armed bytes move with their nodes; not counted in `launches` (bookkeeping for regk_walk_setwatches) */
         regk_walk_keep_armed_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(kp, (const uint8_t *)wk.armed.p, (uint8_t *)wk.armed2.p);
+        /* so do the identities, a replaced node's only while its data bytes stay the same (regk_walk_resolve's
+           bookkeeping, not counted either) */
+        regk_walk_keep_ident_kernel<<<(unsigned)tiles, RP_TILE, 0, s>>>(kp, (const uint32_t *)wk.ident.p, (uint32_t *)wk.ident2.p,
+            (const uint8_t *)wk.snap_bytes[1].p, ds);
         CK(cudaGetLastError());
         *launches += 2;
         CK(cudaMemcpyAsync(kc, kp.counters, 16, cudaMemcpyDeviceToHost, s));
@@ -6394,11 +6474,13 @@ static int walk_rebuild(regk_ctx *ctx, const uint8_t *ds, uint32_t *launches, co
     }
     std::swap(wk.wmark, wk.wmark2);
     std::swap(wk.armed, wk.armed2);
+    std::swap(wk.ident, wk.ident2);
     std::swap(wk.ver, wk.ver2);
     std::swap(wk.own, wk.own2);
     const unsigned long long mc[WM_NCOUNTERS] = {kc[1], 0ull};
     CK(cudaMemcpyAsync(wk.mcount.p, mc, sizeof mc, cudaMemcpyHostToDevice, s));
     CK(cudaStreamSynchronize(s));
+    wk.sgen++;
     wk.m = k;
     wk.path_total = tot[0];
     wk.data_total = tot[1];
@@ -6454,6 +6536,8 @@ int regk_walk_start(regk_ctx *ctx, const uint8_t *roots, const uint64_t *root_of
     CK(cudaSetDevice(ctx->device));
     regk_ctx::Walk &wk = ctx->wk;
     wk.active = wk.framed = false;              /* the earlier walk is gone even if staging fails */
+    wk.sgen++;
+    ctx->wr.have = false;                       /* regk_walk_resolve's kept text goes with the earlier walk */
     std::vector<uint8_t> pb;
     std::vector<unsigned long long> po(n_roots + 1, 0);
     std::vector<uint32_t> pl(n_roots);
@@ -6993,6 +7077,8 @@ int regk_read_walk(regk_ctx *ctx, const uint8_t *bytes, uint64_t len, uint32_t f
         am.watch = wk.framed_watch ? 1u : 0u;
         am.armed = (uint8_t *)wk.armed.p;
         regk_walk_arm_kernel<<<(unsigned)((mf + 255) / 256), 256, 0, s>>>(am);
+        /* regk_walk_resolve's: an appended node has no identity */
+        CK(cudaMemsetAsync((uint32_t *)wk.ident.p + m0, 0xFF, mf * 4, s));
     }
     CK(cudaMemsetAsync(wk.zmax.p, 0, 8, s));
     for (const RepParams *q : {&pg, &pf})
@@ -7032,6 +7118,7 @@ static int walk_append(regk_ctx *ctx, const uint8_t *ds, const uint8_t *fbytes, 
     regk_ctx::Walk &wk = ctx->wk;
     cudaStream_t s = ctx->stream;
     const uint64_t m0 = wk.m;
+    const void *was[4] = {wk.snap_bytes[0].p, wk.snap_bytes[1].p, wk.snap_off[0].p, wk.snap_off[1].p};
     int rc;
     uint64_t tot[2] = {0, 0};
     for (int g = 0; g < 2; g++) {
@@ -7047,7 +7134,8 @@ static int walk_append(regk_ctx *ctx, const uint8_t *ds, const uint8_t *fbytes, 
             (rc = walk_grow(ctx, wk.snap_off[g], m0 * 8, (m0 + mf + 1) * 8)))
             return rc;
     if ((rc = walk_grow(ctx, wk.ver, m0 * 4, (m0 + mf) * 4 + 16)) || (rc = walk_grow(ctx, wk.own, m0 * 8, (m0 + mf) * 8 + 16)) ||
-        (rc = walk_grow(ctx, wk.wmark, m0 * 4, (m0 + mf) * 4 + 16)) || (rc = walk_grow(ctx, wk.armed, m0, m0 + mf + 16)))
+        (rc = walk_grow(ctx, wk.wmark, m0 * 4, (m0 + mf) * 4 + 16)) || (rc = walk_grow(ctx, wk.armed, m0, m0 + mf + 16)) ||
+        (rc = walk_grow(ctx, wk.ident, m0 * 4, (m0 + mf) * 4 + 16)))
         return rc;
     for (int g = 0; g < 2; g++) {
         WalkAppendParams ap{};
@@ -7068,6 +7156,9 @@ static int walk_append(regk_ctx *ctx, const uint8_t *ds, const uint8_t *fbytes, 
         CK(cudaMemcpyAsync((long long *)wk.own.p + m0, fp.node_own, mf * 8, cudaMemcpyDeviceToDevice, s));
         CK(cudaMemsetAsync((uint32_t *)wk.wmark.p + m0, 0, mf * 4, s));
     }
+    if (mf || was[0] != wk.snap_bytes[0].p || was[1] != wk.snap_bytes[1].p || was[2] != wk.snap_off[0].p ||
+        was[3] != wk.snap_off[1].p)
+        wk.sgen++;
     wk.m = m0 + mf;
     wk.path_total += tot[0];
     wk.data_total += tot[1];
@@ -7580,6 +7671,165 @@ int regk_walk_setwatches(regk_ctx *ctx, const regk_setwatches_opts *o, regk_walk
     out->frames.frame_bytes = (const uint8_t *)src[0];
     out->frames.frame_off = (const uint64_t *)src[1];
     out->frames.kernel_ms = ms;
+    return REGK_OK;
+}
+
+int regk_walk_resolve(regk_ctx *ctx, const regk_resolve_opts *o, regk_walk_answers *out)
+{
+    const char *who = "regk_walk_resolve";
+    if (!ctx || !o || !out)
+        return fail(ctx, REGK_ERR_INVALID_ARG, "regk_walk_resolve: NULL argument");
+    memset(out, 0, sizeof *out);
+    ctx->rsv.valid = false;
+    regk_ctx::Walk &wk = ctx->wk;
+    if (!wk.active)
+        return fail(ctx, REGK_ERR_STATE, "%s: no walk on this context; call regk_walk_start first", who);
+    regk_decode_in in{};
+    in.n = wk.m;
+    in.flags = REGK_IN_DEVICE;
+    in.path_total = wk.path_total;
+    in.json_total = wk.data_total;
+    in.path_bytes = (const uint8_t *)wk.snap_bytes[0].p;
+    in.path_off = (const uint64_t *)wk.snap_off[0].p;
+    in.json_bytes = (const uint8_t *)wk.snap_bytes[1].p;
+    in.json_off = (const uint64_t *)wk.snap_off[1].p;
+    /* 1. regk_resolve's passes, unchanged: everything but the text */
+    ResolveRun r;
+    int rc;
+    if ((rc = resolve_meta(ctx, &in, o, who, &r)))
+        return rc;
+    regk_ctx::WalkResolve &wr = ctx->wr;
+    cudaStream_t s = ctx->stream;
+    const uint64_t m = r.m, T = r.text_total;
+    const bool full = !wr.have || wr.dflt_host != o->default_host_ttl || wr.dflt_srv != o->default_srv_ttl;
+    const int nx = 1 - wr.cur;
+    for (Event &ev : wr.ev)
+        if ((rc = ensure_event(ctx, ev)))
+            return rc;
+    if ((rc = ensure_dev(ctx, wr.text[nx], T + 16)) || (rc = ensure_dev(ctx, wr.run[nx], m * 32 + 16)) ||
+        (rc = ensure_dev(ctx, wr.text[wr.cur], 16)) || (rc = ensure_dev(ctx, wr.run[wr.cur], 16)))
+        return rc;
+    /* every host buffer the results need, first: nothing after the stamp can fail on an allocation */
+    if (!r.dev_out) {
+        regk_ctx::Resolve &rb = ctx->rsv;
+        HostBuf *hb[6] = {&rb.h_q_kind, &rb.h_q_node, &rb.h_sec_off, &rb.h_text, &rb.h_cls, &rb.h_unres};
+        const size_t sz[6] = {(size_t)r.nq, (size_t)r.nq * 8, (size_t)(2 * r.nq + 1) * 8, (size_t)T, (size_t)m, (size_t)r.n_unres * 8};
+        for (int k = 0; k < 6; k++)
+            if ((rc = ensure_host(ctx, *hb[k], sz[k] + 16)))
+                return rc;
+    }
+    WalkResolveParams w{};
+    w.r = r.p;
+    w.r.text = (uint8_t *)wr.text[nx].p;
+    w.ident = (const uint32_t *)wk.ident.p;
+    w.run_old = (const unsigned long long *)wr.run[wr.cur].p;
+    w.run_new = (unsigned long long *)wr.run[nx].p;
+    w.ident_out = (uint32_t *)wk.ident.p;
+    w.text_total = T;
+    uint64_t n_fresh = m, formatted = T, nseg = 0;
+    float part = 0;
+    const unsigned g2m = (unsigned)((2 * m + 255) / 256);
+    if (full) {
+        /* 2. nothing to reuse: regk_resolve's emit into this call's text */
+        CK(cudaEventRecord(wr.ev[2], s));
+        if (m && T) {
+            regk_resolve_emit_kernel<<<g2m, 256, 0, s>>>(w.r);
+            CK(cudaGetLastError());
+            r.launches++;
+        }
+    } else if (m) {
+        /* 2. plan the pieces; 3. segments and scratch offsets */
+        const uint64_t n_slots = 4 * m, tiles = (n_slots + RV_TILE - 1) / RV_TILE, nsup = tiles / SUPER + 1;
+        const size_t tb = 2 * (tiles + nsup) * 8;
+        if ((rc = ensure_dev(ctx, wr.kind, n_slots + 16)) || (rc = ensure_dev(ctx, wr.len, n_slots * 4 + 16)) ||
+            (rc = ensure_dev(ctx, wr.src, n_slots * 8 + 16)) || (rc = ensure_dev(ctx, wr.dest, n_slots * 8 + 16)) ||
+            (rc = ensure_dev(ctx, wr.totals, tb)) || (rc = ensure_dev(ctx, wr.count, WR_NCOUNTERS * 8)))
+            return rc;
+        w.n_slots = n_slots;
+        w.kind = (uint8_t *)wr.kind.p;
+        w.len = (uint32_t *)wr.len.p;
+        w.src = (unsigned long long *)wr.src.p;
+        w.dest = (unsigned long long *)wr.dest.p;
+        unsigned long long *tt = (unsigned long long *)wr.totals.p;
+        for (int k = 0; k < 2; k++) {
+            w.stile[k] = tt + (size_t)k * (tiles + nsup);
+            w.ssuper[k] = w.stile[k] + tiles;
+        }
+        w.counters = (unsigned long long *)wr.count.p;
+        CK(cudaMemsetAsync(wr.kind.p, 0, n_slots, s));
+        CK(cudaMemsetAsync(wr.totals.p, 0, tb, s));
+        CK(cudaMemsetAsync(wr.count.p, 0, WR_NCOUNTERS * 8, s));
+        CK(cudaEventRecord(wr.ev[0], s));
+        regk_walk_resolve_plan_kernel<<<g2m, 256, 0, s>>>(w);
+        regk_walk_resolve_seg_count_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(w);
+        CK(cudaGetLastError());
+        r.launches += 2;
+        CK(cudaEventRecord(wr.ev[1], s));
+        std::vector<unsigned long long> sup(2 * nsup + WR_NCOUNTERS);
+        for (int k = 0; k < 2; k++)
+            CK(cudaMemcpyAsync(sup.data() + k * nsup, w.ssuper[k], nsup * 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(sup.data() + 2 * nsup, w.counters, WR_NCOUNTERS * 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        cudaEventElapsedTime(&part, wr.ev[0], wr.ev[1]);
+        r.ms += part;
+        formatted = 0;
+        for (uint64_t q = 0; q < nsup; q++) {
+            nseg += sup[q];
+            formatted += sup[nsup + q];
+        }
+        n_fresh = sup[2 * nsup + WR_C_FRESH_NODES];
+        if ((rc = ensure_dev(ctx, wr.seg_src, nseg * 8 + 16)) || (rc = ensure_dev(ctx, wr.seg_dest, nseg * 8 + 16)) ||
+            (rc = ensure_dev(ctx, wr.seg_sel, nseg + 16)) || (rc = ensure_dev(ctx, wr.seg_len, nseg * 4 + 16)) ||
+            (rc = ensure_dev(ctx, wr.seg_off, (nseg + 1) * 8 + 16)) || (rc = ensure_dev(ctx, wr.scratch, formatted + 16)))
+            return rc;
+        w.seg_src = (unsigned long long *)wr.seg_src.p;
+        w.seg_dest = (unsigned long long *)wr.seg_dest.p;
+        w.seg_sel = (uint8_t *)wr.seg_sel.p;
+        w.seg_len = (uint32_t *)wr.seg_len.p;
+        w.n_seg = nseg;
+        w.scratch = (uint8_t *)wr.scratch.p;
+        /* 4. the formatted pieces; 5. the text, output-stationary, from the old text and the scratch stream */
+        CK(cudaEventRecord(wr.ev[2], s));
+        regk_walk_resolve_seg_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(w);
+        r.launches++;
+        if (formatted) {
+            regk_walk_resolve_fresh_kernel<<<g2m, 256, 0, s>>>(w);
+            r.launches++;
+        }
+        if (nseg) {
+            regk_walk_resolve_seg_len_kernel<<<(unsigned)((nseg + 255) / 256), 256, 0, s>>>(w);
+            r.launches++;
+        }
+        CK(cudaGetLastError());
+        uint64_t packed = 0;
+        if ((rc = walk_pack(ctx, nseg, (const uint8_t *)wr.text[wr.cur].p, w.scratch, w.seg_src, w.seg_sel, w.seg_len,
+                 wr.text[nx], wr.seg_off, &packed, &r.launches)))
+            return rc;
+        w.r.text = (uint8_t *)wr.text[nx].p;
+    } else {
+        CK(cudaEventRecord(wr.ev[2], s));
+    }
+    /* 6. stamp: this call's run offsets and identities, for the next call */
+    if (m) {
+        regk_walk_resolve_stamp_kernel<<<g2m, 256, 0, s>>>(w);
+        CK(cudaGetLastError());
+        r.launches++;
+    }
+    CK(cudaEventRecord(wr.ev[3], s));
+    if ((rc = resolve_publish(ctx, r, wr.text[nx].p, wr.ev[2], wr.ev[3], &out->answers, who)))
+        return rc;
+    ctx->rsv.walk = true;
+    ctx->rsv.walk_sgen = wk.sgen;
+    wr.cur = nx;
+    wr.have = true;
+    wr.dflt_host = o->default_host_ttl;
+    wr.dflt_srv = o->default_srv_ttl;
+    wr.segments = nseg;
+    out->n_fresh = n_fresh;
+    out->copied_bytes = T - formatted;
+    out->formatted_bytes = formatted;
+    out->full = full ? 1u : 0u;
     return REGK_OK;
 }
 
