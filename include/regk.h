@@ -1213,8 +1213,28 @@ int         regk_resolve(regk_ctx *ctx, const regk_decode_in *snapshot, const re
  * PARITY UNPINNED (Binder is absent): its rcode for empty non-terminals and names outside its zones; AA and the
  * header bits; answer order and shuffling; its truncation policy; case handling; the form of error responses.  The
  * wire format is RFC 1035, 2782 and 6891.
+ * ---- with REGK_DNS_PTR: reverse lookups.  Rules 1-8 are unchanged; rule 9 gains a third kind of owner:
+ *   reverse name  exactly six labels o4.o3.o2.o1.in-addr.arpa: the last two equal "in-addr" and "arpa"
+ *                 case-insensitively, each octet label 1-3 ASCII digits of value <= 255 without a leading zero ("0"
+ *                 is one, "00", "01" and "256" are not); its address is o1.o2.o3.o4.  Any other name, a partial one
+ *                 such as 3.2.1.in-addr.arpa included, is not a reverse name.
+ *   targets(a)    every snapshot node c with a REGK_Q_HOST_A query whose addr(c) is a, in ascending node order (so
+ *                 ops_host and rr_host records, and nodes that are not class OK, are never targets)
+ *   A reverse name owns PTR when its address has a target; A and SRV ownership are as above.  QTYPE PTR (12) on a
+ *   PTR owner: ANSWER with one PTR RR per target; any other QTYPE on a name that owns A, SRV or PTR: NODATA;
+ *   otherwise NXDOMAIN.  node[i] of a PTR answer is its smallest target.
+ *   PTR    owner 0xC00C, TYPE 12, CLASS IN, TTL a_ttl(c), RDLENGTH L + 2, name(c) uncompressed (RFC 1035 3.3.12):
+ *          14 + L bytes for a name of L text bytes; targets in order
+ *   Size limit as above: the longest prefix of the PTR RRs that fits, no additionals; tc is 1 exactly when a PTR RR
+ *   was left out.
+ *   The reverse index is built once per resolve, on the first REGK_DNS_PTR call after it (launches counts it there:
+ *   two compaction kernels, then, when there is a host node, the radix sort as one and two prefix kernels); a call without the flag neither builds nor
+ *   drops it and launches exactly the kernels it launched before the flag existed.
+ * PARITY UNPINNED (Binder is absent): whether Binder answers PTR at all, its owner set and their order, the TTL, and
+ * its rcode for partial reverse names.  The wire format is RFC 1035 3.3.12 and 3.5.
  */
 #define REGK_DNS_TCP (1u << 8)      /* regk_dns_opts.flags: a 65535-byte limit (no TCP length prefix is written) */
+#define REGK_DNS_PTR (1u << 11)     /* regk_dns_opts.flags: answer PTR for in-addr.arpa names (below) */
 
 typedef struct regk_dns_in {
     const uint8_t  *msgs;           /* k query messages, back to back */
@@ -1225,7 +1245,7 @@ typedef struct regk_dns_in {
 } regk_dns_in;
 
 typedef struct regk_dns_opts {
-    uint32_t flags;                 /* REGK_OUT_DEVICE | REGK_DNS_TCP */
+    uint32_t flags;                 /* REGK_OUT_DEVICE | REGK_DNS_TCP | REGK_DNS_PTR */
     uint32_t udp_payload;           /* the server's EDNS0 UDP size, 512..65535 (e.g. 1232) */
 } regk_dns_opts;
 

@@ -544,6 +544,7 @@ class CDnsOut(C.Structure):          # regk_dns_out
 (DNS_ANSWER, DNS_NODATA, DNS_NXDOMAIN, DNS_FORMERR, DNS_NOTIMP, DNS_REFUSED, DNS_BADVERS,
  DNS_DROPPED) = range(8)                                             # DnsResponses.status
 FLAG_DNS_TCP = 1 << 8                                                # CDnsOpts.flags
+FLAG_DNS_PTR = 1 << 11                                               # CDnsOpts.flags: PTR for in-addr.arpa names
 
 
 class DnsResponses:
@@ -1352,12 +1353,13 @@ class Context:
         self._check(rc)
         return out if device else Answers(out)
 
-    def answer_dns(self, msgs, off, udp_payload: int = 1232, tcp: bool = False, device: bool = False):
+    def answer_dns(self, msgs, off, udp_payload: int = 1232, tcp: bool = False, device: bool = False, ptr: bool = False):
         """regk_dns_answer: responses to the query messages msgs[off[i]:off[i+1]] (NumPy uint8 bytes and int64 / uint64
         offsets, or contiguous CUDA uint8 and int64 tensors), answered from the last resolve() on this context.
-        udp_payload is the server's EDNS0 UDP size; tcp=True allows 65535 bytes.  Returns a DnsResponses, or the raw
-        CDnsOut (arrays on the device) with device=True."""
-        flags = (FLAG_OUT_DEVICE if device else 0) | (FLAG_DNS_TCP if tcp else 0)
+        udp_payload is the server's EDNS0 UDP size; tcp=True allows 65535 bytes; ptr=True answers PTR queries for
+        in-addr.arpa names with the names of the hosts at that address.  Returns a DnsResponses, or the raw CDnsOut
+        (arrays on the device) with device=True."""
+        flags = (FLAG_OUT_DEVICE if device else 0) | (FLAG_DNS_TCP if tcp else 0) | (FLAG_DNS_PTR if ptr else 0)
         if hasattr(msgs, "data_ptr"):
             import torch
             if not msgs.is_cuda or msgs.dtype != torch.uint8 or not msgs.is_contiguous():

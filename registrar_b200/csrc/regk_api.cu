@@ -41,6 +41,7 @@
 #include "regk_setwatches.cuh"
 #include "regk_resolve.cuh"
 #include "regk_dns.cuh"
+#include "regk_dns_ptr.cuh"
 #include "regk_walk.cuh"
 #include "regk_walk_watch.cuh"
 #include "regk_walk_setwatches.cuh"
@@ -352,11 +353,13 @@ struct regk_ctx {
         const uint64_t *po = nullptr, *jo = nullptr;
     } rsv;
     /* regk_dns_answer (regk_dns.cuh): the per-resolve preparation (of resolve generation prep_gen), the staged queries,
-       the per-query arrays and the responses */
+       the per-query arrays and the responses.  REGK_DNS_PTR (regk_dns_ptr.cuh): the reverse index of resolve generation
+       ptr_gen (0: not built), its n host nodes, the sort's inputs and temporary storage, its tile totals */
     struct Dns {
-        uint64_t prep_gen = 0;
+        uint64_t prep_gen = 0, ptr_gen = 0, ptr_n = 0;
         DevBuf ip4, cum[3], ptotals, in[2], scratch, status, tc, node, meta, nans, nadd, ans_bytes, qtotals, resp_off, rr_base,
             count, resp;
+        DevBuf pkey_in, pval_in, pkey, pval, pbytes, ptr_tmp, ptr_totals, ptr_count;
         HostBuf h_count, h_resp_off, h_resp, h_status, h_tc, h_node;
         Event ev[4];
     } dns;
@@ -6004,8 +6007,9 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: unknown input flag bits 0x%x", who, in->flags & ~REGK_IN_DEVICE);
     if (in->reserved)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: reserved must be 0", who);
-    if (o->flags & ~(REGK_OUT_DEVICE | REGK_DNS_TCP))
-        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: unknown flag bits 0x%x", who, o->flags & ~(REGK_OUT_DEVICE | REGK_DNS_TCP));
+    if (o->flags & ~(REGK_OUT_DEVICE | REGK_DNS_TCP | REGK_DNS_PTR))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: unknown flag bits 0x%x", who,
+            o->flags & ~(REGK_OUT_DEVICE | REGK_DNS_TCP | REGK_DNS_PTR));
     if (o->udp_payload < 512u || o->udp_payload > 65535u)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: udp_payload %u outside 512..65535", who, o->udp_payload);
     const regk_ctx::Resolve &rb = ctx->rsv;
@@ -6017,7 +6021,7 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
     if (ctx->pending)
         return fail(ctx, REGK_ERR_STATE, "%s: batches are still in flight; finish them first", who);
     const uint64_t k = in->k, m = rb.m;
-    const bool in_dev = in->flags & REGK_IN_DEVICE, dev_out = o->flags & REGK_OUT_DEVICE;
+    const bool in_dev = in->flags & REGK_IN_DEVICE, dev_out = o->flags & REGK_OUT_DEVICE, ptr = o->flags & REGK_DNS_PTR;
     if (k && !in->off)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: %llu messages need offsets", who, (unsigned long long)k);
     CK(cudaSetDevice(ctx->device));
@@ -6066,6 +6070,19 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
     for (int j = 0; j < 3; j++)
         if ((rc = ensure_dev(ctx, db.cum[j], (m + 1) * 8)))
             return rc;
+    /* the reverse index, sized for every node a host node */
+    const bool build_ptr = ptr && db.ptr_gen != rb.gen;
+    if (build_ptr) {
+        db.ptr_gen = 0;
+        size_t sort_bytes = 0;
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr,
+            (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)std::max<uint64_t>(m, 1), 0, 32, s));
+        if ((rc = ensure_dev(ctx, db.pkey_in, m * 4 + 16)) || (rc = ensure_dev(ctx, db.pval_in, m * 4 + 16)) ||
+            (rc = ensure_dev(ctx, db.pkey, m * 4 + 16)) || (rc = ensure_dev(ctx, db.pval, m * 4 + 16)) ||
+            (rc = ensure_dev(ctx, db.pbytes, (m + 1) * 8)) || (rc = ensure_dev(ctx, db.ptr_tmp, sort_bytes + 16)) ||
+            (rc = ensure_dev(ctx, db.ptr_totals, 2 * (ptiles + pnsup) * 8)) || (rc = ensure_dev(ctx, db.ptr_count, 16)))
+            return rc;
+    }
     DnsParams p{};
     p.m = m;
     p.path = rb.pb;
@@ -6111,6 +6128,18 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
     p.resp_off = (unsigned long long *)db.resp_off.p;
     p.rr_base = (unsigned long long *)db.rr_base.p;
     p.counters = (unsigned long long *)db.count.p;
+    DnsPtrParams x{};
+    x.n = db.ptr_n;
+    x.key = x.skey = (uint32_t *)db.pkey.p;
+    x.val = x.sval = (uint32_t *)db.pval.p;
+    x.bytes = x.sbytes = (unsigned long long *)db.pbytes.p;
+    x.key_in = (uint32_t *)db.pkey_in.p;
+    x.val_in = (uint32_t *)db.pval_in.p;
+    x.htile[0] = (unsigned long long *)db.ptr_totals.p;
+    x.hsuper[0] = x.htile[0] + ptiles;
+    x.btile[0] = x.hsuper[0] + pnsup;
+    x.bsuper[0] = x.btile[0] + ptiles;
+    x.count = (unsigned long long *)db.ptr_count.p;
     unsigned long long *hc = (unsigned long long *)db.h_count.p;
     uint32_t launches = 0;
     float ms = 0, part = 0;
@@ -6133,6 +6162,36 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
             launches += 2;
         }
     }
+    /* 1b. once per resolve with REGK_DNS_PTR: the reverse index (its count read back to size the sort) */
+    if (build_ptr) {
+        CK(cudaMemsetAsync(db.ptr_totals.p, 0, 2 * (ptiles + pnsup) * 8, s));
+        CK(cudaMemsetAsync(db.ptr_count.p, 0, 8, s));
+        CK(cudaMemsetAsync(db.pbytes.p, 0, 8, s));
+        if (m) {
+            regk_dns_ptr_count_kernel<<<(unsigned)ptiles, RV_TILE, 0, s>>>(p, x);
+            regk_dns_ptr_compact_kernel<<<(unsigned)ptiles, RV_TILE, 0, s>>>(p, x);
+            CK(cudaGetLastError());
+            launches += 2;
+        }
+        CK(cudaEventRecord(db.ev[1], s));
+        CK(cudaMemcpyAsync(hc, db.ptr_count.p, 8, cudaMemcpyDeviceToHost, s));
+        if ((rc = sync_or_fail(ctx, s, who)))
+            return rc;
+        cudaEventElapsedTime(&part, db.ev[0], db.ev[1]);
+        ms += part;
+        CK(cudaEventRecord(db.ev[0], s));
+        x.n = hc[0];
+        if (x.n) {
+            const uint64_t btiles = (x.n + RV_TILE - 1) / RV_TILE;
+            size_t tmp = db.ptr_tmp.cap;
+            CK(cub::DeviceRadixSort::SortPairs(db.ptr_tmp.p, tmp, (const uint32_t *)x.key_in, x.skey, (const uint32_t *)x.val_in,
+                x.sval, (int)x.n, 0, 32, s));
+            regk_dns_ptr_len_kernel<<<(unsigned)btiles, RV_TILE, 0, s>>>(p, x);
+            regk_dns_ptr_scan_kernel<<<(unsigned)btiles, RV_TILE, 0, s>>>(p, x);
+            CK(cudaGetLastError());
+            launches += 3;                                  /* the radix sort counted as one */
+        }
+    }
     /* 2. device offsets, before any message byte is read */
     if (k && in_dev) {
         regk_dns_check_kernel<<<(unsigned)((k + 255) / 256), 256, 0, s>>>(p);
@@ -6145,13 +6204,17 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
         if (hc[DNS_C_BAD] != ~0ull)
             return fail(ctx, REGK_ERR_INVALID_ARG, "%s: message %llu: offsets not monotone, past total or longer than 65535 bytes",
                 who, hc[DNS_C_BAD]);
-        cudaEventElapsedTime(&ms, db.ev[0], db.ev[1]);
+        cudaEventElapsedTime(&part, db.ev[0], db.ev[1]);
+        ms += part;
         CK(cudaEventRecord(db.ev[0], s));
     }
     db.prep_gen = rb.gen;
     /* 3. parse, look up and cut; 4. place */
     if (k) {
-        regk_dns_parse_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p);
+        if (ptr)
+            regk_dns_parse_ptr_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p, x);
+        else
+            regk_dns_parse_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p);
         regk_dns_place_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(p);
         CK(cudaGetLastError());
         launches += 2;
@@ -6172,7 +6235,10 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
         regk_dns_emit_head_kernel<<<(unsigned)((k + 255) / 256), 256, 0, s>>>(p);
         launches++;
         if (n_rr) {
-            regk_dns_emit_rr_kernel<<<(unsigned)((n_rr + 255) / 256), 256, 0, s>>>(p, n_rr);
+            if (ptr)
+                regk_dns_emit_rr_ptr_kernel<<<(unsigned)((n_rr + 255) / 256), 256, 0, s>>>(p, n_rr, x);
+            else
+                regk_dns_emit_rr_kernel<<<(unsigned)((n_rr + 255) / 256), 256, 0, s>>>(p, n_rr);
             launches++;
         }
         CK(cudaGetLastError());
@@ -6205,6 +6271,10 @@ int regk_dns_answer(regk_ctx *ctx, const regk_dns_in *in, const regk_dns_opts *o
     out->tc = (const uint8_t *)dsrc[3];
     out->node = (const uint64_t *)dsrc[4];
     out->kernel_ms = ms;
+    if (build_ptr) {
+        db.ptr_gen = rb.gen;
+        db.ptr_n = x.n;
+    }
     return REGK_OK;
 }
 

@@ -26,7 +26,8 @@ namespace regk {
 
 enum : uint8_t { DNS_ANSWER = 0, DNS_NODATA = 1, DNS_NXDOMAIN = 2, DNS_FORMERR = 3, DNS_NOTIMP = 4, DNS_REFUSED = 5,
                  DNS_BADVERS = 6, DNS_DROPPED = 7 };               /* include/regk.h REGK_DNS_* */
-enum : uint32_t { DNS_K_NONE = 0, DNS_K_HOST_A = 1, DNS_K_SERVICE_A = 2, DNS_K_SRV = 3 };
+enum : uint32_t { DNS_K_NONE = 0, DNS_K_HOST_A = 1, DNS_K_SERVICE_A = 2, DNS_K_SRV = 3,
+                  DNS_K_PTR = 4 };                  /* regk_dns_ptr.cuh: meta's kind field is 3 bits there */
 constexpr uint32_t DNS_A_RR = 16;               /* pointer owner, type, class, TTL, RDLENGTH, IPv4 */
 constexpr uint32_t DNS_OPT_RR = 11;
 constexpr uint32_t DNS_PTR_MAX = 0x3FFF;        /* a compression pointer's reach (RFC 1035 4.1.4) */
@@ -169,6 +170,10 @@ struct DnsFit {
     uint32_t nans, nadd, ans_bytes, tc;
 };
 
+struct DnsSpan {
+    uint32_t f, e;                              /* positions [f, e) */
+};
+
 /* What of a query's RRs fits in L bytes after `base` bytes of header, question and OPT.  A host A: one RR.  A service
    (children at sorted positions [f, e)): A, one RR per child; SRV, the prefixes S (SRV bytes), N (SRV RRs) and A
    (additional RRs) over the sorted positions, whose cut-off child and port come from a binary search and a division.
@@ -258,17 +263,9 @@ RG_HD void dns_put_a(uint8_t *o, uint32_t owner, uint32_t ttl, uint32_t addr)
     dns_put32(o, addr);
 }
 
-/* an SRV RR to the dotted name t of tn bytes: owner 0xC00C, priority 0, weight 10, port, the uncompressed target */
-RG_HD void dns_put_srv(uint8_t *o, uint32_t ttl, uint32_t port, const uint8_t *t, uint32_t tn)
+/* the dotted name t of tn bytes as an uncompressed wire name of tn + 2 bytes */
+RG_HD void dns_put_name(uint8_t *o, const uint8_t *t, uint32_t tn)
 {
-    o = dns_put16(o, 0xC00Cu);
-    o = dns_put16(o, 33);
-    o = dns_put16(o, 1);
-    o = dns_put32(o, ttl);
-    o = dns_put16(o, 8u + tn);
-    o = dns_put16(o, 0);
-    o = dns_put16(o, 10);
-    o = dns_put16(o, port);
     uint8_t *len = o++;
     uint32_t run = 0;
     for (uint32_t k = 0; k < tn; k++) {
@@ -283,6 +280,20 @@ RG_HD void dns_put_srv(uint8_t *o, uint32_t ttl, uint32_t port, const uint8_t *t
     }
     *len = (uint8_t)run;
     *o = 0;
+}
+
+/* an SRV RR to the dotted name t of tn bytes: owner 0xC00C, priority 0, weight 10, port, the uncompressed target */
+RG_HD void dns_put_srv(uint8_t *o, uint32_t ttl, uint32_t port, const uint8_t *t, uint32_t tn)
+{
+    o = dns_put16(o, 0xC00Cu);
+    o = dns_put16(o, 33);
+    o = dns_put16(o, 1);
+    o = dns_put32(o, ttl);
+    o = dns_put16(o, 8u + tn);
+    o = dns_put16(o, 0);
+    o = dns_put16(o, 10);
+    o = dns_put16(o, port);
+    dns_put_name(o, t, tn);
 }
 
 }  /* namespace regk */
@@ -407,8 +418,20 @@ __device__ __forceinline__ uint64_t dns_find(const DnsParams &p, unsigned long l
     }
 }
 
+/* No reverse names (regk_dns_parse_kernel, regk_dns_emit_rr_kernel): what the bodies below ask of a reverse index
+   (regk_dns_ptr.cuh DnsRev) when `on`, folded away here */
+struct DnsNoRev {
+    static constexpr bool on = false;
+    static constexpr uint32_t kind_mask = 3u;   /* the kind bits of meta these kernels read */
+    __device__ DnsSpan owner(const uint8_t *, const DnsMsg &) const { return DnsSpan{0, 0}; }
+    __device__ uint64_t node(uint32_t) const { return ~0ull; }
+    __device__ DnsFit fit(uint32_t, uint32_t, uint32_t) const { return DnsFit{0, 0, 0, 0}; }
+    __device__ void emit(const DnsParams &, uint8_t *, uint64_t, uint32_t) const {}
+};
+
 /* ---- parse: rules, lookup and the truncation cut, one thread per message ---- */
-__global__ void __launch_bounds__(RV_TILE) regk_dns_parse_kernel(const DnsParams p)
+template <class Rev>
+__device__ __forceinline__ void dns_parse_body(const DnsParams &p, const Rev &rev)
 {
     __shared__ unsigned int s_cnt[9];
     const uint64_t i = (uint64_t)blockIdx.x * RV_TILE + threadIdx.x;
@@ -449,9 +472,19 @@ __global__ void __launch_bounds__(RV_TILE) regk_dns_parse_kernel(const DnsParams
                 kind = DNS_K_SRV;
                 node = own_s;
             } else {
-                status = (own_a != ~0ull || own_s != ~0ull) ? DNS_NODATA : DNS_NXDOMAIN;
+                /* a reverse name's targets (sorted positions), looked up only where they decide the answer */
+                const bool owns = own_a != ~0ull || own_s != ~0ull;
+                const DnsSpan pt = Rev::on && (r.qtype == 12u || !owns) ? rev.owner(msg, r) : DnsSpan{0, 0};
+                if (Rev::on && r.qtype == 12u && pt.f < pt.e) {
+                    kind = DNS_K_PTR;
+                    node = rev.node(pt.f);
+                    const uint32_t L = dns_limit(p.tcp != 0, r.opt, r.req_size, p.udp_payload);
+                    fit = rev.fit(pt.f, pt.e, L - r.qend - (r.opt ? DNS_OPT_RR : 0u));
+                } else {
+                    status = (owns || pt.f < pt.e) ? DNS_NODATA : DNS_NXDOMAIN;
+                }
             }
-            if (kind != DNS_K_NONE) {
+            if (kind != DNS_K_NONE && (!Rev::on || kind != DNS_K_PTR)) {
                 const uint32_t f = kind == DNS_K_HOST_A ? 0u : p.first[node], e = kind == DNS_K_HOST_A ? 0u : p.end[node];
                 const uint32_t L = dns_limit(p.tcp != 0, r.opt, r.req_size, p.udp_payload);
                 fit = dns_fit(kind, f, e, p.cum[0], p.cum[1], p.cum[2], L, r.qend + (r.opt ? DNS_OPT_RR : 0u), r.qend);
@@ -478,6 +511,11 @@ __global__ void __launch_bounds__(RV_TILE) regk_dns_parse_kernel(const DnsParams
     }
     if (threadIdx.x < 9 && s_cnt[threadIdx.x])
         atomicAdd(p.counters + (threadIdx.x < 8 ? DNS_C_STATUS + threadIdx.x : DNS_C_TC), (unsigned long long)s_cnt[threadIdx.x]);
+}
+
+__global__ void __launch_bounds__(RV_TILE) regk_dns_parse_kernel(const DnsParams p)
+{
+    dns_parse_body(p, DnsNoRev{});
 }
 
 /* ---- place: resp_off and rr_base, and the totals ---- */
@@ -543,7 +581,8 @@ __global__ void __launch_bounds__(256) regk_dns_emit_head_kernel(const DnsParams
 }
 
 /* ---- emit_rr: one thread per RR ---- */
-__global__ void __launch_bounds__(256) regk_dns_emit_rr_kernel(const DnsParams p, unsigned long long n_rr)
+template <class Rev>
+__device__ __forceinline__ void dns_emit_rr_body(const DnsParams &p, unsigned long long n_rr, const Rev &rev)
 {
     const unsigned long long r = (unsigned long long)blockIdx.x * 256 + threadIdx.x;
     if (r >= n_rr)
@@ -557,12 +596,16 @@ __global__ void __launch_bounds__(256) regk_dns_emit_rr_kernel(const DnsParams p
             hi = mid - 1;
     }
     const uint64_t q = lo;
-    const uint32_t t = (uint32_t)(r - p.rr_base[q]), meta = p.meta[q], qend = meta & 511u, kind = (meta >> 11) & 3u;
+    const uint32_t t = (uint32_t)(r - p.rr_base[q]), meta = p.meta[q], qend = meta & 511u, kind = (meta >> 11) & Rev::kind_mask;
     const uint32_t nans = p.nans[q];
     const uint64_t s = p.node[q];
     uint8_t *o = p.resp + p.resp_off[q] + qend;
     if (kind == DNS_K_HOST_A) {
         dns_put_a(o, 12u, (uint32_t)p.ttl[s], p.ip4[s]);
+        return;
+    }
+    if (Rev::on && kind == DNS_K_PTR) {
+        rev.emit(p, o, s, t);
         return;
     }
     const uint32_t f = p.first[s], e = p.end[s];
@@ -586,6 +629,11 @@ __global__ void __launch_bounds__(256) regk_dns_emit_rr_kernel(const DnsParams p
     const uint32_t ta = t - nans;                       /* additional ta: the child of the (ta+1)-th first SRV RR */
     const uint32_t ci = dns_upper(A, f, e, ta), c = p.sval[ci];
     dns_put_a(o + p.ans_bytes[q] + ta * DNS_A_RR, qend + (uint32_t)(S[ci] - S[f]) + 18u, (uint32_t)p.ttl[c], p.ip4[c]);
+}
+
+__global__ void __launch_bounds__(256) regk_dns_emit_rr_kernel(const DnsParams p, unsigned long long n_rr)
+{
+    dns_emit_rr_body(p, n_rr, DnsNoRev{});
 }
 
 }  /* namespace regk */

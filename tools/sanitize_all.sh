@@ -15,6 +15,7 @@ for tool in memcheck racecheck synccheck; do
   timeout 900 compute-sanitizer --tool $tool python tests/sanitize_lifetime_run.py 2>&1 | tail -4
   timeout 900 compute-sanitizer --tool $tool python tests/sanitize_resolve_run.py 2>&1 | tail -4
   timeout 900 compute-sanitizer --tool $tool python tests/sanitize_dns_run.py 2>&1 | tail -4
+  timeout 900 compute-sanitizer --tool $tool python tests/sanitize_dns_ptr_run.py 2>&1 | tail -4
   timeout 900 compute-sanitizer --tool $tool python tests/sanitize_walk_run.py 2>&1 | tail -4
   timeout 900 compute-sanitizer --tool $tool python tests/sanitize_walk_watch_run.py 2>&1 | tail -4
   timeout 900 compute-sanitizer --tool $tool python tests/sanitize_walk_setwatches_run.py 2>&1 | tail -4
