@@ -1126,10 +1126,46 @@ int         regk_setwatches_requests(regk_ctx *ctx, const regk_setwatches_opts *
  * launches counts the radix sort that groups the children as one; kernel_ms spans every pass but the host's reads.
  * PARITY UNPINNED: Binder's default TTLs are parameters (the README's SRV example implies a host default of 30:
  * README.md:383-392 sets no ttl and :433 shows 30); Binder's answer order; a service record with a middle-level ttl
- * (the README's authcache example, :511-523) is not a form this library writes and is REGK_RSV_NOT_RECORD here.
+ * (the README's authcache example, :511-523) is not a form this library writes and is REGK_RSV_NOT_RECORD here
+ * unless REGK_RESOLVE_ANY_FORM is set.
+ *
+ * ---- with REGK_RESOLVE_ANY_FORM (regk_resolve and regk_walk_resolve): records in any JSON form Binder reads.  Without
+ * the flag nothing changes (the same kernels, launches and bytes).  With it:
+ *   1. The canonical recogniser still decides first: every node it accepts keeps exactly its class, record and
+ *      answers.  The general reader decides the CANDIDATES only: nodes with non-empty data and a path ('/' first) that
+ *      the canonical recogniser classes REGK_RSV_NOT_RECORD.
+ *   2. A candidate is REGK_RSV_NOT_RECORD unless its payload is exactly one JSON object (RFC 8259), optionally
+ *      surrounded by JSON whitespace (space, TAB, LF, CR); with at most 64 containers nested; bytes >= 0x80 only inside
+ *      strings (not validated as UTF-8); and no member name anywhere holding a backslash (an escaped name could decode
+ *      to "ttl"; names are compared raw).  Duplicate member names: the last one wins, as in JSON.parse.  String values
+ *      are taken verbatim, escapes left as they are (so an escaped type, address or srvce fails the rules below:
+ *      UNKNOWN_TYPE, BAD_ADDRESS, BAD_NAME).  Unknown members at any depth are skipped (and grammar-checked).
+ *   3. Service record: the top-level "type" is the string "service"; top.service is an object; top.service.service is
+ *      an object with "srvce" (a string), "proto" (a string) and "port" (an integer 0..2^32-1); the middle object's
+ *      "type" is not required.  srv_ttl = the first present of service.service.ttl, service.ttl, ttl.
+ *   4. Host record: the top-level "type" is a string other than "service".  inner = the top-level member whose name
+ *      equals the type bytes raw (before or after "type"), an object; inner.address, a string, is the address; the
+ *      top-level "address" is ignored (absent, different or of any type); inner.ports is optional, and if present an
+ *      array of integers 0..2^32-1 ([] allowed).  a_ttl = the first present of inner.ttl and the top-level ttl.
+ *   5. Every "ttl" member of the inspected objects (top, service and service.service of a service record; top and
+ *      inner of a host record), the port and each ports element is a JSON integer -?(0|[1-9][0-9]*): no fraction, no
+ *      exponent, not -0; a ttl fits in int32.  Anything else there (null, a string, 30.0, ...) is REGK_RSV_NOT_RECORD.
+ *      Numbers in skipped members may take any JSON form.
+ *   6. From there on everything is as without the flag: BAD_NAME, UNKNOWN_TYPE, BAD_ADDRESS, BAD_TTL (on the chosen
+ *      TTL), BAD_PORT, the children, the queries, the text, regk_dns_answer (REGK_DNS_PTR included) and the walk's
+ *      identity rules.
+ *   7. regk_walk_resolve: a call whose REGK_RESOLVE_ANY_FORM differs from the last successful call's is full, as a
+ *      change of default TTLs is.
+ *   8. launches counts 2 more kernels (candidate count and compaction), and 1 more (the reader) when there is at least
+ *      one candidate; the flag's classify replaces the plain one.
+ * PARITY UNPINNED (Binder is absent): Binder's handling of escaped member names, of non-integer or null TTLs and
+ * ports, and of a host record without an inner address but with a top-level one; its nesting limit; whether it
+ * compares the type value decoded.
  */
+#define REGK_RESOLVE_ANY_FORM (1u << 12)    /* regk_resolve_opts.flags: read records in any JSON form (above) */
+
 typedef struct regk_resolve_opts {
-    uint32_t flags;                 /* REGK_OUT_DEVICE */
+    uint32_t flags;                 /* REGK_OUT_DEVICE | REGK_RESOLVE_ANY_FORM */
     int32_t  default_host_ttl;      /* A TTL of a host record without "ttl" (>= 0) */
     int32_t  default_srv_ttl;       /* SRV TTL of a service record without "ttl" (>= 0) */
     uint32_t reserved;              /* 0 */
@@ -1141,7 +1177,8 @@ typedef struct regk_resolve_opts {
 
 #define REGK_RSV_OK           0u    /* node_cls[]; first failing rule decides, in this order: */
 #define REGK_RSV_EMPTY        1u    /* empty data: a directory node; answers nothing; not listed */
-#define REGK_RSV_NOT_RECORD   2u    /* regk_decode found no canonical host or service record, or a bad path */
+#define REGK_RSV_NOT_RECORD   2u    /* regk_decode found no canonical host or service record (nor, with
+                                       REGK_RESOLVE_ANY_FORM, the general reader any record), or a bad path */
 #define REGK_RSV_BAD_NAME     3u    /* a DNS name it would own is not a valid name */
 #define REGK_RSV_UNKNOWN_TYPE 4u    /* host record whose type bytes are not one of the README's seven */
 #define REGK_RSV_BAD_ADDRESS  5u    /* host record address not a dotted-quad IPv4 (no leading zeros) */
@@ -1506,7 +1543,7 @@ int         regk_walk_setwatches(regk_ctx *ctx, const regk_setwatches_opts *opts
  *   regk_walk_start clears everything, the kept text included.  This bookkeeping is not counted in any walk call's
  *   launches or kernel_ms, and no walk call's outputs change.
  * REUSE: full = 1 when there was no successful regk_walk_resolve since the last regk_walk_start, or its
- *   default_host_ttl / default_srv_ttl differ from this call's: n_fresh = m, copied_bytes = 0, every line formatted.
+ *   default_host_ttl / default_srv_ttl or REGK_RESOLVE_ANY_FORM differ from this call's: n_fresh = m, copied_bytes = 0, every line formatted.
  *   Otherwise a HOST_A section is copied from the last call's text when its node has an identity, and a service child's
  *   A line, SRV lines and additional line when the child and its service both have one; everything else is formatted.
  *   This is exact: a node's class, roles and TTL depend only on its own path, data and opts; whether a node is a child

@@ -545,6 +545,7 @@ class CDnsOut(C.Structure):          # regk_dns_out
  DNS_DROPPED) = range(8)                                             # DnsResponses.status
 FLAG_DNS_TCP = 1 << 8                                                # CDnsOpts.flags
 FLAG_DNS_PTR = 1 << 11                                               # CDnsOpts.flags: PTR for in-addr.arpa names
+FLAG_RESOLVE_ANY_FORM = 1 << 12                                      # CResolveOpts.flags: records in any JSON form
 
 
 class DnsResponses:
@@ -1341,12 +1342,14 @@ class Context:
         return out if device else SetWatches(out)
 
     # -- what DNS answers for a snapshot --
-    def resolve(self, snapshot, default_host_ttl: int, default_srv_ttl: int, device: bool = False):
+    def resolve(self, snapshot, default_host_ttl: int, default_srv_ttl: int, device: bool = False, any_form: bool = False):
         """regk_resolve: the A and SRV answers the host and service records of `snapshot` define (a batch.Snapshot,
-        host or CUDA, or anything with cdecode_in(), such as a Replies or a Walk).  Returns an Answers, or the raw CAnswers
-        (device pointers) with device=True."""
+        host or CUDA, or anything with cdecode_in(), such as a Replies or a Walk).  any_form=True also reads records in
+        any JSON form Binder reads (REGK_RESOLVE_ANY_FORM), for a registry this library did not write.  Returns an
+        Answers, or the raw CAnswers (device pointers) with device=True."""
         cin, keep = snapshot.cdecode_in()
-        o = CResolveOpts(FLAG_OUT_DEVICE if device else 0, int(default_host_ttl), int(default_srv_ttl), 0)
+        o = CResolveOpts((FLAG_OUT_DEVICE if device else 0) | (FLAG_RESOLVE_ANY_FORM if any_form else 0), int(default_host_ttl),
+                         int(default_srv_ttl), 0)
         out = CAnswers()
         rc = self._lib.regk_resolve(self._h, C.byref(cin), C.byref(o), C.byref(out))
         del keep
@@ -1521,12 +1524,14 @@ class Context:
         w, _ = self._walk_levels(exchange, int(xid_base) % 2 ** 32, r.n_frontier, True, getattr(self, "_walk", None))
         return r, w
 
-    def walk_resolve(self, default_host_ttl: int, default_srv_ttl: int, device: bool = False):
+    def walk_resolve(self, default_host_ttl: int, default_srv_ttl: int, device: bool = False, any_form: bool = False):
         """regk_walk_resolve: the answers of the walk's snapshot as it stands, exactly what resolve(walk, ...) returns,
         with every line whose inputs did not change since the last walk_resolve() copied from that call's text.
+        any_form as in resolve(); a call whose any_form differs from the last one's formats everything.
         answer_dns() then answers from it until the walk's snapshot changes.  Returns a WalkAnswers, or the raw
         CWalkAnswers (device pointers) with device=True."""
-        o = CResolveOpts(FLAG_OUT_DEVICE if device else 0, int(default_host_ttl), int(default_srv_ttl), 0)
+        o = CResolveOpts((FLAG_OUT_DEVICE if device else 0) | (FLAG_RESOLVE_ANY_FORM if any_form else 0), int(default_host_ttl),
+                         int(default_srv_ttl), 0)
         out = CWalkAnswers()
         self._check(self._lib.regk_walk_resolve(self._h, C.byref(o), C.byref(out)))
         return out if device else WalkAnswers(out)

@@ -40,6 +40,7 @@
 #include "regk_events.cuh"
 #include "regk_setwatches.cuh"
 #include "regk_resolve.cuh"
+#include "regk_resolve_any.cuh"
 #include "regk_dns.cuh"
 #include "regk_dns_ptr.cuh"
 #include "regk_walk.cuh"
@@ -342,7 +343,8 @@ struct regk_ctx {
     struct Resolve {
         DevBuf in[4], table, slot, hash, rec, dom, ports, cls, roles, ttl, key, val, skey, sval, first, end, cum[3], totals,
             count, node_q, q_kind, q_node, sec_off, unres, text, sort_tmp;
-        HostBuf h_count, h_q_kind, h_q_node, h_sec_off, h_text, h_cls, h_unres;
+        DevBuf any_list, any_totals, any_count;     /* REGK_RESOLVE_ANY_FORM: the candidates, their tile totals, count */
+        HostBuf h_count, h_q_kind, h_q_node, h_sec_off, h_text, h_cls, h_unres, h_any;
         Event ev[5];
         /* the last call succeeded: regk_dns_answer answers against it (the snapshot streams it read, its table size) */
         bool valid = false;
@@ -416,6 +418,7 @@ struct regk_ctx {
         bool have = false;
         int cur = 0;
         int32_t dflt_host = 0, dflt_srv = 0;
+        bool any = false;                       /* the last call's REGK_RESOLVE_ANY_FORM */
         uint64_t segments = 0;
         DevBuf text[2], run[2], kind, len, src, dest, totals, count, seg_src, seg_dest, seg_sel, seg_len, seg_off, scratch;
         Event ev[4];
@@ -5691,8 +5694,8 @@ static int resolve_meta(regk_ctx *ctx, const regk_decode_in *in, const regk_reso
 {
     if (in->flags & REGK_DECODE_LAST)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: REGK_DECODE_LAST names no snapshot; pass the snapshot's streams", who);
-    if (o->flags & ~REGK_OUT_DEVICE)
-        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: unknown flag bits 0x%x", who, o->flags & ~REGK_OUT_DEVICE);
+    if (o->flags & ~(REGK_OUT_DEVICE | REGK_RESOLVE_ANY_FORM))
+        return fail(ctx, REGK_ERR_INVALID_ARG, "%s: unknown flag bits 0x%x", who, o->flags & ~(REGK_OUT_DEVICE | REGK_RESOLVE_ANY_FORM));
     if (o->reserved)
         return fail(ctx, REGK_ERR_INVALID_ARG, "%s: reserved must be 0", who);
     if (o->default_host_ttl < 0 || o->default_srv_ttl < 0)
@@ -5773,6 +5776,10 @@ static int resolve_meta(regk_ctx *ctx, const regk_decode_in *in, const regk_reso
     for (int k = 0; k < 3; k++)
         if ((rc = ensure_dev(ctx, rb.cum[k], (m + 1) * 8)))
             return rc;
+    const bool any = o->flags & REGK_RESOLVE_ANY_FORM;
+    if (any && ((rc = ensure_dev(ctx, rb.any_list, m * 4 + 16)) || (rc = ensure_dev(ctx, rb.any_totals, (tiles + nsup) * 8)) ||
+                (rc = ensure_dev(ctx, rb.any_count, 16)) || (rc = ensure_host(ctx, rb.h_any, 16))))
+        return rc;
     CK(cudaMemsetAsync(rb.table.p, 0, slots * 4, s));
     CK(cudaMemsetAsync(rb.totals.p, 0, totals_bytes, s));
     CK(cudaMemsetAsync(rb.count.p, 0, RV_NCOUNTERS * 8, s));
@@ -5874,9 +5881,42 @@ static int resolve_meta(regk_ctx *ctx, const regk_decode_in *in, const regk_reso
         if ((rc = set_smem_limit(ctx, (const void *)regk_decode_kernel, dsmem)))
             return rc;
         regk_decode_kernel<<<(unsigned)((m + DEC_TILE - 1) / DEC_TILE), DEC_TILE, dsmem, s>>>(dp);
-        /* 3. classify, 4. join, 5. group, 6. size and place */
         const unsigned g256 = (unsigned)((m + 255) / 256);
-        regk_resolve_classify_kernel<<<g256, 256, 0, s>>>(p);
+        if (any) {
+            /* 2b. REGK_RESOLVE_ANY_FORM: the candidates in node order, then the general reader over them */
+            AnyParams ap{};
+            ap.m = m;
+            ap.json = jb;
+            ap.json_off = (const unsigned long long *)jo;
+            ap.json_limit = dp.json_limit;
+            ap.dec = (Decoded *)rb.rec.p;
+            ap.ports = (uint32_t *)rb.ports.p;
+            ap.list = (uint32_t *)rb.any_list.p;
+            for (int k = 0; k < 3; k++) {
+                ap.tile_total[k] = (unsigned long long *)rb.any_totals.p;
+                ap.super_total[k] = ap.tile_total[k] + tiles;
+            }
+            ap.count = (unsigned long long *)rb.any_count.p;
+            CK(cudaMemsetAsync(rb.any_totals.p, 0, (tiles + nsup) * 8, s));
+            regk_resolve_any_count_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(ap);
+            regk_resolve_any_compact_kernel<<<(unsigned)tiles, RV_TILE, 0, s>>>(ap);
+            CK(cudaGetLastError());
+            launches += 2;
+            unsigned long long *hn = (unsigned long long *)rb.h_any.p;
+            CK(cudaMemcpyAsync(hn, rb.any_count.p, 8, cudaMemcpyDeviceToHost, s));
+            if ((rc = sync_or_fail(ctx, s, who)))
+                return rc;
+            if (*hn) {
+                regk_resolve_any_read_kernel<<<(unsigned)((*hn + 255) / 256), 256, 0, s>>>(ap, (uint32_t)*hn);
+                CK(cudaGetLastError());
+                launches++;
+            }
+        }
+        /* 3. classify, 4. join, 5. group, 6. size and place */
+        if (any)
+            regk_resolve_classify_any_kernel<<<g256, 256, 0, s>>>(p);
+        else
+            regk_resolve_classify_kernel<<<g256, 256, 0, s>>>(p);
         regk_resolve_join_kernel<<<g256, 256, 0, s>>>(p);
         CK(cudaGetLastError());
         size_t tmp = rb.sort_tmp.cap;
@@ -7771,7 +7811,8 @@ int regk_walk_resolve(regk_ctx *ctx, const regk_resolve_opts *o, regk_walk_answe
     regk_ctx::WalkResolve &wr = ctx->wr;
     cudaStream_t s = ctx->stream;
     const uint64_t m = r.m, T = r.text_total;
-    const bool full = !wr.have || wr.dflt_host != o->default_host_ttl || wr.dflt_srv != o->default_srv_ttl;
+    const bool any = o->flags & REGK_RESOLVE_ANY_FORM;
+    const bool full = !wr.have || wr.dflt_host != o->default_host_ttl || wr.dflt_srv != o->default_srv_ttl || wr.any != any;
     const int nx = 1 - wr.cur;
     for (Event &ev : wr.ev)
         if ((rc = ensure_event(ctx, ev)))
@@ -7895,6 +7936,7 @@ int regk_walk_resolve(regk_ctx *ctx, const regk_resolve_opts *o, regk_walk_answe
     wr.have = true;
     wr.dflt_host = o->default_host_ttl;
     wr.dflt_srv = o->default_srv_ttl;
+    wr.any = any;
     wr.segments = nseg;
     out->n_fresh = n_fresh;
     out->copied_bytes = T - formatted;

@@ -122,8 +122,13 @@ struct RvNode {
     int32_t ttl;                                /* a_ttl of a host record, srv_ttl of a service record */
 };
 
+/* Decoded.flags bits above the public REGK_DEC_* (internal, never returned by regk_decode): REGK_RESOLVE_ANY_FORM's
+   general reader (regk_resolve_any.cuh) read the node, and found a ttl in it */
+enum : uint32_t { RV_DEC_ANY_READ = 1u << 16, RV_DEC_TTL_IN = 1u << 17 };
+
 /* Node j from its regk_decode record (host_nodes = 0), its data, its domain and its ports: the first failing rule of
-   include/regk.h REGK_RSV_* decides the class */
+   include/regk.h REGK_RSV_* decides the class.  ANY: a node the general reader read says itself whether it has a ttl. */
+template <bool ANY = false>
 RG_HD RvNode rv_classify(const Decoded &d, const uint8_t *json, uint32_t jn, const uint8_t *dom, const uint32_t *ports,
     int32_t dflt_host, int32_t dflt_srv)
 {
@@ -156,7 +161,7 @@ RG_HD RvNode rv_classify(const Decoded &d, const uint8_t *json, uint32_t jn, con
         name_ok = name_ok && o.done();
     }
     const uint32_t tr = host ? rv_type_roles(json + d.type_pos, d.type_len) : 0u;
-    const bool ttl_in = rv_ttl_present(d, json, jn);
+    const bool ttl_in = (ANY && (d.flags & RV_DEC_ANY_READ)) ? (d.flags & RV_DEC_TTL_IN) != 0 : rv_ttl_present(d, json, jn);
     const uint32_t np = svc ? 1u : (d.nports == 0xFFFFFFFFu ? 0u : d.nports);
     uint32_t maxport = 0;
     for (uint32_t k = 0; k < np; k++)
@@ -366,8 +371,9 @@ __device__ __forceinline__ void rv_tile_bases(unsigned long long *const (&tile_t
         base[k] = s_base[k];
 }
 
-/* ---- classify: duplicate path, class, roles, TTL ---- */
-__global__ void __launch_bounds__(256) regk_resolve_classify_kernel(const ResolveParams p)
+/* ---- classify: duplicate path, class, roles, TTL (ANY: regk_resolve_any.cuh's variant) ---- */
+template <bool ANY>
+__device__ __forceinline__ void rv_classify_node(const ResolveParams &p)
 {
     const uint64_t j = (uint64_t)blockIdx.x * 256 + threadIdx.x;
     if (j >= p.m)
@@ -376,11 +382,16 @@ __global__ void __launch_bounds__(256) regk_resolve_classify_kernel(const Resolv
         atomicMin(p.counters + RV_C_DUP, (unsigned long long)j);
     const unsigned long long q0 = p.json_off[j];
     const Decoded d = p.dec[j];
-    const RvNode r = rv_classify(d, p.json + q0, (uint32_t)(p.json_off[j + 1] - q0), p.dom + p.path_off[j], p.ports + (q0 >> 1),
-        p.dflt_host, p.dflt_srv);
+    const RvNode r = rv_classify<ANY>(d, p.json + q0, (uint32_t)(p.json_off[j + 1] - q0), p.dom + p.path_off[j],
+        p.ports + (q0 >> 1), p.dflt_host, p.dflt_srv);
     p.cls[j] = r.cls;
     p.roles[j] = r.roles;
     p.ttl[j] = r.ttl;
+}
+
+__global__ void __launch_bounds__(256) regk_resolve_classify_kernel(const ResolveParams p)
+{
+    rv_classify_node<false>(p);
 }
 
 /* ---- join: the service node each candidate child belongs to ---- */

@@ -20,5 +20,6 @@ for tool in memcheck racecheck synccheck; do
   timeout 900 compute-sanitizer --tool $tool python tests/sanitize_walk_watch_run.py 2>&1 | tail -4
   timeout 900 compute-sanitizer --tool $tool python tests/sanitize_walk_setwatches_run.py 2>&1 | tail -4
   timeout 900 compute-sanitizer --tool $tool python tests/sanitize_walk_resolve_run.py 2>&1 | tail -4
+  timeout 900 compute-sanitizer --tool $tool python tests/sanitize_resolve_any_run.py 2>&1 | tail -4
 done > gpurun_out/r2_sanitizer_new.txt 2>&1
 cat gpurun_out/r2_sanitizer_new.txt
